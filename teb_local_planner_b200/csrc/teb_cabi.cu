@@ -61,7 +61,6 @@ struct tebgpu_ctx {
                             kept as an independently mapped, bit-identical implementation,
                           3 / 4 k_solve_lat (twisted factorisation, system resident in shared memory) always / while the
                             systems of a round fit LAT_WAVES waves of resident CTAs (the latency regime; DEFAULT) */
-  int ring = 0;        /* solver prefetch ring: 0 = 10 rows (default), else 10 / 20 / 30 rows (TEBGPU_RING, experiments) */
   int eval_v1 = 0;     /* TEBGPU_EVAL_V1=1: first-generation trial evaluation (warp per trial, chunk per lane) */
   int ka_staged = 1;   /* kernel A output: 1 (default) shared-memory slot + TMA bulk store per lane, 0 direct 128-bit global stores */
   int last_spec_k = 0; /* round-0 width of the later LM iterations of the last optimize call */
@@ -346,16 +345,11 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb<10>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb<20>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb<30>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb<20>, cudaFuncAttributeMaxDynamicSharedMemorySize, tpb_ring_bytes(20)));
-  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb<30>, cudaFuncAttributeMaxDynamicSharedMemorySize, tpb_ring_bytes(30)));
+  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CUDA_TRY(c, cudaFuncSetAttribute(k_solve_lat, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
   if (const char* e = std::getenv("TEBGPU_LAT_TIMING")) { const int v = std::atoi(e); CUDA_TRY(c, cudaMemcpyToSymbol(g_lat_timing, &v, sizeof(int))); }
   if (const char* e = std::getenv("TEBGPU_WARP_SOLVER")) { const int m = std::atoi(e); if (m >= 0 && m <= 4) c->warp_solver = m; }
   if (const char* e = std::getenv("TEBGPU_GRAPH")) { const int m = std::atoi(e); if (m >= 0 && m <= 2) c->graph_mode = m; }
-  if (const char* e = std::getenv("TEBGPU_RING")) { const int r = std::atoi(e); if (r == 10 || r == 20 || r == 30) c->ring = r; }
   CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval<2, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval<2, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval<3, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -673,12 +667,8 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
         const bool fork = overlap && rounds > 1 && !kp.has_vor;
         cudaStream_t rs = st;
         auto launch_solve = [&](const SpecBufs& spec, int K, int round, cudaStream_t s) {
-          /* ring depth: 10 rows unless TEBGPU_RING asks for 20 / 30. Deeper rings do
-           * not shorten the chain - a lone solver warp is bound by its own fp64 issue rate (~75 DFMA per pivot at 2
-           * cycles each), not by the prefetch distance - and they cost residency (20 rows: 3 warps per SM). */
           const int bk = B * K;
           const int warps = (bk + 31) / 32;
-          const int ring = ctx->ring == 0 ? 10 : ctx->ring;
           /* k_solve_warp: the sequential order spread over a warp (cross-check only) */
           const bool warp_solver = ctx->warp_solver == 1 || (ctx->warp_solver == 2 && bk <= ctx->sms * 8);
           const size_t smem_lat = solve_lat_smem_bytes(bt->n_cap);
@@ -694,13 +684,11 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
             const long long cap = LAT_WAVES * lat_wave < bk ? LAT_WAVES * lat_wave : bk;
             sl.lat_cap = (int32_t)cap;
             k_solve_lat<<<(unsigned)cap, 32, smem_lat, s>>>(db, sl, it, round, g);
-            k_solve_tpb<10><<<warps, 32, tpb_ring_bytes(10), s>>>(db, sl, it, round, g);
+            k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, sl, it, round, g);
             ++launches;
           }
           else if (warp_solver) k_solve_warp<<<(bk + SW_WARPS - 1) / SW_WARPS, 32 * SW_WARPS, 0, s>>>(db, spec, it, round, g);
-          else if (ring == 30) k_solve_tpb<30><<<warps, 32, tpb_ring_bytes(30), s>>>(db, spec, it, round, g);
-          else if (ring == 20) k_solve_tpb<20><<<warps, 32, tpb_ring_bytes(20), s>>>(db, spec, it, round, g);
-          else k_solve_tpb<10><<<warps, 32, tpb_ring_bytes(10), s>>>(db, spec, it, round, g);
+          else k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, spec, it, round, g);
           ++launches;
         };
         for (int round = 0; round < rounds; ++round, ++g) {
@@ -791,7 +779,7 @@ static uint64_t graph_key(const tebgpu_ctx* ctx, const TebBatch* bt, const TebOp
   mix(bt, sizeof(*bt));
   mix(a, sizeof(*a));
   mix(&ctx->params_version, sizeof(ctx->params_version));
-  const int sw[11] = {ctx->solver, ctx->spec_k, ctx->linearize_variant, ctx->ka_staged, ctx->eval_v1, ctx->ring, ctx->overlap, ctx->eval_minb, ctx->warp_solver, ctx->eval_mode, ctx->split};
+  const int sw[10] = {ctx->solver, ctx->spec_k, ctx->linearize_variant, ctx->ka_staged, ctx->eval_v1, ctx->overlap, ctx->eval_minb, ctx->warp_solver, ctx->eval_mode, ctx->split};
   mix(sw, sizeof(sw));
   mix(&st, sizeof(st));
   return h;

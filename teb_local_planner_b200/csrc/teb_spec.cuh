@@ -9,7 +9,7 @@
  * iterations (measured trial histogram: 1:51 %, 2:12 %, 3:17 %, 4:15 %, 5:5 %, 6:0.2 %).
  *
  *   k_solve_tpb   one THREAD per (band, trial): banded LDL^T (half bandwidth 10) with the 11x11 active window held in
- *                 registers (fully unrolled by 11 so every index is static), rows of H streamed from HBM/L2, factor
+ *                 registers (fully unrolled by 11 so every index is static), rows of H staged per band in shared memory, factor
  *                 rows streamed out in the band's profile (only the columns' structurally non-zero entries),
  *                 forward substitution fused, back substitution from the streamed factor.
  *                 Replaces LinearSolverCSparse::solve (optimal_planner.cpp:169-172).
@@ -81,14 +81,29 @@ __device__ __forceinline__ double band_lambda_init(const DevBatch& db, int b, in
 }
 
 /* ------------------------------------------------------------------ k_solve_tpb
- * One warp per CTA. Every thread owns a private ring of TPB_RING row slots in shared memory ([slot][16-byte pair][lane]
- * so that a warp access is conflict free) that cp.async (LDGSTS) fills TPB_RING rows ahead of their use: the H rows
- * during the factorisation, the factor rows during the back substitution. No registers are spent on prefetching and
- * the global latency is off the dependent chain. 10 slots (30 KB) instead of 11 let SEVEN solver warps share an SM
- * (7 x 31 KB <= 227 KB; 254 registers x 32 x 7 fits the register file), which is what makes 8192 bands x 4 trials a
- * single wave on the 132 SMs of an H100. */
-constexpr int TPB_RING_MIN = 10;
-__host__ __device__ constexpr int tpb_ring_bytes(int ring) { return ring * 6 * 32 * 16; }
+ * One warp per CTA, 31 KB of shared memory, reused by the two phases:
+ *   factorisation     the H|b rows of the bands the warp's lanes serve (16 bands at K = 2, at most 6 at K = 6) are
+ *                     staged as chunks of TPB_CHUNK consecutive rows: one bulk copy (cp.async.bulk, one mbarrier per
+ *                     buffer) per band and chunk, double-buffered, so the next chunk is in flight while the current one
+ *                     is installed. The K lanes of a band read the same staged rows. A row is 96 bytes and the bands
+ *                     of a warp lie 76.8 KB apart (C3), so one contiguous ~1 KB run per band replaces a 96-byte piece
+ *                     per lane and row.
+ *   back substitution every thread owns a private ring of TPB_RING row slots ([slot][16-byte pair][lane], conflict free)
+ *                     that cp.async (LDGSTS) fills TPB_RING factor rows ahead of their use.
+ * No registers are spent on prefetching and the global latency is off the dependent chain. 31 KB per warp lets SEVEN
+ * solver warps share an SM (7 x 32 KB <= 228 KB; 236 registers x 32 x 7 fits the register file), which is what makes
+ * 8192 bands x 4 trials a single wave on the 132 SMs of an H100. */
+constexpr int TPB_RING = 10;
+constexpr int TPB_RING_BYTES = TPB_RING * 6 * 32 * 16;
+constexpr int TPB_CHUNK = 10;        /* rows per staged chunk */
+constexpr int TPB_STAGE_BANDS = 16;  /* bands per warp at K = 2, the smallest width (K is even) */
+/* bytes per band and buffer: an odd multiple of 16, so that the LDS.128 of 8 lanes reading 8 different bands hit
+ * 8 different bank quads */
+constexpr int TPB_STAGE_STRIDE = TPB_CHUNK * HROW * 8 + 16;
+constexpr int TPB_STAGE_BYTES = 2 * TPB_STAGE_BANDS * TPB_STAGE_STRIDE;
+constexpr int TPB_SMEM_BYTES = TPB_STAGE_BYTES + 2 * 8; /* + one mbarrier per buffer */
+static_assert(TPB_RING_BYTES <= TPB_STAGE_BYTES, "the back substitution's ring reuses the staging buffers");
+static_assert((TPB_STAGE_STRIDE / 16) % 2 == 1, "staging stride: odd number of 16-byte units");
 
 /* Factor layout of k_solve_tpb: the profile of the band. Unknown r = 4i + c is pose i (c = 0, 1, 2) or dt_i (c = 3);
  * the widest edges (acceleration: poses i..i+2, dt_i, dt_i+1) couple row r with columns >= 4i - 8 (c < 3) or 4i - 4
@@ -115,70 +130,107 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int NPEND>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(NPEND) : "memory"); }
 
-/* TPB_RING = prefetch distance in rows = slots of the private ring: 10 rows (30 KB per warp, 7 warps per SM) is the
- * default; 20 / 30 exist for experiments (TEBGPU_RING) and were slower (they cost residency). */
-template <int TPB_RING>
 __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int iteration, int round, int g) {
-  extern __shared__ __align__(16) unsigned char ring_raw[];
+  extern __shared__ __align__(16) unsigned char tpb_raw[];
   const int lane = threadIdx.x;
   const int t = blockIdx.x * 32 + lane;
   const int SPEC_K = sp.K;
   /* system t = K * slot + k; round 0: slot = band, retry rounds: slot indexes the compact list of round g */
   const int slot = t / SPEC_K;
   const int k = t - slot * SPEC_K;
-  if (retry_round_takes_lat(sp, round, g)) return; /* k_solve_lat does this round */
+  if (retry_round_takes_lat(sp, round, g)) return; /* the whole grid: k_solve_lat does this round */
   const int b = spec_band(db, sp, round, g, slot);
-  if (b < 0) return; /* threads are independent: no warp-level primitive below */
-  bool work = true;
-  const BandState* st = &db.state[b];
-  if (!st->active) work = false;
-  const int q0 = (round == 0) ? 0 : sp.qmax[b];
+  /* A lane without a system (no band, inactive band, trial past g2o's 10) stays in the factorisation as an empty
+   * system (N = 0, identity rows only) until the warp's staging is done: the warp stages the rows together. */
+  bool work = b >= 0;
+  if (work && !db.state[b].active) work = false;
+  const int q0 = (!work || round == 0) ? 0 : sp.qmax[b];
   if (q0 + k >= 10) work = false;
-  if (!work) return;
-  const int n = db.n[b];
+  const int n = work ? db.n[b] : 0;
   const int N = 4 * n;
-  double lambda, ni;
-  if (round == 0 && iteration == 0) { lambda = band_lambda_init(db, b, n); ni = 2; }
-  else { lambda = st->lambda; ni = st->ni; }
-  spec_lambda(lambda, ni, k);
+  const int Nw = (int)__reduce_max_sync(0xffffffffu, (unsigned)N); /* the factorisation runs to the warp's largest N */
+  if (Nw == 0) return; /* the whole warp: no system (retry rounds: past the end of the list) */
+  double lambda = 0, ni = 2;
+  if (work) {
+    const BandState* st = &db.state[b];
+    if (round == 0 && iteration == 0) { lambda = band_lambda_init(db, b, n); ni = 2; }
+    else { lambda = st->lambda; ni = st->ni; }
+    spec_lambda(lambda, ni, k);
+  }
 
-  const double* gH = db.Hb + (size_t)b * 4 * db.n_cap * HROW;
   /* factor and solution live in warp-interleaved scratch ([row][16-byte pair][lane] / [row][lane]) so that the 32
    * threads of a warp - 32 different (band, trial) systems - store and load contiguous 512 / 256 byte runs */
   double2* gL = reinterpret_cast<double2*>(sp.Lf + (size_t)blockIdx.x * 32 * 4 * db.n_cap * HROW) + lane;
   double* gx = sp.dx + (size_t)blockIdx.x * 32 * 4 * db.n_cap + lane;
-  double* res = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
-  const uint32_t ring = smem_u32(ring_raw) + (uint32_t)lane * 16u;                 /* + (slot*6 + pair)*512 */
-  const double2* ringp = reinterpret_cast<const double2*>(ring_raw) + lane;       /* [(slot*6 + pair)*32]  */
+
+  /* H|b staging: chunk c (rows c TPB_CHUNK ..) of the warp's bands goes to buffer c & 1, band at (slot - slot0) x stride.
+   * The first lane of a band in this warp copies it; if that lane has no system, neither have the band's later lanes
+   * (k is larger). Rows are copied up to the band's N only, so never past 4 n_cap. */
+  uint64_t* bar = reinterpret_cast<uint64_t*>(tpb_raw + TPB_STAGE_BYTES);
+  const int slot0 = (blockIdx.x * 32) / SPEC_K;
+  const bool stager = work && (k == 0 || lane == 0);
+  const double* gH = db.Hb + (size_t)(work ? b : 0) * 4 * db.n_cap * HROW;
+  const unsigned char* stage_band = tpb_raw + (slot - slot0) * TPB_STAGE_STRIDE;
+  auto stage_chunk = [&](int c) {
+    const int r0 = c * TPB_CHUNK;
+    const uint32_t bytes = stager && r0 < N ? (uint32_t)(min(TPB_CHUNK, N - r0) * HROW * 8) : 0u;
+    const uint32_t total = __reduce_add_sync(0xffffffffu, bytes);
+    if (lane == 0) mbar_expect_tx(bar + (c & 1), total);
+    __syncwarp();
+    if (bytes)
+      tma_load_1d(const_cast<unsigned char*>(stage_band) + (c & 1) * TPB_STAGE_BANDS * TPB_STAGE_STRIDE, gH + (size_t)r0 * HROW,
+                  bytes, bar + (c & 1));
+  };
+  /* row r of chunk c, position r - c TPB_CHUNK */
+  auto staged_row = [&](int c, int pos) {
+    return reinterpret_cast<const double2*>(stage_band + (c & 1) * TPB_STAGE_BANDS * TPB_STAGE_STRIDE + pos * HROW * 8);
+  };
+  /* chunk c + 1 goes to the buffer chunk c - 1 used: every lane has read it (the fence orders those generic-proxy
+   * reads before the bulk copy's writes), then wait for chunk c */
+  auto next_chunk = [&](int c) {
+    fence_proxy_async();
+    __syncwarp();
+    stage_chunk(c + 1);
+    mbar_wait(bar + (c & 1), (uint32_t)(c >> 1) & 1u);
+  };
+  if (lane == 0) {
+    mbar_init(bar, 1);
+    mbar_init(bar + 1, 1);
+    mbar_fence_init();
+  }
+  __syncwarp();
+  stage_chunk(0);
+  stage_chunk(1);
+  mbar_wait(bar, 0);
 
   /* E[k][m]: H[r][r-k] of the window row r with r % 11 == m; Y[m]: its right-hand side */
   double E[11][11], Y[11];
-  /* prologue: rows 0..10 straight into the window, rows 11..21 into the ring */
+  /* prologue: rows 0..10 straight into the window (N >= 12 for every lane with a system) */
+  static_assert(TPB_CHUNK == 10, "the prologue's rows 0..10 are chunk 0 and the first row of chunk 1");
 #pragma unroll
   for (int m = 0; m < 11; ++m) {
-    const double2* src = reinterpret_cast<const double2*>(gH + (size_t)m * HROW); /* N >= 12 */
+    if (m == TPB_CHUNK) next_chunk(1);
     double h[12];
+    if (m < N) {
+      const double2* src = staged_row(m / TPB_CHUNK, m % TPB_CHUNK);
 #pragma unroll
-    for (int v = 0; v < 6; ++v) { const double2 d2 = __ldg(src + v); h[2 * v] = d2.x; h[2 * v + 1] = d2.y; }
-    if (row_is_real(m, n)) h[0] += lambda;
+      for (int v = 0; v < 6; ++v) { const double2 d2 = src[v]; h[2 * v] = d2.x; h[2 * v + 1] = d2.y; }
+      if (row_is_real(m, n)) h[0] += lambda;
+    } else {
+#pragma unroll
+      for (int v = 0; v < 12; ++v) h[v] = 0.0;
+      h[0] = 1.0;
+    }
 #pragma unroll
     for (int kk = 0; kk < 11; ++kk) E[kk][m] = (kk <= m) ? h[kk] : 0.0;
     Y[m] = h[11];
   }
-#pragma unroll
-  for (int m = 0; m < TPB_RING; ++m) {
-    const int r = 11 + m;
-    if (r < N) {
-#pragma unroll
-      for (int v = 0; v < 6; ++v) cp_async16(ring + (uint32_t)((m * 6 + v) * 512), gH + (size_t)r * HROW + 2 * v);
-    }
-    cp_async_commit();
-  }
   bool ok = true;
-  int rs = 0; /* ring slot that holds row j + 11 */
-  /* rows N .. Npad-1 are identity rows: every block of 11 pivots runs unconditionally, which keeps the register
-   * window's liveness static (a data-dependent early exit makes the compiler keep all 121 slots alive) */
-  for (int j0 = 0; j0 < N; j0 += 11) {
+  int cr = 1, pr = 1; /* chunk and position of row j + 11 */
+  /* rows from N up to the warp's largest N, padded to a multiple of 11, are identity rows: every block of 11 pivots
+   * runs unconditionally, which keeps the register window's liveness static (a data-dependent early exit makes the
+   * compiler keep all 121 slots alive) */
+  for (int j0 = 0; j0 < Nw; j0 += 11) {
 #pragma unroll
     for (int s = 0; s < 11; ++s) {
       const int j = j0 + s;
@@ -207,13 +259,17 @@ __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int 
         }
         if (u == 10 && live && c == 0) dst[5 * 32] = make_double2(lu, 0.0);
       }
-      /* install row j + 11 (copied into ring slot rs TPB_RING pivots ago), then refill the slot with row j + 11 + TPB_RING */
-      cp_async_wait<TPB_RING - 1>();
+      /* install row j + 11 from the staged chunk */
       const int rn = j + 11;
+      if (pr == TPB_CHUNK) { /* warp-uniform: j advances in lockstep */
+        next_chunk(++cr);
+        pr = 0;
+      }
       if (rn < N) {
+        const double2* src = staged_row(cr, pr);
 #pragma unroll
-        for (int v = 0; v < 5; ++v) { const double2 d2 = ringp[(rs * 6 + v) * 32]; E[2 * v][s] = d2.x; E[2 * v + 1][s] = d2.y; }
-        const double2 d2 = ringp[(rs * 6 + 5) * 32];
+        for (int v = 0; v < 5; ++v) { const double2 d2 = src[v]; E[2 * v][s] = d2.x; E[2 * v + 1][s] = d2.y; }
+        const double2 d2 = src[5];
         E[10][s] = d2.x;
         Y[s] = d2.y;
         if (row_is_real(rn, n)) E[0][s] += lambda;
@@ -223,22 +279,24 @@ __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int 
         E[0][s] = 1.0;
         Y[s] = 0.0;
       }
-      if (rn + TPB_RING < N) {
-#pragma unroll
-        for (int v = 0; v < 6; ++v) cp_async16(ring + (uint32_t)((rs * 6 + v) * 512), gH + (size_t)(rn + TPB_RING) * HROW + 2 * v);
-      }
-      cp_async_commit();
-      rs = (rs + 1 == TPB_RING) ? 0 : rs + 1;
+      ++pr;
     }
   }
-  cp_async_wait<0>();
+  /* chunk cr + 1 holds no row below any lane's N (all of them were installed), so it completes at once; waiting for
+   * it keeps the bulk copies off the shared memory the back substitution reuses */
+  mbar_wait(bar + ((cr + 1) & 1), (uint32_t)((cr + 1) >> 1) & 1u);
+  __syncwarp();
+  if (!work) return;
+  double* res = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
   res[5] = ok ? 1.0 : 0.0;
   res[6] = lambda;
   if (!ok) return; /* CSparse failure: k_trial_eval uses dx = b */
 
   /* back substitution x_j = z_j - sum_u L[j+u][j] x_{j+u}; X[m]: x of the row with r % 11 == m.
-   * The factor rows written above are read back through the same cp.async ring, 11 rows ahead: tpb_pairs(j & 3) of the
-   * slot's 6 pairs. */
+   * The factor rows written above are read back through a per-lane cp.async ring in the staging buffers, TPB_RING rows
+   * ahead: tpb_pairs(j & 3) of the slot's 6 pairs. */
+  const uint32_t ring = smem_u32(tpb_raw) + (uint32_t)lane * 16u;               /* + (slot*6 + pair)*512 */
+  const double2* ringp = reinterpret_cast<const double2*>(tpb_raw) + lane;     /* [(slot*6 + pair)*32]  */
   auto fetch_row = [&](int slot, int j) {
     const double2* src = tpb_row(gL, j);
     const int np = tpb_pairs(j & 3);
@@ -256,7 +314,7 @@ __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int 
     if (j < N) fetch_row(c, j);
     cp_async_commit();
   }
-  rs = 0;
+  int rs = 0; /* ring slot that holds row j */
   for (int j0 = jtop; j0 >= 0; j0 -= 11) {
 #pragma unroll
     for (int s = 10; s >= 0; --s) {
