@@ -311,6 +311,31 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which);
 int32_t tebgpu_build_system(tebgpu_ctx* ctx, const TebBatch* batch, int32_t outer_index,
                             double* Hb_out, double* chi2_out, int32_t device_ptrs);
 
+/* Solve only: the linear solve of the LM step, (H + lambda_k I_real) x = b for bands 0 .. B-1 and trials k = 0 .. K-1,
+ * through the kernel the context's solver selects (tebgpu_set_solver; for solver 2 the mapping of
+ * tebgpu_set_warp_solver, launched by the same code as in tebgpu_optimize_batch). Test / profiling entry point of the
+ * solve kernels. HOST buffers:
+ *   Hb [B][4 n_cap][12]  system in kernel A's layout; NULL: the one the last tebgpu_build_system left in the context
+ *                        (n and n_cap must then be the ones of that call);
+ *   n [B]                poses per band, 3 .. n_cap;
+ *   lambda, nu [B]       damping at the first trial of the round; trial k uses lambda nu (2 nu) ... (k factors), as
+ *                        g2o's retries do. NULL: LM iteration 0, lambda = 1e-5 max |H_rr| over the real rows from kernel
+ *                        A's partials (only valid after tebgpu_build_system);
+ *   active [B]           or NULL (every band active); an inactive band solves nothing;
+ *   K                    trials per band: 2, 4, 6 or 8;
+ *   qmax [B], list       NULL / 0: round 0 over all bands. Otherwise a retry round over the list_len bands of `list`
+ *                        (in that order) whose first qmax[b] trials were already used: trials with qmax[b] + k >= 10 are
+ *                        not solved. Needs lambda;
+ *   lat_cap              retry rounds with solve mapping 4: > 0 launches both k_solve_lat (lat_cap systems) and
+ *                        k_solve_tpb, the list length decides on the device which one works; 0: automatic.
+ * Outputs: dx_out [B][K][4 n_cap], ok_out [B][K] (1 solved, 0 not positive definite or not finite), lambda_out [B][K].
+ * The solver scratch is filled with all-ones bytes (a NaN) before the launch, and what a kernel did not write is
+ * returned as that pattern: the rows >= 4 n of a band, the systems that did not run, dx of a failed solve. */
+int32_t tebgpu_solve_system(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, const double* Hb, const int32_t* n,
+                            const double* lambda, const double* nu, const int32_t* active, int32_t K, const int32_t* qmax,
+                            const int32_t* list, int32_t list_len, int32_t lat_cap, double* dx_out, double* ok_out,
+                            double* lambda_out);
+
 /* TebOptimalPlanner::computeCurrentCost called OUTSIDE optimizeTEB (optimal_planner.cpp:1041-1094, graph rebuilt with
  * weight multiplier 1, errors evaluated at the current state): HOST buffers; writes cost[], chi2[], status[]. */
 int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* batch, const TebOptimizeArgs* args);

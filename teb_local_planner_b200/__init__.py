@@ -80,6 +80,9 @@ def load_library(build_if_missing=False):
     L.tebgpu_h_signature.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, C.c_int32]
     L.tebgpu_build_system.restype = C.c_int32
     L.tebgpu_build_system.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, vp, C.c_int32]
+    L.tebgpu_solve_system.restype = C.c_int32
+    L.tebgpu_solve_system.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32,
+                                      vp, vp, vp]
     L.tebgpu_select_best.restype = C.c_int32
     L.tebgpu_select_best.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double]
     L.tebgpu_auto_resize_host.restype = C.c_int32
@@ -229,6 +232,32 @@ class TebGpu:
         self._check(self.lib.tebgpu_build_system(self.ctx, C.byref(bs), outer_index, Hb.ctypes.data, chi2.ctypes.data, 0),
                     "tebgpu_build_system")
         return Hb, chi2
+
+    def solve_system(self, n, K, Hb=None, n_cap=None, lam=None, nu=None, active=None, qmax=None, order=None, lat_cap=0):
+        """Solve (H + lambda_k I_real) x = b for every band and trial k < K with the context's solver / solve mapping
+        (tebgpu_solve_system). Hb [B][4 n_cap][12] or None (the system of the last build_system: pass n_cap); lam / nu
+        [B] or None (LM iteration 0: lambda from kernel A); active [B] or None; qmax [B] + order (list of bands): a
+        retry round over `order`. Returns (dx [B][K][4 n_cap], ok [B][K], lambda [B][K]); what no kernel wrote keeps
+        the all-ones NaN pattern."""
+        import numpy as np
+        n = np.ascontiguousarray(n, dtype=np.int32)
+        B = n.size
+        if Hb is not None:
+            Hb = np.ascontiguousarray(Hb, dtype=np.float64)
+            n_cap = Hb.shape[1] // 4
+        f64 = lambda a: None if a is None else np.ascontiguousarray(np.broadcast_to(a, (B,)), dtype=np.float64)
+        lam, nu = f64(lam), f64(nu)
+        active = None if active is None else np.ascontiguousarray(active, dtype=np.int32)
+        qmax = None if qmax is None else np.ascontiguousarray(qmax, dtype=np.int32)
+        order = None if order is None else np.ascontiguousarray(order, dtype=np.int32)
+        dx = np.empty((B, K, 4 * n_cap))
+        ok = np.empty((B, K))
+        lam_used = np.empty((B, K))
+        self._check(self.lib.tebgpu_solve_system(self.ctx, B, int(n_cap), abi.ptr(Hb), n.ctypes.data, abi.ptr(lam), abi.ptr(nu),
+                                                 abi.ptr(active), int(K), abi.ptr(qmax), abi.ptr(order),
+                                                 0 if order is None else order.size, int(lat_cap), dx.ctypes.data,
+                                                 ok.ctypes.data, lam_used.ctypes.data), "tebgpu_solve_system")
+        return dx, ok, lam_used
 
     def close(self):
         if self.ctx:

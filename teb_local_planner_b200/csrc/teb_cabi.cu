@@ -553,6 +553,39 @@ static DevBatch make_devbatch(tebgpu_ctx* ctx, const TebBatch* bt) {
   return d;
 }
 
+/* The solve launch of one round of the speculative solver (solver 2) over the db.B bands, K trials each, on stream s:
+ * the kernel tebgpu_set_warp_solver selects, its grid and shared memory. Shared by issue_optimize and
+ * tebgpu_solve_system. lat_cap > 0 (retry rounds, mode 4) forces the dual launch with that many k_solve_lat systems;
+ * 0 sizes it automatically. Returns the number of kernels launched. */
+static int launch_spec_solve(const tebgpu_ctx* ctx, const DevBatch& db, const SpecBufs& spec, int K, int it, int round, int g,
+                             cudaStream_t s, int lat_cap) {
+  const int bk = db.B * K;
+  const int warps = (bk + 31) / 32;
+  /* k_solve_warp: the sequential order spread over a warp (cross-check only) */
+  const bool warp_solver = ctx->warp_solver == 1 || (ctx->warp_solver == 2 && bk <= ctx->sms * 8);
+  const size_t smem_lat = solve_lat_smem_bytes(db.n_cap);
+  /* automatic: while the round's systems fit LAT_WAVES waves of resident CTAs (one warp + its whole system per CTA)
+   * the twisted solver's short per-wave chain beats the fixed time a thread-per-system solve takes
+   * regardless of the count */
+  const long long lat_wave = smem_lat <= 232448 ? (long long)ctx->sms * (232448 / smem_lat > 16 ? 16 : 232448 / smem_lat) : 0;
+  const bool dual = round > 0 && ctx->warp_solver == 4 && lat_wave > 0;
+  const bool lat_solver = lat_wave > 0 && (ctx->warp_solver == 3 || (ctx->warp_solver == 4 && bk <= LAT_WAVES * lat_wave && lat_cap == 0));
+  if (lat_solver) k_solve_lat<<<bk, 32, smem_lat, s>>>(db, spec, it, round, g);
+  else if (dual) {
+    /* retry round of the throughput regime: both mappings are launched, the list length decides on the device */
+    SpecBufs sl = spec;
+    long long cap = lat_cap > 0 ? lat_cap : LAT_WAVES * lat_wave;
+    cap = cap < bk ? cap : bk;
+    sl.lat_cap = (int32_t)cap;
+    k_solve_lat<<<(unsigned)cap, 32, smem_lat, s>>>(db, sl, it, round, g);
+    k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, sl, it, round, g);
+    return 2;
+  }
+  else if (warp_solver) k_solve_warp<<<(bk + SW_WARPS - 1) / SW_WARPS, 32 * SW_WARPS, 0, s>>>(db, spec, it, round, g);
+  else k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, spec, it, round, g);
+  return 1;
+}
+
 /* the launch sequence of one optimizeTEB over the batch, issued on `st` (directly, or into a stream capture) */
 static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args, cudaStream_t st) {
   DevBatch db = make_devbatch(ctx, bt);
@@ -667,29 +700,7 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
         const bool fork = overlap && rounds > 1 && !kp.has_vor;
         cudaStream_t rs = st;
         auto launch_solve = [&](const SpecBufs& spec, int K, int round, cudaStream_t s) {
-          const int bk = B * K;
-          const int warps = (bk + 31) / 32;
-          /* k_solve_warp: the sequential order spread over a warp (cross-check only) */
-          const bool warp_solver = ctx->warp_solver == 1 || (ctx->warp_solver == 2 && bk <= ctx->sms * 8);
-          const size_t smem_lat = solve_lat_smem_bytes(bt->n_cap);
-          /* automatic: while the round's systems fit LAT_WAVES waves of resident CTAs (one warp + its whole system per CTA)
-           * the twisted solver's short per-wave chain beats the fixed time a thread-per-system solve takes
-           * regardless of the count */
-          const long long lat_wave = smem_lat <= 232448 ? (long long)ctx->sms * (232448 / smem_lat > 16 ? 16 : 232448 / smem_lat) : 0;
-          const bool lat_solver = lat_wave > 0 && (ctx->warp_solver == 3 || (ctx->warp_solver == 4 && bk <= LAT_WAVES * lat_wave));
-          if (lat_solver) k_solve_lat<<<bk, 32, smem_lat, s>>>(db, spec, it, round, g);
-          else if (round > 0 && ctx->warp_solver == 4 && lat_wave > 0) {
-            /* retry round of the throughput regime: both mappings are launched, the list length decides on the device */
-            SpecBufs sl = spec;
-            const long long cap = LAT_WAVES * lat_wave < bk ? LAT_WAVES * lat_wave : bk;
-            sl.lat_cap = (int32_t)cap;
-            k_solve_lat<<<(unsigned)cap, 32, smem_lat, s>>>(db, sl, it, round, g);
-            k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, sl, it, round, g);
-            ++launches;
-          }
-          else if (warp_solver) k_solve_warp<<<(bk + SW_WARPS - 1) / SW_WARPS, 32 * SW_WARPS, 0, s>>>(db, spec, it, round, g);
-          else k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, spec, it, round, g);
-          ++launches;
+          launches += launch_spec_solve(ctx, db, spec, K, it, round, g, s, 0);
         };
         for (int round = 0; round < rounds; ++round, ++g) {
           const int K = sched[round];
@@ -1080,6 +1091,103 @@ int32_t tebgpu_build_system(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_i
     delete[] hn;
   }
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_solve_system(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, const double* Hb, const int32_t* n,
+                            const double* lambda, const double* nu, const int32_t* active, int32_t K, const int32_t* qmax,
+                            const int32_t* list, int32_t list_len, int32_t lat_cap, double* dx_out, double* ok_out,
+                            double* lambda_out) {
+  if (!ctx || !n || !dx_out || !ok_out || !lambda_out) return TEBGPU_ERR_INVALID_ARG;
+  if (B < 1 || n_cap < 3 || !(K == 2 || K == 4 || K == 6 || K == 8)) { ctx->err = "bad solve dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (B > ctx->lim.max_bands || n_cap > ctx->lim.max_poses) { ctx->err = "solve exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+  const bool retry = qmax != nullptr;
+  if (retry && (!list || list_len < 0 || list_len > B || !lambda)) { ctx->err = "a retry round needs its list and lambda"; return TEBGPU_ERR_INVALID_ARG; }
+  if ((lambda == nullptr) != (nu == nullptr)) { ctx->err = "lambda and nu go together"; return TEBGPU_ERR_INVALID_ARG; }
+  if (lat_cap < 0 || (lat_cap > 0 && (!retry || ctx->solver != 2 || ctx->warp_solver != 4))) {
+    ctx->err = "lat_cap applies to retry rounds of solve mapping 4";
+    return TEBGPU_ERR_INVALID_ARG;
+  }
+  for (int b = 0; b < B; ++b)
+    if (n[b] < 3 || n[b] > n_cap) { ctx->err = "n[b] outside 3 .. n_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  if (retry)
+    for (int s = 0; s < list_len; ++s)
+      if (list[s] < 0 || list[s] >= B || qmax[list[s]] < 0 || qmax[list[s]] > 10) { ctx->err = "bad retry list"; return TEBGPU_ERR_INVALID_ARG; }
+  const bool use_bcr = ctx->solver == 1 && n_cap <= BCR_MAX_POSES && kb_bcr_smem_bytes(n_cap, 0) <= 232448 &&
+                       ctx->lim.max_poses <= BCR_MAX_POSES;
+  if (ctx->solver == 1 && !use_bcr) { ctx->err = "block cyclic reduction needs max_poses <= 256"; return TEBGPU_ERR_UNSUPPORTED; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t per_band = (size_t)4 * n_cap * HROW;
+  if (Hb) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->Hb, Hb, (size_t)B * per_band * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_n, n, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  std::vector<BandState> bs((size_t)B);
+  for (int b = 0; b < B; ++b) {
+    std::memset(&bs[b], 0, sizeof(BandState));
+    bs[b].lambda = lambda ? lambda[b] : 0.0;
+    bs[b].ni = nu ? nu[b] : 2.0;
+    bs[b].active = active ? (active[b] != 0) : 1;
+  }
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->state, bs.data(), (size_t)B * sizeof(BandState), cudaMemcpyHostToDevice, st));
+  DevBatch db;
+  std::memset(&db, 0, sizeof(db));
+  db.B = B; db.n_cap = n_cap; db.S = 1;
+  db.n = ctx->d_n; db.Hb = ctx->Hb; db.state = ctx->state; db.dmax_parts = ctx->dmax_parts; db.defer = ctx->defer;
+  db.tile = ctx->linearize_variant == 1 ? TP : KA2_TP; /* the tiles of kernel A's partials (tebgpu_build_system) */
+  db.chunks = (n_cap + db.tile - 1) / db.tile;
+  SpecBufs spec = ctx->spec;
+  spec.K = K; spec.sel_list = nullptr; spec.sel_cnt = nullptr; spec.defer = nullptr; spec.skip_tag = 0; spec.lat_cap = 0;
+  /* retry rounds read list g % SPEC_LISTS and its length cnt[g]: round 1 = running round index 1 */
+  const int round = retry ? 1 : 0, g = retry ? 1 : 0;
+  const int it = lambda ? 1 : 0; /* iteration 0 of round 0 takes lambda from kernel A's partials */
+  if (retry) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(spec.qmax, qmax, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (list_len > 0)
+      CUDA_TRY(ctx, cudaMemcpyAsync(spec.list + (size_t)(g % SPEC_LISTS) * B, list, (size_t)list_len * sizeof(int32_t),
+                                    cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(spec.cnt + g, &list_len, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  }
+  const int bk = B * K;
+  const size_t sys = (size_t)((bk + 31) / 32) * 32;    /* whole warps of systems */
+  const size_t dx_len = sys * 4 * n_cap;
+  CUDA_TRY(ctx, cudaMemsetAsync(spec.dx, 0xff, dx_len * sizeof(double), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(spec.res, 0xff, (size_t)B * SPEC_K_MAX * RES_STRIDE * sizeof(double), st));
+  if (ctx->solver == 2) {
+    ctx->launches = launch_spec_solve(ctx, db, spec, K, it, round, g, st, lat_cap);
+  } else if (use_bcr) {
+    const size_t smem = kb_bcr_smem_bytes(n_cap, 0);
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_solve_seq<1, KB_BCR_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_solve_seq<1, KB_BCR_THREADS><<<bk, KB_BCR_THREADS, smem, st>>>(db, spec, it, round, g);
+    ctx->launches = 1;
+  } else {
+    const size_t smem = per_band * sizeof(double) + 16;
+    if (smem > 232448) { ctx->err = "band staging exceeds shared memory"; return TEBGPU_ERR_CAPACITY; }
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_solve_seq<0, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_solve_seq<0, 32><<<bk, 32, smem, st>>>(db, spec, it, round, g);
+    ctx->launches = 1;
+  }
+  CUDA_TRY(ctx, cudaGetLastError());
+  std::vector<double> dx(dx_len), res((size_t)B * SPEC_K_MAX * RES_STRIDE);
+  CUDA_TRY(ctx, cudaMemcpyAsync(dx.data(), spec.dx, dx_len * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(res.data(), spec.res, res.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  /* system t = K slot + k sits in lane t & 31 of warp t >> 5, row r at r * 32; slot = band (round 0) or list position */
+  std::memset(dx_out, 0xff, (size_t)B * K * 4 * n_cap * sizeof(double));
+  const int slots = retry ? list_len : B;
+  for (int s = 0; s < slots; ++s) {
+    const int b = retry ? list[s] : s;
+    for (int k = 0; k < K; ++k) {
+      const size_t t = (size_t)K * s + k;
+      const double* src = dx.data() + (t >> 5) * 32 * 4 * n_cap + (t & 31);
+      double* dst = dx_out + ((size_t)b * K + k) * 4 * n_cap;
+      for (int r = 0; r < 4 * n_cap; ++r) dst[r] = src[(size_t)r * 32];
+    }
+  }
+  for (int b = 0; b < B; ++b)
+    for (int k = 0; k < K; ++k) {
+      ok_out[(size_t)b * K + k] = res[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + 5];
+      lambda_out[(size_t)b * K + k] = res[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + 6];
+    }
   return TEBGPU_OK;
 }
 

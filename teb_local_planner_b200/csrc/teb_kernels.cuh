@@ -1134,7 +1134,8 @@ __device__ __forceinline__ void eval_chi2_parts(const KParams& kp, const DevBatc
 
 /* ------------------------------------------------------------------ banded LDL^T + substitutions, one warp, in
  * shared memory. Hs[N][12]: on entry band + rhs, on exit L (unit lower, offsets 1..10), 1/d (offset 0) and the
- * solution (offset 11). Returns false on a non-positive / non-finite pivot (LinearSolverCSparse would fail). */
+ * solution (offset 11). Returns false on a non-positive / non-finite pivot (LinearSolverCSparse would fail) or a
+ * non-finite solution. */
 __device__ __forceinline__ bool warp_band_solve(double* Hs, int N, int n, double lambda) {
   const int lane = threadIdx.x & 31;
   /* trailing-window entries handled by this lane: e in {lane, lane+32, lane+64}; e < 55 -> (u,q), 1<=q<=u<=10;
@@ -1190,7 +1191,9 @@ __device__ __forceinline__ bool warp_band_solve(double* Hs, int N, int n, double
     if (lane >= 1 && lane <= 10 && j - lane >= 0) Hs[(j - lane) * HROW + 11] -= Hs[j * HROW + lane] * xj;
     __syncwarp();
   }
-  return true;
+  /* and every component of the solution finite (a NaN in b leaves the pivots alone): the rule of every solve kernel */
+  for (int j = lane; j < N; j += 32) ok = ok && isfinite(Hs[j * HROW + 11]);
+  return __all_sync(0xffffffffu, ok);
 }
 
 /* ------------------------------------------------------------------ block cyclic reduction (BCR) solver
@@ -1203,6 +1206,7 @@ __device__ __forceinline__ bool warp_band_solve(double* Hs, int N, int n, double
  *   W^L = C^-1 A_ip, W^R = C^-1 A_iq (stored transposed in q's coupling slot), w = C^-1 b_i,
  *   D_p -= W^L^T W^L, D_q -= W^R^T W^R, A_qp(new) = -W^R^T W^L, b_p -= W^L^T w, b_q -= W^R^T w,
  *   back-substitution x_i = C^-T (w - W^L x_p - W^R x_q). Only C^-1 (packed lower) is stored. */
+__host__ __device__ inline int bcr_blocks(int n_cap) { return (4 * n_cap + 7) / 8; }
 struct BcrSmem {
   double* Dp;     /* [m][36] packed lower diagonal blocks -> C^-1 after elimination */
   double* L0;     /* [m][64] level-0 left couplings A_{i,i-1}, row major             */
@@ -1410,6 +1414,60 @@ __device__ __forceinline__ void bcr_solve(const BcrSmem& S, int m, int* s_fail) 
     }
     __syncthreads();
   }
+  /* a solve also fails on a non-finite solution (a NaN in b leaves the pivots alone): the rule of every solve kernel */
+  for (int r = tid; r < 8 * m; r += NT)
+    if (!isfinite(S.xs[r])) *s_fail = 1;
+  __syncthreads();
+}
+
+/* BCR staging: the band rows [N][12] (+ lambda on the real diagonals) expanded into the 8x8 blocks of S (coalesced
+ * 16-byte loads of each 96-byte row); rows N .. 8m - 1 are identity rows. b0 receives the right-hand side. */
+template <int NT>
+__device__ __forceinline__ void bcr_stage(const BcrSmem& S, double* b0, const double* gH, int N, int n, int m, double lambda) {
+  for (int r = threadIdx.x; r < 8 * m; r += NT) {
+    const int i = r >> 3, a = r & 7;
+    double* Lrow = S.L0 + 64 * i + 8 * a;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) Lrow[c] = 0.0;
+    double* Dblk = S.Dp + 36 * i;
+    if (r < N) {
+      const double2* src = reinterpret_cast<const double2*>(gH + (size_t)r * HROW);
+      double h[12];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) { const double2 v2 = src[k]; h[2 * k] = v2.x; h[2 * k + 1] = v2.y; }
+      if (row_is_real(r, n)) h[0] += lambda;
+#pragma unroll
+      for (int k = 0; k < 11; ++k) {
+        const int c = a - k;
+        if (c >= 0) Dblk[PIDX(a, c)] = h[k];
+        else if (c >= -8) Lrow[8 + c] = h[k];
+      }
+      S.bs[r] = h[11];
+      b0[r] = h[11];
+    } else {
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        if (c <= a) Dblk[PIDX(a, c)] = (c == a) ? 1.0 : 0.0;
+      S.bs[r] = 0.0;
+      b0[r] = 0.0;
+    }
+  }
+}
+
+/* shared-memory carve-up of the BCR solver for n_cap poses (kb_bcr_smem_bytes) and a system of m blocks; b0: [8 m] */
+__device__ __forceinline__ BcrSmem bcr_carve(double* base, int n_cap, int m, double*& b0) {
+  const int mc = bcr_blocks(n_cap);
+  BcrSmem S;
+  S.Dp = base;
+  S.L0 = S.Dp + 36 * mc;
+  S.Lpool = S.L0 + 64 * mc;
+  S.bs = S.Lpool + 64 * (mc + 12);
+  S.xs = S.bs + 8 * mc;
+  b0 = S.xs + 8 * mc;
+  S.off[0] = 0;
+  S.off[1] = 0;
+  for (int l = 1; l < 11; ++l) S.off[l + 1] = S.off[l] + ((m + (1 << l) - 1) >> l);
+  return S;
 }
 
 /* ------------------------------------------------------------------ k_lm_step ("kernel B"), CTA per band.
@@ -1421,7 +1479,6 @@ constexpr int KB_BCR_THREADS = 256;
 __host__ __device__ inline size_t kb_smem_bytes(int n_cap, int M_cap) {
   return ((size_t)4 * n_cap * HROW + (size_t)4 * n_cap + 64) * sizeof(double) + (size_t)M_cap * sizeof(TebObstacle) + 64;
 }
-__host__ __device__ inline int bcr_blocks(int n_cap) { return (4 * n_cap + 7) / 8; }
 __host__ __device__ inline size_t kb_bcr_smem_bytes(int n_cap, int M_cap) {
   const size_t m = bcr_blocks(n_cap);
   /* Dp 36m + L0 64m + Lpool 64(m + 12) + bs 8m + xs 8m + b0 8m + trial poses 4 n_cap + scratch 64 */
@@ -1451,19 +1508,9 @@ __global__ void __launch_bounds__(NT, SOLVER == 1 ? 2 : 1) k_lm_step_t(DevBatch 
     Hs = reinterpret_cast<double*>(smem_raw);
     sT = Hs + (size_t)4 * db.n_cap * HROW;
   } else {
-    const int mc = bcr_blocks(db.n_cap);
     m = (N + 7) / 8;
-    double* base = reinterpret_cast<double*>(smem_raw);
-    S.Dp = base;
-    S.L0 = S.Dp + 36 * mc;
-    S.Lpool = S.L0 + 64 * mc;
-    S.bs = S.Lpool + 64 * (mc + 12);
-    S.xs = S.bs + 8 * mc;
-    b0 = S.xs + 8 * mc;
-    sT = b0 + 8 * mc;
-    S.off[0] = 0;
-    S.off[1] = 0;
-    for (int l = 1; l < 11; ++l) S.off[l + 1] = S.off[l] + ((m + (1 << l) - 1) >> l);
+    S = bcr_carve(reinterpret_cast<double*>(smem_raw), db.n_cap, m, b0);
+    sT = b0 + 8 * bcr_blocks(db.n_cap);
   }
   sRed = sT + (size_t)4 * db.n_cap; /* 64 doubles scratch */
   uint64_t* bar = reinterpret_cast<uint64_t*>(sRed + 56);
@@ -1530,35 +1577,7 @@ __global__ void __launch_bounds__(NT, SOLVER == 1 ? 2 : 1) k_lm_step_t(DevBatch 
       __syncthreads();
       ok2 = s_flag[0] != 0;
     } else {
-      /* expand the band rows into 8x8 blocks (coalesced 16-byte loads of each 96-byte row) */
-      for (int r = tid; r < 8 * m; r += NT) {
-        const int i = r >> 3, a = r & 7;
-        double* Lrow = S.L0 + 64 * i + 8 * a;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) Lrow[c] = 0.0;
-        double* Dblk = S.Dp + 36 * i;
-        if (r < N) {
-          const double2* src = reinterpret_cast<const double2*>(gH + (size_t)r * HROW);
-          double h[12];
-#pragma unroll
-          for (int k = 0; k < 6; ++k) { const double2 v2 = src[k]; h[2 * k] = v2.x; h[2 * k + 1] = v2.y; }
-          if (row_is_real(r, n)) h[0] += lambda;
-#pragma unroll
-          for (int k = 0; k < 11; ++k) {
-            const int c = a - k;
-            if (c >= 0) Dblk[PIDX(a, c)] = h[k];
-            else if (c >= -8) Lrow[8 + c] = h[k];
-          }
-          S.bs[r] = h[11];
-          b0[r] = h[11];
-        } else {
-#pragma unroll
-          for (int c = 0; c < 8; ++c)
-            if (c <= a) Dblk[PIDX(a, c)] = (c == a) ? 1.0 : 0.0;
-          S.bs[r] = 0.0;
-          b0[r] = 0.0;
-        }
-      }
+      bcr_stage<NT>(S, b0, gH, N, n, m, lambda);
       if (tid == 0) s_flag[1] = 0;
       __syncthreads();
       bcr_solve<NT>(S, m, &s_flag[1]);

@@ -152,8 +152,11 @@ __global__ void __launch_bounds__(32 * SW_WARPS) k_solve_warp(DevBatch db, SpecB
     cur ^= 1;
   }
   cp_async_wait<0>();
-  if (lane == 0) { res[5] = ok ? 1.0 : 0.0; res[6] = lambda; }
-  if (!ok) return; /* CSparse failure: k_trial_eval2 uses dx = b */
+  if (lane == 0) res[6] = lambda;
+  if (!ok) { /* CSparse failure: k_trial_eval2 uses dx = b */
+    if (lane == 0) res[5] = 0.0;
+    return;
+  }
   __syncwarp();
   __threadfence_block();
 
@@ -177,12 +180,15 @@ __global__ void __launch_bounds__(32 * SW_WARPS) k_solve_warp(DevBatch db, SpecB
     if (mine && (u == 10 || Rr == N - 1)) acc = ring[(r & (SW_RING - 1)) * HROW]; /* z_r */
     const double xR = __shfl_sync(0xffffffffu, acc, Rr & 15);
     if (lane == (Rr & 15)) gx[(size_t)Rr * 32] = xR;
+    ok = ok && isfinite(xR); /* every lane sees every x_R */
     if (mine && u >= 1) acc -= fr[u] * xR;
     const int rp = Rr - 1 - SW_AHEAD;
     if (rp >= 0) prefetch_row(gF, rp);
     cp_async_commit();
   }
   cp_async_wait<0>();
+  /* success: every pivot positive and finite, every component of the solution finite (the rule of every solve kernel) */
+  if (lane == 0) res[5] = ok ? 1.0 : 0.0;
 }
 
 }  // namespace tebgpu

@@ -288,9 +288,8 @@ __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int 
   __syncwarp();
   if (!work) return;
   double* res = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
-  res[5] = ok ? 1.0 : 0.0;
   res[6] = lambda;
-  if (!ok) return; /* CSparse failure: k_trial_eval uses dx = b */
+  if (!ok) { res[5] = 0.0; return; } /* CSparse failure: k_trial_eval uses dx = b */
 
   /* back substitution x_j = z_j - sum_u L[j+u][j] x_{j+u}; X[m]: x of the row with r % 11 == m.
    * The factor rows written above are read back through a per-lane cp.async ring in the staging buffers, TPB_RING rows
@@ -342,6 +341,70 @@ __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int 
     }
   }
   cp_async_wait<0>();
+  /* the solve succeeded iff every pivot was positive and finite and every component of the solution is finite: the
+   * rule of every solve kernel (a NaN in b leaves the pivots alone). Every row subtracts l_1 x_{j+1} (tpb_len >= 7), and
+   * a product with a NaN or an infinity is never finite (0 * inf is NaN), so a non-finite component reaches x_0: one
+   * test of x_0 is the test of the whole solution, off the per-row chain */
+  res[5] = isfinite(X[0]) ? 1.0 : 0.0;
+}
+
+/* ------------------------------------------------------------------ k_solve_seq: solvers 0 / 1 on one system
+ * The solve of k_lm_step_t (sequential warp LDL^T, warp_band_solve, or block cyclic reduction, bcr_solve) for one
+ * (band, trial) system per CTA, staged as k_lm_step_t stages its band and written where k_solve_tpb writes: dx in the
+ * warp-interleaved scratch, res[5] / res[6]. Only tebgpu_solve_system launches it: it lets the tests give those device
+ * functions the same systems as the speculative solver's kernels. */
+template <int SOLVER, int NT>
+__global__ void __launch_bounds__(NT) k_solve_seq(DevBatch db, SpecBufs sp, int iteration, int round, int g) {
+  extern __shared__ __align__(128) unsigned char seq_raw[];
+  const int t = blockIdx.x;
+  const int SPEC_K = sp.K;
+  const int slot = t / SPEC_K;
+  const int k = t - slot * SPEC_K;
+  const int b = spec_band(db, sp, round, g, slot);
+  if (b < 0) return;
+  const BandState* st = &db.state[b];
+  if (!st->active) return;
+  const int q0 = (round == 0) ? 0 : sp.qmax[b];
+  if (q0 + k >= 10) return;
+  const int n = db.n[b];
+  const int N = 4 * n;
+  double lambda, ni;
+  if (round == 0 && iteration == 0) { lambda = band_lambda_init(db, b, n); ni = 2; }
+  else { lambda = st->lambda; ni = st->ni; }
+  spec_lambda(lambda, ni, k);
+  const double* gH = db.Hb + (size_t)b * 4 * db.n_cap * HROW;
+  double* gx = sp.dx + (size_t)(t >> 5) * 32 * 4 * db.n_cap + (t & 31);
+  double* res = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
+  __shared__ int s_fail;
+  bool ok;
+  if constexpr (SOLVER == 0) {
+    double* Hs = reinterpret_cast<double*>(seq_raw);
+    uint64_t* bar = reinterpret_cast<uint64_t*>(Hs + (size_t)4 * db.n_cap * HROW);
+    if (threadIdx.x == 0) {
+      mbar_init(bar, 1);
+      mbar_fence_init();
+      const uint32_t bytes = (uint32_t)N * HROW * 8u;
+      mbar_expect_tx(bar, bytes);
+      tma_load_1d(Hs, gH, bytes, bar);
+    }
+    __syncwarp();
+    mbar_wait(bar, 0);
+    ok = warp_band_solve(Hs, N, n, lambda);
+    if (ok)
+      for (int r = threadIdx.x; r < N; r += NT) gx[(size_t)r * 32] = Hs[r * HROW + 11];
+  } else {
+    const int m = (N + 7) / 8;
+    double* b0;
+    const BcrSmem S = bcr_carve(reinterpret_cast<double*>(seq_raw), db.n_cap, m, b0);
+    bcr_stage<NT>(S, b0, gH, N, n, m, lambda);
+    if (threadIdx.x == 0) s_fail = 0;
+    __syncthreads();
+    bcr_solve<NT>(S, m, &s_fail);
+    ok = s_fail == 0;
+    if (ok)
+      for (int r = threadIdx.x; r < N; r += NT) gx[(size_t)r * 32] = S.xs[r];
+  }
+  if (threadIdx.x == 0) { res[5] = ok ? 1.0 : 0.0; res[6] = lambda; }
 }
 
 /* Accept / reject replay (OptimizationAlgorithmLevenberg::solve, SURVEY App. A.4), sequential over the K trials of one
