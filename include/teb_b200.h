@@ -268,6 +268,12 @@ int32_t tebgpu_set_speculation(tebgpu_ctx* ctx, int32_t k);
  *      single planning request - and k_solve_tpb above that. */
 int32_t tebgpu_set_warp_solver(tebgpu_ctx* ctx, int32_t mode);
 
+/* Form of k_solve_tpb (the thread-per-system mapping above): 0 (default) automatic by speculation width, 1 the LDL^T
+ * factor streamed through device memory and read back by the back substitution, 11 / 22 / 33 the factor not stored but
+ * recomputed from window checkpoints in segments of that many rows (k_solve_tpb_rc). Same bits in every form; only
+ * memory traffic and time differ. The environment variable TEBGPU_SOLVE_FORM sets the initial value. */
+int32_t tebgpu_set_solve_form(tebgpu_ctx* ctx, int32_t form);
+
 /* CUDA-graph replay of the launch sequence of tebgpu_optimize_batch(_device): 0 never, 1 always, 2 (default) in the
  * latency regime only (a batch of at most ~2300 bands, e.g. one planning request of 32 candidates, where the 130-170
  * kernel launches of one optimizeTEB are comparable to the kernels themselves). A sequence is captured once per distinct

@@ -68,6 +68,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_set_warp_solver.argtypes = [vp, C.c_int32]
     L.tebgpu_set_graph.restype = C.c_int32
     L.tebgpu_set_graph.argtypes = [vp, C.c_int32]
+    L.tebgpu_set_solve_form.restype = C.c_int32
+    L.tebgpu_set_solve_form.argtypes = [vp, C.c_int32]
     L.tebgpu_get_info.restype = C.c_int64
     L.tebgpu_get_info.argtypes = [vp, C.c_int32]
     L.tebgpu_set_profiling.restype = C.c_int32
@@ -145,6 +147,11 @@ class TebGpu:
     def set_warp_solver(self, mode):
         """solve kernel mapping: 0 thread per system, 1 warp per system, 2 by regime"""
         self._check(self.lib.tebgpu_set_warp_solver(self.ctx, int(mode)), "tebgpu_set_warp_solver")
+
+    def set_solve_form(self, form):
+        """k_solve_tpb's factor: 0 automatic, 1 streamed through device memory, 11 / 22 / 33 recomputed in segments of
+        that many rows"""
+        self._check(self.lib.tebgpu_set_solve_form(self.ctx, int(form)), "tebgpu_set_solve_form")
 
     def set_graph(self, mode):
         """CUDA-graph replay of the launch sequence: 0 never, 1 always, 2 automatic (latency regime)"""

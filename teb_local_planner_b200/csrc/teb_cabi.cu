@@ -61,6 +61,8 @@ struct tebgpu_ctx {
                             kept as an independently mapped, bit-identical implementation,
                           3 / 4 k_solve_lat (twisted factorisation, system resident in shared memory) always / while the
                             systems of a round fit LAT_WAVES waves of resident CTAs (the latency regime; DEFAULT) */
+  int solve_form = 0;  /* k_solve_tpb's factor (TEBGPU_SOLVE_FORM / tebgpu_set_solve_form): 0 automatic (tpb_form),
+                          1 streamed through HBM, 11 / 22 / 33 recomputed in segments of that many rows */
   int eval_v1 = 0;     /* TEBGPU_EVAL_V1=1: first-generation trial evaluation (warp per trial, chunk per lane) */
   int ka_staged = 1;   /* kernel A output: 1 (default) shared-memory slot + TMA bulk store per lane, 0 direct 128-bit global stores */
   int last_spec_k = 0; /* round-0 width of the later LM iterations of the last optimize call */
@@ -346,6 +348,12 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+#define RC_ATTR(C)                                                                                                         \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb_rc<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, tpb_rc_smem_bytes(C, 2))); \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_solve_tpb_rc<C>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  RC_ATTR(11) RC_ATTR(22) RC_ATTR(33)
+#undef RC_ATTR
+  if (const char* e = std::getenv("TEBGPU_SOLVE_FORM")) { const int m = std::atoi(e); if (m == 0 || m == 1 || m == 11 || m == 22 || m == 33) c->solve_form = m; }
   CUDA_TRY(c, cudaFuncSetAttribute(k_solve_lat, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
   if (const char* e = std::getenv("TEBGPU_LAT_TIMING")) { const int v = std::atoi(e); CUDA_TRY(c, cudaMemcpyToSymbol(g_lat_timing, &v, sizeof(int))); }
   if (const char* e = std::getenv("TEBGPU_WARP_SOLVER")) { const int m = std::atoi(e); if (m >= 0 && m <= 4) c->warp_solver = m; }
@@ -553,6 +561,18 @@ static DevBatch make_devbatch(tebgpu_ctx* ctx, const TebBatch* bt) {
   return d;
 }
 
+/* Form of k_solve_tpb: 0 the factor streamed through HBM (k_solve_tpb), else the segment length C of the recompute form
+ * (k_solve_tpb_rc<C>). Automatic: C = 22, the fastest form at every width measured (K = 2, 4, 6; DESIGN §8). The
+ * checkpoints of the recompute form must fit the factor scratch of a warp (only very short bands at C = 11 would not). */
+constexpr int TPB_RC_AUTO_C = 22;
+static int tpb_form(const tebgpu_ctx* ctx, int n_cap) {
+  int C = ctx->solve_form;
+  if (C == 0) C = TPB_RC_AUTO_C;
+  if (C == 1) return 0;
+  const long long segs = (4LL * n_cap + C - 1) / C;
+  return segs * TPB_RC_CKPT_PAIRS <= 4LL * n_cap * (HROW / 2) ? C : 0;
+}
+
 /* The solve launch of one round of the speculative solver (solver 2) over the db.B bands, K trials each, on stream s:
  * the kernel tebgpu_set_warp_solver selects, its grid and shared memory. Shared by issue_optimize and
  * tebgpu_solve_system. lat_cap > 0 (retry rounds, mode 4) forces the dual launch with that many k_solve_lat systems;
@@ -570,6 +590,16 @@ static int launch_spec_solve(const tebgpu_ctx* ctx, const DevBatch& db, const Sp
   const long long lat_wave = smem_lat <= 232448 ? (long long)ctx->sms * (232448 / smem_lat > 16 ? 16 : 232448 / smem_lat) : 0;
   const bool dual = round > 0 && ctx->warp_solver == 4 && lat_wave > 0;
   const bool lat_solver = lat_wave > 0 && (ctx->warp_solver == 3 || (ctx->warp_solver == 4 && bk <= LAT_WAVES * lat_wave && lat_cap == 0));
+  /* k_solve_tpb in the form tebgpu_set_solve_form selects: the factor streamed through HBM, or recomputed per
+   * segment of C rows (k_solve_tpb_rc) */
+  auto launch_tpb = [&](const SpecBufs& sb) {
+    switch (tpb_form(ctx, db.n_cap)) {
+      case 11: k_solve_tpb_rc<11><<<warps, 32, tpb_rc_smem_bytes(11, K), s>>>(db, sb, it, round, g); break;
+      case 22: k_solve_tpb_rc<22><<<warps, 32, tpb_rc_smem_bytes(22, K), s>>>(db, sb, it, round, g); break;
+      case 33: k_solve_tpb_rc<33><<<warps, 32, tpb_rc_smem_bytes(33, K), s>>>(db, sb, it, round, g); break;
+      default: k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, sb, it, round, g);
+    }
+  };
   if (lat_solver) k_solve_lat<<<bk, 32, smem_lat, s>>>(db, spec, it, round, g);
   else if (dual) {
     /* retry round of the throughput regime: both mappings are launched, the list length decides on the device */
@@ -578,11 +608,11 @@ static int launch_spec_solve(const tebgpu_ctx* ctx, const DevBatch& db, const Sp
     cap = cap < bk ? cap : bk;
     sl.lat_cap = (int32_t)cap;
     k_solve_lat<<<(unsigned)cap, 32, smem_lat, s>>>(db, sl, it, round, g);
-    k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, sl, it, round, g);
+    launch_tpb(sl);
     return 2;
   }
   else if (warp_solver) k_solve_warp<<<(bk + SW_WARPS - 1) / SW_WARPS, 32 * SW_WARPS, 0, s>>>(db, spec, it, round, g);
-  else k_solve_tpb<<<warps, 32, TPB_SMEM_BYTES, s>>>(db, spec, it, round, g);
+  else launch_tpb(spec);
   return 1;
 }
 
@@ -790,7 +820,7 @@ static uint64_t graph_key(const tebgpu_ctx* ctx, const TebBatch* bt, const TebOp
   mix(bt, sizeof(*bt));
   mix(a, sizeof(*a));
   mix(&ctx->params_version, sizeof(ctx->params_version));
-  const int sw[10] = {ctx->solver, ctx->spec_k, ctx->linearize_variant, ctx->ka_staged, ctx->eval_v1, ctx->overlap, ctx->eval_minb, ctx->warp_solver, ctx->eval_mode, ctx->split};
+  const int sw[11] = {ctx->solver, ctx->spec_k, ctx->linearize_variant, ctx->ka_staged, ctx->eval_v1, ctx->overlap, ctx->eval_minb, ctx->warp_solver, ctx->eval_mode, ctx->split, ctx->solve_form};
   mix(sw, sizeof(sw));
   mix(&st, sizeof(st));
   return h;
@@ -848,6 +878,12 @@ int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const 
 int32_t tebgpu_set_warp_solver(tebgpu_ctx* ctx, int32_t mode) {
   if (!ctx || mode < 0 || mode > 4) return TEBGPU_ERR_INVALID_ARG;
   ctx->warp_solver = mode;
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_set_solve_form(tebgpu_ctx* ctx, int32_t form) {
+  if (!ctx || !(form == 0 || form == 1 || form == 11 || form == 22 || form == 33)) return TEBGPU_ERR_INVALID_ARG;
+  ctx->solve_form = form;
   return TEBGPU_OK;
 }
 

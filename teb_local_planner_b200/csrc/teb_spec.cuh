@@ -11,7 +11,9 @@
  *   k_solve_tpb   one THREAD per (band, trial): banded LDL^T (half bandwidth 10) with the 11x11 active window held in
  *                 registers (fully unrolled by 11 so every index is static), rows of H staged per band in shared memory, factor
  *                 rows streamed out in the band's profile (only the columns' structurally non-zero entries),
- *                 forward substitution fused, back substitution from the streamed factor.
+ *                 forward substitution fused, back substitution from the streamed factor. The default form,
+ *                 k_solve_tpb_rc, does not store the factor: it recomputes it from window checkpoints, segment by
+ *                 segment, with bit-identical results.
  *                 Replaces LinearSolverCSparse::solve (optimal_planner.cpp:169-172).
  *   k_trial_eval  one CTA per band, one WARP per trial: trial state x [+] dx, trial chi2 by family, computeScale();
  *                 then one thread replays the accept / reject chain in order and the CTA commits the accepted trial
@@ -130,6 +132,51 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int NPEND>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(NPEND) : "memory"); }
 
+/* One pivot of the banded LDL^T on the 11-periodic register window (s = j mod 11, static once unrolled): the pivot
+ * test, the rank-1 update of rows j+1 .. j+10 and their right-hand sides, and factor row j handed to put(pair, a, b) as
+ * 16-byte pairs (z_j, L[j+1][j]), (L[j+2][j], L[j+3][j]) .. (L[j+10][j], 0). Every form of k_solve_tpb (the streamed
+ * factorisation, the recompute form's forward pass and its replay) runs this one function, so the compiler emits the
+ * same operation sequence for every window entry and the factor, z and x are the same bits in every form. */
+template <class Put>
+__device__ __forceinline__ void tpb_pivot(double (&E)[11][11], double (&Y)[11], const int s, bool& ok, Put&& put) {
+  const double d = E[0][s];
+  if (!(d > 0) || !isfinite(d)) ok = false;
+  const double inv = 1.0 / d;
+  const double yj = Y[s];
+  double cu[11];
+#pragma unroll
+  for (int u = 1; u <= 10; ++u) cu[u] = E[u][(s + u) % 11];
+  double lprev = yj * inv; /* z_j */
+#pragma unroll
+  for (int u = 1; u <= 10; ++u) {
+    const double lu = cu[u] * inv;
+#pragma unroll
+    for (int q = 1; q <= u; ++q) E[u - q][(s + u) % 11] -= lu * cu[q];
+    Y[(s + u) % 11] -= lu * yj;
+    /* pair (u - 1) / 2 complete at odd u */
+    if (u & 1) put(u / 2, lprev, lu);
+    else lprev = lu;
+    if (u == 10) put(5, lu, 0.0);
+  }
+}
+/* row rn (< N: the staged H|b row src, lambda on the diagonal of a real unknown; else an identity row) into window slot s */
+__device__ __forceinline__ void tpb_install(double (&E)[11][11], double (&Y)[11], const int s, const double2* src, int rn, int N,
+                                            int n, double lambda) {
+  if (rn < N) {
+#pragma unroll
+    for (int v = 0; v < 5; ++v) { const double2 d2 = src[v]; E[2 * v][s] = d2.x; E[2 * v + 1][s] = d2.y; }
+    const double2 d2 = src[5];
+    E[10][s] = d2.x;
+    Y[s] = d2.y;
+    if (row_is_real(rn, n)) E[0][s] += lambda;
+  } else {
+#pragma unroll
+    for (int kk = 1; kk < 11; ++kk) E[kk][s] = 0.0;
+    E[0][s] = 1.0;
+    Y[s] = 0.0;
+  }
+}
+
 __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int iteration, int round, int g) {
   extern __shared__ __align__(16) unsigned char tpb_raw[];
   const int lane = threadIdx.x;
@@ -234,51 +281,19 @@ __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int 
 #pragma unroll
     for (int s = 0; s < 11; ++s) {
       const int j = j0 + s;
-      const double d = E[0][s];
-      if (!(d > 0) || !isfinite(d)) ok = false;
-      const double inv = 1.0 / d;
-      const double yj = Y[s];
-      double cu[11];
-#pragma unroll
-      for (int u = 1; u <= 10; ++u) cu[u] = E[u][(s + u) % 11];
       const bool live = j < N;
       const int c = j & 3; /* j advances in lockstep across the warp: warp-uniform */
       double2* dst = tpb_row(gL, j); /* pair v at dst[v * 32] */
-      double lprev = yj * inv;       /* z_j */
-#pragma unroll
-      for (int u = 1; u <= 10; ++u) {
-        const double lu = cu[u] * inv;
-#pragma unroll
-        for (int q = 1; q <= u; ++q) E[u - q][(s + u) % 11] -= lu * cu[q];
-        Y[(s + u) % 11] -= lu * yj;
-        /* factor row j: z_j, L[j+1..j+tpb_len(c)][j], pair (u - 1) / 2 complete at odd u */
-        if (u & 1) {
-          if (live && u / 2 < tpb_pairs(c)) dst[(u / 2) * 32] = make_double2(lprev, lu);
-        } else {
-          lprev = lu;
-        }
-        if (u == 10 && live && c == 0) dst[5 * 32] = make_double2(lu, 0.0);
-      }
+      /* factor row j: z_j, L[j+1..j+tpb_len(c)][j] */
+      tpb_pivot(E, Y, s, ok, [&](int v, double a, double b2) {
+        if (live && v < tpb_pairs(c)) dst[v * 32] = make_double2(a, b2);
+      });
       /* install row j + 11 from the staged chunk */
-      const int rn = j + 11;
       if (pr == TPB_CHUNK) { /* warp-uniform: j advances in lockstep */
         next_chunk(++cr);
         pr = 0;
       }
-      if (rn < N) {
-        const double2* src = staged_row(cr, pr);
-#pragma unroll
-        for (int v = 0; v < 5; ++v) { const double2 d2 = src[v]; E[2 * v][s] = d2.x; E[2 * v + 1][s] = d2.y; }
-        const double2 d2 = src[5];
-        E[10][s] = d2.x;
-        Y[s] = d2.y;
-        if (row_is_real(rn, n)) E[0][s] += lambda;
-      } else {
-#pragma unroll
-        for (int kk = 1; kk < 11; ++kk) E[kk][s] = 0.0;
-        E[0][s] = 1.0;
-        Y[s] = 0.0;
-      }
+      tpb_install(E, Y, s, staged_row(cr, pr), j + 11, N, n, lambda);
       ++pr;
     }
   }
@@ -346,6 +361,255 @@ __global__ void __launch_bounds__(32) k_solve_tpb(DevBatch db, SpecBufs sp, int 
    * a product with a NaN or an infinity is never finite (0 * inf is NaN), so a non-finite component reaches x_0: one
    * test of x_0 is the test of the whole solution, off the per-row chain */
   res[5] = isfinite(X[0]) ? 1.0 : 0.0;
+}
+
+/* ------------------------------------------------------------------ k_solve_tpb_rc: k_solve_tpb without the factor in HBM
+ * k_solve_tpb moves each factor row to HBM and back (160 of its 192-216 bytes per system and row). This form does not
+ * store the factor; it recomputes it, segment by segment, C rows at a time (C a multiple of 11, so that a segment starts
+ * where the register window's slot indices are static):
+ *   forward pass   the pivot loop of k_solve_tpb without factor stores. At every segment start j0 each lane saves the
+ *                  window's live state: row j0 + t keeps E[0..t][t] (66 entries), and the 11 Y: 77 doubles, 39 pairs
+ *                  [segment][pair][lane] in sp.Lf (616 bytes per segment instead of C factor rows).
+ *   back pass      segments from the top: restore the checkpoint, restage the segment's H|b rows (j0 + 11 .. j0 + C + 10),
+ *                  replay the same pivot steps (tpb_pivot), which now put the factor rows into a per-lane segment buffer in
+ *                  shared memory ([pair][lane], the profile layout of k_solve_tpb), then back-substitute the segment from
+ *                  there; the x ring carries over to the next segment down. The next segment's checkpoint loads are issued
+ *                  before this segment's back substitution, which does not need the window's registers.
+ * Staging: chunks of 11 rows (one window block's installs), 1072 bytes per band and buffer (67 x 16: odd), double-buffered
+ * through the whole kernel; the bands per buffer follow K (16 at K = 2, 8 at K = 4, at most 7 at K = 6). Identity rows,
+ * the warp-wide loop to the largest N and the failure rule are those of k_solve_tpb: same bits in every output. */
+constexpr int TPB_RC_CHUNK = 11;
+constexpr int TPB_RC_STRIDE = TPB_RC_CHUNK * HROW * 8 + 16;
+constexpr int TPB_RC_CKPT_PAIRS = 39; /* 66 window entries + 11 right-hand sides + 1 pad */
+static_assert((TPB_RC_STRIDE / 16) % 2 == 1, "staging stride: odd number of 16-byte units");
+/* pair index of factor row j in the profile layout (tpb_row without the lane interleave) */
+__host__ __device__ constexpr int tpb_pair_index(int j) { return (j >> 2) * TPB_GROUP_PAIRS + tpb_pair_off(j & 3); }
+/* pairs of C consecutive factor rows, the worst start j0 mod 4 */
+__host__ __device__ constexpr int tpb_rc_seg_pairs(int C) {
+  int m = 0;
+  for (int r = 0; r < 4; ++r) m = (tpb_pair_index(r + C) - tpb_pair_index(r) > m) ? tpb_pair_index(r + C) - tpb_pair_index(r) : m;
+  return m;
+}
+/* bands a warp's 32 lanes can touch at width K (K even) */
+__host__ __device__ constexpr int tpb_rc_bands(int K) { return (31 + K) / K + (32 % K != 0); }
+/* x parked between the segments: the top row j0 + C - 1 of a segment reads x_{j0+C} .. x_{j0+C+9} (tpb_len <= 10) */
+constexpr int TPB_RC_XPARK = 10;
+/* [2 mbarriers + pad: 16][segment buffer][x park][staging: 2 buffers x bands x stride] */
+__host__ __device__ constexpr int tpb_rc_smem_bytes(int C, int K) {
+  return 16 + tpb_rc_seg_pairs(C) * 32 * 16 + TPB_RC_XPARK * 32 * 8 + 2 * tpb_rc_bands(K) * TPB_RC_STRIDE;
+}
+
+template <int C>
+__global__ void __launch_bounds__(32) k_solve_tpb_rc(DevBatch db, SpecBufs sp, int iteration, int round, int g) {
+  static_assert(C % 11 == 0 && C >= 11, "segments start on the window period");
+  extern __shared__ __align__(16) unsigned char rc_raw[];
+  const int lane = threadIdx.x;
+  const int t = blockIdx.x * 32 + lane;
+  const int SPEC_K = sp.K;
+  const int slot = t / SPEC_K;
+  const int k = t - slot * SPEC_K;
+  if (retry_round_takes_lat(sp, round, g)) return; /* the whole grid: k_solve_lat does this round */
+  const int b = spec_band(db, sp, round, g, slot);
+  /* lanes without a system stay in both passes as empty systems (identity rows only): the warp stages together */
+  bool work = b >= 0;
+  if (work && !db.state[b].active) work = false;
+  const int q0 = (!work || round == 0) ? 0 : sp.qmax[b];
+  if (q0 + k >= 10) work = false;
+  const int n = work ? db.n[b] : 0;
+  const int N = 4 * n;
+  const int Nw = (int)__reduce_max_sync(0xffffffffu, (unsigned)N);
+  if (Nw == 0) return;
+  double lambda = 0, ni = 2;
+  if (work) {
+    const BandState* st = &db.state[b];
+    if (round == 0 && iteration == 0) { lambda = band_lambda_init(db, b, n); ni = 2; }
+    else { lambda = st->lambda; ni = st->ni; }
+    spec_lambda(lambda, ni, k);
+  }
+  double2* gC = reinterpret_cast<double2*>(sp.Lf + (size_t)blockIdx.x * 32 * 4 * db.n_cap * HROW) + lane;
+  double* gx = sp.dx + (size_t)blockIdx.x * 32 * 4 * db.n_cap + lane;
+
+  uint64_t* bar = reinterpret_cast<uint64_t*>(rc_raw);
+  double2* segbuf = reinterpret_cast<double2*>(rc_raw + 16) + lane; /* pair p of the segment at segbuf[p * 32] */
+  double* xpark = reinterpret_cast<double*>(rc_raw + 16 + tpb_rc_seg_pairs(C) * 32 * 16) + lane; /* [m][lane] */
+  unsigned char* stage = rc_raw + 16 + tpb_rc_seg_pairs(C) * 32 * 16 + TPB_RC_XPARK * 32 * 8;
+  const int nb = tpb_rc_bands(SPEC_K);
+  const int slot0 = (blockIdx.x * 32) / SPEC_K;
+  const bool stager = work && (k == 0 || lane == 0);
+  const double* gH = db.Hb + (size_t)(work ? b : 0) * 4 * db.n_cap * HROW;
+  unsigned char* stage_band = stage + (slot - slot0) * TPB_RC_STRIDE;
+  /* chunk ci = rows 11 ci .. 11 ci + 10; the qi-th chunk issued goes to buffer qi & 1, the chunks are consumed in the
+   * order they were issued */
+  int qi = 0, qw = 0;
+  auto issue = [&](int ci) {
+    const int r0 = ci * TPB_RC_CHUNK;
+    const uint32_t bytes = stager && r0 < N ? (uint32_t)(min(TPB_RC_CHUNK, N - r0) * HROW * 8) : 0u;
+    const uint32_t total = __reduce_add_sync(0xffffffffu, bytes);
+    if (lane == 0) mbar_expect_tx(bar + (qi & 1), total);
+    __syncwarp();
+    if (bytes) tma_load_1d(stage_band + (qi & 1) * nb * TPB_RC_STRIDE, gH + (size_t)r0 * HROW, bytes, bar + (qi & 1));
+    ++qi;
+  };
+  auto wait_next = [&]() {
+    mbar_wait(bar + (qw & 1), (uint32_t)(qw >> 1) & 1u);
+    const double2* p = reinterpret_cast<const double2*>(stage_band + (qw & 1) * nb * TPB_RC_STRIDE);
+    ++qw;
+    return p;
+  };
+  /* every lane has read the buffer consumed last (the fence orders those reads before the next bulk copy's writes) */
+  auto release = [&]() {
+    fence_proxy_async();
+    __syncwarp();
+  };
+  if (lane == 0) {
+    mbar_init(bar, 1);
+    mbar_init(bar + 1, 1);
+    mbar_fence_init();
+  }
+  __syncwarp();
+  issue(0);
+  issue(1);
+
+  double E[11][11], Y[11];
+  {
+    const double2* src = wait_next(); /* rows 0 .. 10 */
+#pragma unroll
+    for (int m = 0; m < 11; ++m) {
+      double h[12];
+      if (m < N) {
+#pragma unroll
+        for (int v = 0; v < 6; ++v) { const double2 d2 = src[m * 6 + v]; h[2 * v] = d2.x; h[2 * v + 1] = d2.y; }
+        if (row_is_real(m, n)) h[0] += lambda;
+      } else {
+#pragma unroll
+        for (int v = 0; v < 12; ++v) h[v] = 0.0;
+        h[0] = 1.0;
+      }
+#pragma unroll
+      for (int kk = 0; kk < 11; ++kk) E[kk][m] = (kk <= m) ? h[kk] : 0.0;
+      Y[m] = h[11];
+    }
+  }
+  release();
+  issue(2);
+  bool ok = true;
+  /* ---- forward pass: pivots only, a checkpoint at every segment start */
+  for (int j0 = 0; j0 < Nw; j0 += 11) {
+    if (j0 % C == 0) {
+      double ck[2 * TPB_RC_CKPT_PAIRS];
+      int e = 0;
+#pragma unroll
+      for (int tt = 0; tt < 11; ++tt)
+#pragma unroll
+        for (int kk = 0; kk <= tt; ++kk) ck[e++] = E[kk][tt];
+#pragma unroll
+      for (int tt = 0; tt < 11; ++tt) ck[e++] = Y[tt];
+      ck[e] = 0.0;
+      double2* dst = gC + (size_t)(j0 / C) * TPB_RC_CKPT_PAIRS * 32;
+#pragma unroll
+      for (int p = 0; p < TPB_RC_CKPT_PAIRS; ++p) dst[p * 32] = make_double2(ck[2 * p], ck[2 * p + 1]);
+    }
+    const double2* src = wait_next(); /* rows j0 + 11 .. j0 + 21 */
+#pragma unroll
+    for (int s = 0; s < 11; ++s) {
+      tpb_pivot(E, Y, s, ok, [](int, double, double) {});
+      tpb_install(E, Y, s, src + s * 6, j0 + s + 11, N, n, lambda);
+    }
+    release();
+    issue(j0 / 11 + 3);
+  }
+  while (qw < qi) wait_next(); /* the last two chunks issued hold no rows below any N: then every buffer is idle */
+  release();
+  if (work) {
+    double* res = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
+    res[6] = lambda;
+    if (!ok) res[5] = 0.0; /* CSparse failure: k_trial_eval uses dx = b; the lane stays for the warp's staging */
+  }
+  const bool store = work && ok;
+
+  /* ---- back pass, segment by segment from the top. Producer cursor over the blocks of the pass: segment ps, block pj;
+   * it stays two chunks ahead of the block being replayed, across segment boundaries */
+  const int nseg = (Nw + C - 1) / C;
+  int ps = nseg - 1, pj = ps * C;
+  auto produce = [&]() {
+    if (ps < 0) return;
+    issue(pj / 11 + 1);
+    pj += 11;
+    if (pj >= min(ps * C + C, Nw)) { --ps; pj = ps * C; }
+  };
+  auto restore = [&](int seg) {
+    const double2* srcc = gC + (size_t)seg * TPB_RC_CKPT_PAIRS * 32;
+    double ck[2 * TPB_RC_CKPT_PAIRS];
+#pragma unroll
+    for (int p = 0; p < TPB_RC_CKPT_PAIRS; ++p) { const double2 d2 = srcc[p * 32]; ck[2 * p] = d2.x; ck[2 * p + 1] = d2.y; }
+    int e = 0;
+#pragma unroll
+    for (int tt = 0; tt < 11; ++tt)
+#pragma unroll
+      for (int kk = 0; kk < 11; ++kk) E[kk][tt] = kk <= tt ? ck[e++] : 0.0;
+#pragma unroll
+    for (int tt = 0; tt < 11; ++tt) Y[tt] = ck[e++];
+  };
+  produce();
+  produce();
+  /* x of the rows above the segment, parked in shared memory during the replay (in registers it would push the kernel
+   * past 255 registers); above the top: 0 */
+#pragma unroll
+  for (int m = 0; m < TPB_RC_XPARK; ++m) xpark[m * 32] = 0.0;
+  restore(nseg - 1);
+  for (int seg = nseg - 1; seg >= 0; --seg) {
+    const int j0 = seg * C, j1 = min(j0 + C, Nw);
+    const int p0 = tpb_pair_index(j0);
+    bool ok2 = true;
+    int jb = j0;
+    for (; jb < j1; jb += 11) {
+      const double2* src = wait_next();
+#pragma unroll
+      for (int s = 0; s < 11; ++s) {
+        const int j = jb + s;
+        const int c = j & 3;
+        double2* dst = segbuf + (tpb_pair_index(j) - p0) * 32;
+        tpb_pivot(E, Y, s, ok2, [&](int v, double a, double b2) {
+          if (v < tpb_pairs(c)) dst[v * 32] = make_double2(a, b2);
+        });
+        tpb_install(E, Y, s, src + s * 6, j + 11, N, n, lambda);
+      }
+      release();
+      produce();
+    }
+    if (seg > 0) restore(seg - 1);
+    double X[11]; /* x of the row r with r % 11 == m; slot 10 (row j0 + C + 10) is written before it is read */
+#pragma unroll
+    for (int m = 0; m < 11; ++m) X[m] = m < TPB_RC_XPARK ? xpark[m * 32] : 0.0;
+    /* back substitution x_j = z_j - sum_u L[j+u][j] x_{j+u}, rows jb - 1 .. j0 */
+    for (jb -= 11; jb >= j0; jb -= 11) {
+#pragma unroll
+      for (int s = 10; s >= 0; --s) {
+        const int j = jb + s;
+        const bool live = j < N;
+        const int c = j & 3;
+        const double2* lsrc = segbuf + (tpb_pair_index(j) - p0) * 32;
+        double l[12];
+#pragma unroll
+        for (int v = 0; v < 6; ++v) {
+          double2 d2 = make_double2(0.0, 0.0);
+          if (live && v < tpb_pairs(c)) d2 = lsrc[v * 32];
+          l[2 * v] = d2.x;
+          l[2 * v + 1] = d2.y;
+        }
+        double acc = l[0];
+#pragma unroll
+        for (int u = 10; u >= 1; --u)
+          if (u <= tpb_len(c)) acc -= l[u] * X[(s + u) % 11];
+        X[s] = acc;
+        if (live && store) gx[(size_t)j * 32] = acc;
+      }
+    }
+#pragma unroll
+    for (int m = 0; m < TPB_RC_XPARK; ++m) xpark[m * 32] = X[m];
+  }
+  /* every chunk issued was consumed: no bulk copy is in flight. x_0 is in the park's slot 0 */
+  if (store) sp.res[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + 5] = isfinite(xpark[0]) ? 1.0 : 0.0;
 }
 
 /* ------------------------------------------------------------------ k_solve_seq: solvers 0 / 1 on one system
