@@ -204,7 +204,11 @@ typedef struct TebGpuLimits {
   int32_t max_bands;      /* B capacity */
   int32_t max_poses;      /* n_cap capacity (<= 512) */
   int32_t max_scenes;
-  int32_t max_obstacles;  /* M_cap capacity (<= 1024: 16 association words per pose; the scene's table is staged in shared memory) */
+  int32_t max_obstacles;  /* M_cap capacity, <= 16384. Batches of M_cap <= 1024 stage the scene's table in shared memory;
+                             1025 .. 16384 read it from global memory (L2), chosen per call. The association buffers
+                             take B x n_cap x (2 MW + ceil(MW / 64)) x 8 bytes of device memory, MW = ceil(max_obstacles / 64)
+                             (16384 obstacles: 4.1 KB per pose). Beyond 1024 obstacles solvers 0 / 1, kernel-A variant 1,
+                             TEBGPU_EVAL_V1 and tebgpu_h_signature return TEBGPU_ERR_UNSUPPORTED. */
   int32_t max_viapoints;  /* V_cap capacity */
   int32_t max_obst_vertices; /* PV_cap capacity (0: Point / Circular obstacles only) */
 } TebGpuLimits;

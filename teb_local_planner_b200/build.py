@@ -38,6 +38,7 @@ def build(force=False, verbose=False):
 HOST_DIR = os.path.join(HERE, "host")
 HOST_LIB = os.path.join(HERE, "libteb_local_planner_b200.so")
 HOST_TEST = os.path.join(HOST_DIR, "test", "test_dropin")
+HOST_TEST_LARGE = os.path.join(HOST_DIR, "test", "test_dropin_large")  # the drop-in classes on a 3000-obstacle scene
 HOST_PIN = os.path.join(HOST_DIR, "test", "libteb_host_pin.so")   # test infrastructure: band operations for tests/test_host_pin.py
 HOST_SRCS = [os.path.join(HOST_DIR, "src", f) for f in ("timed_elastic_band.cpp", "optimal_planner.cpp",
                                                          "homotopy_class_planner.cpp", "graph_search.cpp")]
@@ -47,8 +48,9 @@ def build_host(force=False, verbose=False):
     """Drop-in C++ classes (TebOptimalPlanner, HomotopyClassPlanner, TimedElasticBand ...) over the C-ABI + their test."""
     inc = ["-I", os.path.join(os.path.dirname(HERE), "include"), "-I", os.path.join(HOST_DIR, "include")]
     hdrs = [os.path.join(dp, f) for dp, _, fs in os.walk(os.path.join(HOST_DIR, "include")) for f in fs]
-    deps = HOST_SRCS + hdrs + [os.path.join(HOST_DIR, "test", "test_dropin.cpp"), os.path.join(HOST_DIR, "test", "pin_api.cpp"), LIB]
-    outs = (HOST_LIB, HOST_TEST, HOST_PIN)
+    deps = HOST_SRCS + hdrs + [os.path.join(HOST_DIR, "test", "test_dropin.cpp"), os.path.join(HOST_DIR, "test", "pin_api.cpp"),
+                                  os.path.join(HOST_DIR, "test", "test_dropin_large.cpp"), LIB]
+    outs = (HOST_LIB, HOST_TEST, HOST_PIN, HOST_TEST_LARGE)
     if (not force and all(os.path.exists(o) for o in outs)
             and all(os.path.getmtime(d) <= min(os.path.getmtime(o) for o in outs) for d in deps)):
         return HOST_LIB
@@ -61,6 +63,8 @@ def build_host(force=False, verbose=False):
             common + ["-I", "/usr/local/cuda/include", "-o", HOST_TEST, os.path.join(HOST_DIR, "test", "test_dropin.cpp"), "-L", HERE,
                       "-lteb_local_planner_b200", "-lteb_b200", "-L", "/usr/local/cuda/lib64", "-lcudart",
                       "-Wl,-rpath," + HERE, "-Wl,-rpath,/usr/local/cuda/lib64"],
+            common + ["-o", HOST_TEST_LARGE, os.path.join(HOST_DIR, "test", "test_dropin_large.cpp"), "-L", HERE,
+                      "-lteb_local_planner_b200", "-lteb_b200", "-Wl,-rpath," + HERE],
             common + ["-shared", "-o", HOST_PIN, os.path.join(HOST_DIR, "test", "pin_api.cpp"), "-L", HERE,
                       "-lteb_local_planner_b200", "-lteb_b200", "-Wl,-rpath," + HERE]]
     for cmd in cmds:

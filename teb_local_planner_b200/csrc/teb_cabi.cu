@@ -37,7 +37,7 @@ struct tebgpu_ctx {
   int32_t* defer = nullptr;           /* [B] */
   double* d_fp = nullptr;             /* footprint definition for the vertex-list distance path (FP_DOUBLES) */
   double* d_pverts = nullptr;         /* [S][max_obst_vertices][2] mirror of TebBatch.obst_vertices */
-  double* d_hsig = nullptr;           /* [max_bands][max(max_obstacles, 2)] H-signature output of the host-buffer entry point */
+  double* d_hsig = nullptr;           /* [max_bands][max(min(max_obstacles, 1024), 2)] H-signature output of the host-buffer entry point */
   TebGpuLimits lim{};
   TebParams params{};
   bool have_params = false;
@@ -75,6 +75,7 @@ struct tebgpu_ctx {
   double* Hb = nullptr;
   unsigned long long* assoc = nullptr;
   unsigned long long* assoc3 = nullptr;
+  unsigned long long* occ = nullptr;  /* [max_bands][max_poses][ceil(MW / 64)] occupancy words (global-table path) */
   double* dyn_t = nullptr;
   int32_t* via_idx = nullptr;
   double* chi_parts = nullptr;
@@ -201,7 +202,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
 }
 
 static void free_all(tebgpu_ctx* c) {
-  void* ptrs[] = {c->Lf2, c->dx2, c->arrive, c->d_gather, c->d_hsig, c->assoc3, c->dyn_idx, c->dyn_cnt, c->rhs, c->dmax_parts, c->spec.Lf, c->spec.dx, c->spec.res, c->spec.need, c->spec.qmax, c->spec.cnt, c->spec.list, c->defer, c->d_fp, c->d_pverts, c->Hb, c->assoc, c->dyn_t, c->via_idx, c->chi_parts, c->state, c->d_poses, c->d_n, c->d_scene,
+  void* ptrs[] = {c->Lf2, c->dx2, c->arrive, c->d_gather, c->d_hsig, c->assoc3, c->occ, c->dyn_idx, c->dyn_cnt, c->rhs, c->dmax_parts, c->spec.Lf, c->spec.dx, c->spec.res, c->spec.need, c->spec.qmax, c->spec.cnt, c->spec.list, c->defer, c->d_fp, c->d_pverts, c->Hb, c->assoc, c->dyn_t, c->via_idx, c->chi_parts, c->state, c->d_poses, c->d_n, c->d_scene,
                   c->d_obst, c->d_ocount, c->d_via, c->d_vcount, c->d_vs, c->d_vg, c->d_rot, c->d_cost, c->d_chi2,
                   c->d_status, c->d_iters};
   for (void* p : ptrs)
@@ -217,7 +218,7 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
     return TEBGPU_ERR_NO_DEVICE;
   }
   if (lim->max_bands < 1 || lim->max_poses < 3 || lim->max_poses > 512 || lim->max_scenes < 1 || lim->max_obstacles < 0 ||
-      lim->max_obstacles > 64 * MAX_MW || lim->max_viapoints < 0 || lim->max_obst_vertices < 0)
+      lim->max_obstacles > 64 * GT_MAX_MW || lim->max_viapoints < 0 || lim->max_obst_vertices < 0)
     return TEBGPU_ERR_INVALID_ARG;
   tebgpu_ctx* c = new (std::nothrow) tebgpu_ctx();
   if (!c) return TEBGPU_ERR_CUDA;
@@ -242,9 +243,13 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   if (const char* e = std::getenv("TEBGPU_SPEC_K")) { const int k = std::atoi(e); if (k == 2 || k == 4 || k == 6 || k == 8) c->spec_k = k; }
   const size_t B = c->lim.max_bands, nc = c->lim.max_poses, S = c->lim.max_scenes, M = c->lim.max_obstacles,
                V = c->lim.max_viapoints > 0 ? c->lim.max_viapoints : 1;
+  /* the staged kernels (whole table in shared memory) only ever see batches of M_cap <= 1024: larger batches take the
+   * global-table instantiations, whose shared memory does not depend on M_cap */
+  const size_t Ms = M < (size_t)STAGED_MAX_OBST ? M : (size_t)STAGED_MAX_OBST;
   CUDA_TRY(c, cudaMalloc(&c->Hb, B * 4 * nc * HROW * sizeof(double)));
   CUDA_TRY(c, cudaMalloc(&c->assoc, B * nc * c->MW * sizeof(unsigned long long)));
   CUDA_TRY(c, cudaMalloc(&c->assoc3, B * nc * c->MW * sizeof(unsigned long long)));
+  CUDA_TRY(c, cudaMalloc(&c->occ, B * nc * ((c->MW + 63) / 64) * sizeof(unsigned long long)));
   CUDA_TRY(c, cudaMalloc(&c->dyn_t, B * nc * sizeof(double)));
   CUDA_TRY(c, cudaMalloc(&c->via_idx, B * V * sizeof(int32_t)));
   CUDA_TRY(c, cudaMalloc(&c->chi_parts, B * c->chunks * 4 * sizeof(double)));
@@ -254,7 +259,7 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaMalloc(&c->dyn_idx, S * M * sizeof(int32_t)));
   CUDA_TRY(c, cudaMalloc(&c->dyn_cnt, S * sizeof(int32_t)));
   {
-    size_t ev = eval_smem_bytes((int)nc, (int)M, SPEC_K_MAX);
+    size_t ev = eval_smem_bytes((int)nc, (int)Ms, SPEC_K_MAX);
     if (ev > 232448) ev = 232448; /* wide speculation is only chosen when its staging fits (tebgpu_optimize_batch_device) */
     CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev));
     CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev));
@@ -262,17 +267,28 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
     if (const char* e = std::getenv("TEBGPU_EVAL3")) { const int m = std::atoi(e); if (m >= 0 && m <= 2) c->eval_mode = m; }
     if (const char* e = std::getenv("TEBGPU_EVAL_MINB")) c->eval_minb = std::atoi(e) == 3 ? 3 : 2;
     if (const char* e = std::getenv("TEBGPU_EVAL_V1")) c->eval_v1 = std::atoi(e) != 0;
-    size_t ev2 = eval2_smem_bytes((int)nc, (int)M, SPEC_K_MAX);
+    size_t ev2 = eval2_smem_bytes((int)nc, (int)Ms, SPEC_K_MAX);
     if (ev2 > 232448) ev2 = 232448;
 #define EV2_ATTR(G, T)                                                                                                  \
   CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev2));          \
   CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     EV2_ATTR(false, 256) EV2_ATTR(true, 256) EV2_ATTR(false, 512) EV2_ATTR(true, 512)
+    size_t ev2g = eval2_smem_bytes((int)nc, 0, SPEC_K_MAX);
+    if (ev2g > 232448) ev2g = 232448;
+#define EV2G_ATTR(G, T)                                                                                                 \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev2g));   \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    EV2G_ATTR(false, 256) EV2G_ATTR(true, 256) EV2G_ATTR(false, 512) EV2G_ATTR(true, 512)
+#undef EV2G_ATTR
 #undef EV2_ATTR
-    size_t ev3 = eval3_smem_bytes((int)nc, (int)M, SPEC_K_MAX);
+    size_t ev3 = eval3_smem_bytes((int)nc, (int)Ms, SPEC_K_MAX);
     if (ev3 > 232448) ev3 = 232448;
     CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev3));
     CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev3));
+    size_t ev3g = eval3_smem_bytes((int)nc, 0, SPEC_K_MAX);
+    if (ev3g > 232448) ev3g = 232448;
+    CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval3<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev3g));
+    CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval3<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev3g));
   }
   const size_t spec_sys = ((B * SPEC_K_MAX + 31) / 32) * 32; /* whole warps of (band, trial) systems */
   CUDA_TRY(c, cudaMalloc(&c->spec.Lf, spec_sys * 4 * nc * HROW * sizeof(double)));
@@ -298,7 +314,7 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaMalloc(&c->d_fp, FP_DOUBLES * sizeof(double)));
   CUDA_TRY(c, cudaMemset(c->d_fp, 0, FP_DOUBLES * sizeof(double)));
   CUDA_TRY(c, cudaMalloc(&c->d_pverts, (S * (size_t)(lim->max_obst_vertices > 0 ? lim->max_obst_vertices : 1)) * 2 * sizeof(double)));
-  CUDA_TRY(c, cudaMalloc(&c->d_hsig, B * (M > 2 ? M : 2) * sizeof(double)));
+  CUDA_TRY(c, cudaMalloc(&c->d_hsig, B * (Ms > 2 ? Ms : 2) * sizeof(double))); /* tebgpu_h_signature: M_cap <= 1024 */
   CUDA_TRY(c, cudaMalloc(&c->d_vcount, B * sizeof(int32_t)));
   CUDA_TRY(c, cudaMalloc(&c->d_vs, B * 4 * sizeof(double)));
   CUDA_TRY(c, cudaMalloc(&c->d_vg, B * 4 * sizeof(double)));
@@ -309,36 +325,58 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaMalloc(&c->d_iters, B * sizeof(int32_t)));
   CUDA_TRY(c, cudaMemsetAsync(c->dyn_t, 0, B * nc * sizeof(double), c->stream));
   CUDA_TRY(c, cudaMemsetAsync(c->via_idx, 0xff, B * V * sizeof(int32_t), c->stream));
-  c->smem_a = ka_smem_bytes((int)M);
-  c->smem_b = kb_smem_bytes((int)nc, (int)M);
-  c->smem_g = M * sizeof(TebObstacle);
+  c->smem_a = ka_smem_bytes((int)Ms);
+  c->smem_b = kb_smem_bytes((int)nc, (int)Ms);
+  c->smem_g = Ms * sizeof(TebObstacle);
   if (c->smem_b > 232448 || c->smem_a > 232448) {
-    c->err = "shared-memory footprint exceeds 227 KB for these limits (max_poses / max_obstacles too large)";
-    return TEBGPU_ERR_CAPACITY;
+    if (M <= (size_t)STAGED_MAX_OBST) {
+      c->err = "shared-memory footprint exceeds 227 KB for these limits (max_poses / max_obstacles too large)";
+      return TEBGPU_ERR_CAPACITY;
+    }
+    /* a large-scene context: the default path never needs these; solvers 0 / 1 and kernel-A variant 1 take only the
+     * staged batches that fit (check_path) */
+    auto cap = [c](size_t& bytes, const void* f) -> int32_t { /* what is left beside the static shared memory */
+      cudaFuncAttributes fa{};
+      CUDA_TRY(c, cudaFuncGetAttributes(&fa, f));
+      if (bytes > 232448 - fa.sharedSizeBytes) bytes = 232448 - fa.sharedSizeBytes;
+      return TEBGPU_OK;
+    };
+    const void* ka[] = {(const void*)k_linearize<false, false>, (const void*)k_linearize<false, true>,
+                        (const void*)k_linearize<true, false>, (const void*)k_linearize<true, true>};
+    const void* kb[] = {(const void*)k_lm_step_t<0, KB_THREADS, false>, (const void*)k_lm_step_t<0, KB_THREADS, true>};
+    for (const void* f : ka)
+      if (int32_t rc = cap(c->smem_a, f)) return rc;
+    for (const void* f : kb)
+      if (int32_t rc = cap(c->smem_b, f)) return rc;
   }
-  if (ka2_smem_bytes<true>((int)M) > 232448) {
+  if (ka2_smem_bytes<true>((int)Ms) > 232448) {
     c->err = "kernel A staging exceeds 227 KB for these limits (max_obstacles too large)";
     return TEBGPU_ERR_CAPACITY;
   }
 #define KA2_ATTR(H, G, O)                                                                                                    \
-  CUDA_TRY(c, cudaFuncSetAttribute(k_linearize2<H, G, O>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ka2_smem_bytes<H>((int)M))); \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_linearize2<H, G, O>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ka2_smem_bytes<H>((int)Ms))); \
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize2<H, G, O>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   KA2_ATTR(false, false, true) KA2_ATTR(false, true, true) KA2_ATTR(true, false, true) KA2_ATTR(true, true, true)
   KA2_ATTR(false, false, false) KA2_ATTR(false, true, false) KA2_ATTR(true, false, false) KA2_ATTR(true, true, false)
 #undef KA2_ATTR
+#define KA2G_ATTR(H, G)                                                                                                      \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_linearize2<H, G, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ka2_smem_bytes<H>(0))); \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_linearize2<H, G, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  KA2G_ATTR(false, false) KA2G_ATTR(false, true) KA2G_ATTR(true, false) KA2G_ATTR(true, true)
+#undef KA2G_ATTR
   c->ka_staged = 1; /* TMA bulk store per lane: direct 128-bit stores fill only half of each 32-byte sector */
-  if (const char* e = std::getenv("TEBGPU_KA_STAGED")) c->ka_staged = std::atoi(e) != 0;
+  if (const char* e = std::getenv("TEBGPU_KA_STAGED")) c->ka_staged = std::atoi(e) != 0; /* staged path (M_cap <= 1024) only */
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_a));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_a));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_a));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_a));
   CUDA_TRY(c, cudaFuncSetAttribute(k_lm_step_t<0, KB_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_b));
   CUDA_TRY(c, cudaFuncSetAttribute(k_lm_step_t<0, KB_THREADS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_b));
-  if ((int)nc <= BCR_MAX_POSES && kb_bcr_smem_bytes((int)nc, (int)M) <= 232448) {
+  if ((int)nc <= BCR_MAX_POSES && kb_bcr_smem_bytes((int)nc, (int)Ms) <= 232448) {
     CUDA_TRY(c, cudaFuncSetAttribute(k_lm_step_t<1, KB_BCR_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)kb_bcr_smem_bytes((int)nc, (int)M)));
+                                     (int)kb_bcr_smem_bytes((int)nc, (int)Ms)));
     CUDA_TRY(c, cudaFuncSetAttribute(k_lm_step_t<1, KB_BCR_THREADS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)kb_bcr_smem_bytes((int)nc, (int)M)));
+                                     (int)kb_bcr_smem_bytes((int)nc, (int)Ms)));
   }
   CUDA_TRY(c, cudaFuncSetAttribute(k_build_graph<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_g));
   CUDA_TRY(c, cudaFuncSetAttribute(k_build_graph<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_g));
@@ -418,10 +456,40 @@ int32_t tebgpu_set_params(tebgpu_ctx* ctx, const TebParams* p) {
 /* Kernel instantiations: HOLO = holonomic rows (vy, acc y); GEOM = vertex-list shapes (Line / Polygon footprint,
  * Line / Pill / Polygon obstacles) reachable, i.e. the out-of-line generic_distance call is compiled in. The default
  * diff-drive / car-like + Point / Circular configuration runs <false, false>: no extra rows, no call. */
+/* Path of a batch: M_cap <= 1024 runs the staged kernels (the scene's obstacle table copied into shared memory),
+ * 1025 .. 16384 their global-table instantiations (GT: rows read from global memory / L2, association walked via the
+ * occupancy words). Chosen per call; the CUDA-graph key holds M_cap, so it covers the path. */
+static bool global_table(int M_cap) { return M_cap > STAGED_MAX_OBST; }
+
+/* the kernels without a global-table instantiation: TEBGPU_ERR_UNSUPPORTED for such a batch */
+static int32_t check_path(tebgpu_ctx* ctx, const TebBatch* bt, bool solves) {
+  if (!global_table(bt->M_cap)) {
+    /* staged batch in a large-scene context whose staged shared-memory attributes had to be capped */
+    if ((ctx->linearize_variant == 1 && ka_smem_bytes(bt->M_cap) > ctx->smem_a) ||
+        (solves && ctx->solver != 2 && kb_smem_bytes(bt->n_cap, bt->M_cap) > ctx->smem_b)) {
+      ctx->err = "shared-memory footprint exceeds 227 KB for this batch (n_cap / M_cap too large)";
+      return TEBGPU_ERR_CAPACITY;
+    }
+    return TEBGPU_OK;
+  }
+  if (ctx->linearize_variant == 1) { ctx->err = "kernel-A variant 1 supports at most 1024 obstacles per scene"; return TEBGPU_ERR_UNSUPPORTED; }
+  if (solves && ctx->solver != 2) { ctx->err = "solvers 0 and 1 support at most 1024 obstacles per scene"; return TEBGPU_ERR_UNSUPPORTED; }
+  if (solves && ctx->eval_v1) { ctx->err = "TEBGPU_EVAL_V1 supports at most 1024 obstacles per scene"; return TEBGPU_ERR_UNSUPPORTED; }
+  return TEBGPU_OK;
+}
+
 static void launch_linearize(tebgpu_ctx* ctx, const DevBatch& db, const KParams& kp, int B, int M_cap, cudaStream_t st) {
   const bool holo = kp.holo_vel || kp.holo_acc;
   const bool geom = kp.generic != 0;
-  if (ctx->linearize_variant == 1) {
+  if (global_table(M_cap)) { /* output through the staged slot, the default form: TEBGPU_KA_STAGED=0 (direct stores,
+                                same results) applies to the staged path only */
+    const dim3 g2((db.chunks + KA2_W - 1) / KA2_W, B);
+    const size_t sm = holo ? ka2_smem_bytes<true>(0) : ka2_smem_bytes<false>(0);
+    if (holo && geom) k_linearize2<true, true, false, true><<<g2, KA2_THREADS, sm, st>>>(db, kp);
+    else if (holo) k_linearize2<true, false, false, true><<<g2, KA2_THREADS, sm, st>>>(db, kp);
+    else if (geom) k_linearize2<false, true, false, true><<<g2, KA2_THREADS, sm, st>>>(db, kp);
+    else k_linearize2<false, false, false, true><<<g2, KA2_THREADS, sm, st>>>(db, kp);
+  } else if (ctx->linearize_variant == 1) {
     const dim3 grid(db.chunks, B);
     const size_t sm = ka_smem_bytes(M_cap);
     if (holo && geom) k_linearize<true, true><<<grid, KA_THREADS, sm, st>>>(db, kp);
@@ -444,25 +512,35 @@ static void launch_linearize(tebgpu_ctx* ctx, const DevBatch& db, const KParams&
   }
 }
 static void launch_build_graph(const DevBatch& db, const KParams& kp, int B, size_t smem, cudaStream_t st) {
-  if (kp.generic) k_build_graph<true><<<B, 256, smem, st>>>(db, kp);
+  if (global_table(db.M_cap)) {
+    if (kp.generic) k_build_graph<true, true><<<B, 256, 0, st>>>(db, kp);
+    else k_build_graph<false, true><<<B, 256, 0, st>>>(db, kp);
+  } else if (kp.generic) k_build_graph<true><<<B, 256, smem, st>>>(db, kp);
   else k_build_graph<false><<<B, 256, smem, st>>>(db, kp);
 }
 static void launch_vor(const DevBatch& db, const KParams& kp, int B, size_t smem, cudaStream_t st) {
-  if (kp.generic) k_vor<true><<<B, 256, smem, st>>>(db, kp);
+  if (global_table(db.M_cap)) {
+    if (kp.generic) k_vor<true, true><<<B, 256, 0, st>>>(db, kp);
+    else k_vor<false, true><<<B, 256, 0, st>>>(db, kp);
+  } else if (kp.generic) k_vor<true><<<B, 256, smem, st>>>(db, kp);
   else k_vor<false><<<B, 256, smem, st>>>(db, kp);
 }
 static size_t eval_bytes(const tebgpu_ctx* ctx, int n_cap, int M_cap, int K) {
+  if (global_table(M_cap)) M_cap = 0; /* no copy of the table: the trial width is not limited by M_cap */
   return ctx->eval_v1 ? eval_smem_bytes(n_cap, M_cap, K) : eval2_smem_bytes(n_cap, M_cap, K);
 }
 static void launch_trial_eval(tebgpu_ctx* ctx, const SpecBufs& spec, const DevBatch& db, const KParams& kp, int B, int K,
                               size_t smem, int it, int round, int g, int tag, cudaStream_t st) {
   /* latency regime: a CTA per (band, trial) instead of a CTA per band while that still fits ~3 CTAs per SM */
-  const size_t smem3 = eval3_smem_bytes(db.n_cap, db.M_cap, K);
+  const bool gt = global_table(db.M_cap);
+  const size_t smem3 = eval3_smem_bytes(db.n_cap, gt ? 0 : db.M_cap, K);
   if (!ctx->eval_v1 && smem3 <= 232448 && (ctx->eval_mode == 1 || (ctx->eval_mode == 2 && (long long)B * K <= ctx->sms * 3))) {
     int warps = ev2_tiles(db.n_cap);
     warps = warps < 1 ? 1 : (warps > 16 ? 16 : warps);
     const dim3 grid(K, B);
-    if (kp.generic) k_trial_eval3<true><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
+    if (gt && kp.generic) k_trial_eval3<true, true><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
+    else if (gt) k_trial_eval3<false, true><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
+    else if (kp.generic) k_trial_eval3<true><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
     else k_trial_eval3<false><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
     return;
   }
@@ -478,7 +556,12 @@ static void launch_trial_eval(tebgpu_ctx* ctx, const SpecBufs& spec, const DevBa
     warps = warps < 2 ? 2 : (warps > 8 ? 8 : warps);
     if (wide) warps = 2 * warps;
     const int nt = 32 * warps;
-    if (kp.generic) {
+    if (gt) {
+      if (kp.generic && relaxed) k_trial_eval2<true, 512, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+      else if (kp.generic) k_trial_eval2<true, 256, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+      else if (relaxed) k_trial_eval2<false, 512, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+      else k_trial_eval2<false, 256, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+    } else if (kp.generic) {
       if (relaxed) k_trial_eval2<true, 512><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
       else k_trial_eval2<true, 256><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
     } else {
@@ -558,6 +641,7 @@ static DevBatch make_devbatch(tebgpu_ctx* ctx, const TebBatch* bt) {
   d.chunks = (bt->n_cap + d.tile - 1) / d.tile;
   d.obst_vertices = bt->PV_cap > 0 ? bt->obst_vertices : nullptr; d.PV_cap = bt->PV_cap;
   d.defer = ctx->defer; d.a_list = nullptr; d.a_cnt = nullptr; d.skip_tag = 0;
+  d.occ = ctx->occ; d.OW = (d.MW + 63) / 64;
   return d;
 }
 
@@ -628,7 +712,7 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
   const size_t smem_bcr = kb_bcr_smem_bytes(bt->n_cap, bt->M_cap);
   const bool use_bcr = ctx->solver == 1 && bt->n_cap <= BCR_MAX_POSES && smem_bcr <= 232448 &&
                        ctx->lim.max_poses <= BCR_MAX_POSES;
-  const size_t smem_g = (size_t)(bt->M_cap > 0 ? bt->M_cap : 1) * sizeof(TebObstacle);
+  const size_t smem_g = (size_t)(bt->M_cap > 0 ? bt->M_cap : 1) * sizeof(TebObstacle); /* staged path only */
   /* speculation width: one solver warp per SM sub-partition is the latency-optimal regime (SMs x 4 x 32 lanes);
    * below it the wider speculation is free and removes the second round, above it the factor traffic dominates */
   /* Speculation schedule: widths of the rounds of one LM iteration (they add up to g2o's 10 trials).
@@ -829,6 +913,8 @@ static uint64_t graph_key(const tebgpu_ctx* ctx, const TebBatch* bt, const TebOp
 int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args, void* cuda_stream) {
   int32_t rc = check_batch(ctx, bt);
   if (rc) return rc;
+  rc = check_path(ctx, bt, true);
+  if (rc) return rc;
   if (!args || args->iterations_innerloop < 0 || args->iterations_outerloop < 0) { ctx->err = "bad optimize args"; return TEBGPU_ERR_INVALID_ARG; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
@@ -1015,6 +1101,8 @@ int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimi
   int32_t rc = check_batch(ctx, bt);
   if (rc) return rc;
   if (!args) return TEBGPU_ERR_INVALID_ARG;
+  rc = check_path(ctx, bt, false);
+  if (rc) return rc;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   rc = upload_batch(ctx, bt);
   if (rc) return rc;
@@ -1041,6 +1129,9 @@ int32_t tebgpu_h_signature(tebgpu_ctx* ctx, const TebBatch* bt, int32_t use_time
   int32_t rc = check_batch(ctx, bt);
   if (rc) return rc;
   if (!h_out) return TEBGPU_ERR_INVALID_ARG;
+  /* The 2-D signature is a product over the M - 1 obstacle differences (long double in the reference); at thousands of
+   * obstacles it leaves the fp64 range, so large scenes need a design of their own (DESIGN §9). */
+  if (global_table(bt->M_cap)) { ctx->err = "the H-signature supports at most 1024 obstacles per scene"; return TEBGPU_ERR_UNSUPPORTED; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   TebBatch d = *bt;
   if (!device_ptrs) {
@@ -1076,6 +1167,8 @@ int32_t tebgpu_h_signature(tebgpu_ctx* ctx, const TebBatch* bt, int32_t use_time
 int32_t tebgpu_build_system(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_index, double* Hb_out, double* chi2_out,
                             int32_t device_ptrs) {
   int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  rc = check_path(ctx, bt, false);
   if (rc) return rc;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   TebBatch d = *bt;

@@ -38,7 +38,9 @@ constexpr int ESTR = 10;               /* residual slots per anchor: vx|v, omega
 constexpr int START_E = 21;            /* start-edge block: 3 rows x 7 columns, then its 3 residuals */
 constexpr int HROW = 12;               /* doubles per band row: 11 band entries + rhs */
 constexpr int KB_THREADS = 128;
-constexpr int MAX_MW = 16;             /* association bitmask words per pose (<= 1024 obstacles per scene) */
+constexpr int MAX_MW = 16;             /* association bitmask words per pose of the staged path (<= 1024 obstacles per scene) */
+constexpr int STAGED_MAX_OBST = 64 * MAX_MW; /* largest M_cap whose table the staged kernels copy into shared memory */
+constexpr int GT_MAX_MW = 256;         /* association words per pose of the global-table path (<= 16384 obstacles per scene) */
 
 struct BandState {
   double lambda, ni, current_chi, chi2_final;
@@ -89,7 +91,33 @@ struct DevBatch {
   const int32_t* a_cnt;
   int32_t* defer;             /* [B] tag of the inner iteration in which the band was queued for a retry round */
   int32_t skip_tag;
+  /* global-table path (M_cap > STAGED_MAX_OBST): occupancy words of the association, bit w of word w >> 6 set iff
+   * association word w of the pose is non-zero, so that per-iteration kernels read only the words that hold bits */
+  unsigned long long* occ;    /* [B][n_cap][OW] */
+  int32_t OW;                 /* ceil(MW / 64) */
 };
+
+/* Global-table path: the obstacles associated with pose row pr = b * n_cap + i, in increasing index order (the order
+ * of the staged kernels' walk over all MW words): visit(w, m) for obstacle m of association word w. Only the words the
+ * pose's occupancy words mark non-zero are read. */
+template <class F>
+__device__ __forceinline__ void walk_assoc_occ(const DevBatch& db, size_t pr, F&& visit) {
+  const unsigned long long* am = db.assoc + pr * db.MW;
+  const unsigned long long* oc = db.occ + pr * db.OW;
+  for (int o = 0; o < db.OW; ++o) {
+    unsigned long long ow = oc[o];
+    while (ow) {
+      const int w = (o << 6) + __ffsll((long long)ow) - 1;
+      ow &= ow - 1;
+      unsigned long long mask = am[w];
+      while (mask) {
+        const int m = (w << 6) + __ffsll((long long)mask) - 1;
+        mask &= mask - 1;
+        visit(w, m);
+      }
+    }
+  }
+}
 
 /* A band belongs to the side stream's share when it was queued for retry rounds in the iteration with tag `skip_tag` -
  * or, meanwhile, AGAIN in the following one: the side stream's own round 0 of the current iteration may re-queue it
@@ -195,11 +223,14 @@ __global__ void k_auto_resize(DevBatch db, KParams kp) {
   db.n[b] = nn;
 }
 
-/* ------------------------------------------------------------------ k_build_graph (CTA per band) */
-template <bool GEOM>
+/* ------------------------------------------------------------------ k_build_graph (CTA per band)
+ * GT = global-table path (M_cap > STAGED_MAX_OBST): obstacle rows are read from global memory (L2) instead of a
+ * shared-memory copy of the scene's table, the non-legacy association runs one warp per pose with the obstacles across
+ * the lanes, and the occupancy words of every pose are written at the end. */
+template <bool GEOM, bool GT = false>
 __global__ void __launch_bounds__(256) k_build_graph(DevBatch db, KParams kp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  TebObstacle* so = reinterpret_cast<TebObstacle*>(smem_raw);
+  TebObstacle* so_s = reinterpret_cast<TebObstacle*>(smem_raw);
   const int b = linearize_band(db, blockIdx.x);
   if (b < 0) return;
   BandState* st = &db.state[b];
@@ -219,14 +250,74 @@ __global__ void __launch_bounds__(256) k_build_graph(DevBatch db, KParams kp) {
   const int s = db.scene_id[b];
   const int M = db.obst_count[s];
   const TebObstacle* go = db.obstacles + (size_t)s * db.M_cap;
-  for (int m = threadIdx.x; m < M; m += blockDim.x) so[m] = go[m];
+  if constexpr (!GT)
+    for (int m = threadIdx.x; m < M; m += blockDim.x) so_s[m] = go[m];
   __syncthreads();
+  const TebObstacle* so = GT ? go : so_s;
   const double* P = db.poses + (size_t)b * db.n_cap * 4;
   const double* pool = db.obst_vertices + (size_t)s * db.PV_cap * 2; /* only dereferenced for vertex-list obstacles */
   unsigned long long* assoc = db.assoc + (size_t)b * db.n_cap * db.MW;
 
   unsigned long long* assoc3 = db.assoc3 + (size_t)b * db.n_cap * db.MW;
-  if (!kp.p.legacy_obstacle_association) {
+  if (GT && !kp.p.legacy_obstacle_association) {
+    /* the same association, one warp per pose: the force-inclusion bits of each 64-obstacle word are two ballots; the
+     * closest left / right obstacle within the cutoff is a warp argmin over (dist, m) taken lexicographically, i.e. the
+     * lowest index among equal distances - what the sequential strict-< scan keeps. A NaN distance fails every
+     * comparison and never becomes a candidate, as in the scan. */
+    const int first_vertex = kp.has_vor ? 0 : 1;
+    const int lane = threadIdx.x & 31;
+    const double force_d = kp.p.min_obstacle_dist * kp.p.obstacle_association_force_inclusion_factor;
+    const double cut_d = kp.p.min_obstacle_dist * kp.p.obstacle_association_cutoff_factor;
+    for (int i = threadIdx.x >> 5; i < n; i += blockDim.x >> 5) {
+      unsigned long long* am = assoc + (size_t)i * db.MW;
+      if (!(kp.has_obst && i >= first_vertex && i <= n - 2)) {
+        for (int w = lane; w < db.MW; w += 32) am[w] = 0ull;
+        continue;
+      }
+      const double px = P[4 * i], py = P[4 * i + 1], th = P[4 * i + 2];
+      double sn, cs;
+      sincos(th, &sn, &cs);
+      double left_min = 1.7976931348623157e308, right_min = 1.7976931348623157e308;
+      int left = INT_MAX, right = INT_MAX; /* INT_MAX: none (sorts after every index) */
+      for (int w = 0; w < db.MW; ++w) {
+        unsigned half[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = (w << 6) + (h << 5) + lane;
+          bool force = false;
+          if (m < M) {
+            const TebObstacle ob = go[m];
+            if (!(kp.p.include_dynamic_obstacles && ob.dynamic)) {
+              const double dist = robot_obstacle_distance_only<GEOM>(kp, pool, px, py, cs, sn, ob, ob.x, ob.y, 0.0, 0.0);
+              if (dist < force_d) {
+                force = true;
+              } else if (!(dist > cut_d)) {
+                const double cx = ob.x - px, cy = ob.y - py;
+                if (cs * cy - cx * sn > 0) {
+                  if (dist < left_min) { left_min = dist; left = m; }
+                } else {
+                  if (dist < right_min) { right_min = dist; right = m; }
+                }
+              }
+            }
+          }
+          half[h] = __ballot_sync(0xffffffffu, force);
+        }
+        if (lane == 0) am[w] = ((unsigned long long)half[1] << 32) | half[0];
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const double ld = __shfl_xor_sync(0xffffffffu, left_min, o), rd = __shfl_xor_sync(0xffffffffu, right_min, o);
+        const int lm = __shfl_xor_sync(0xffffffffu, left, o), rm = __shfl_xor_sync(0xffffffffu, right, o);
+        if (ld < left_min || (ld == left_min && lm < left)) { left_min = ld; left = lm; }
+        if (rd < right_min || (rd == right_min && rm < right)) { right_min = rd; right = rm; }
+      }
+      if (lane == 0) {
+        if (left != INT_MAX) am[left >> 6] |= 1ull << (left & 63);
+        if (right != INT_MAX) am[right >> 6] |= 1ull << (right & 63);
+      }
+    }
+  } else if (!kp.p.legacy_obstacle_association) {
     /* AddEdgesObstacles association (optimal_planner.cpp:484-547); pose 0 takes part only to feed
      * EdgeVelocityObstacleRatio (first_vertex, :482) */
     const int first_vertex = kp.has_vor ? 0 : 1;
@@ -350,18 +441,48 @@ __global__ void __launch_bounds__(256) k_build_graph(DevBatch db, KParams kp) {
       }
     }
   }
+  if constexpr (GT) { /* occupancy words: bit w of the pose's word w >> 6 iff association word w is non-zero */
+    __syncthreads();
+    unsigned long long* occ = db.occ + (size_t)b * db.n_cap * db.OW;
+    for (int k = threadIdx.x; k < n * db.OW; k += blockDim.x) {
+      const int i = k / db.OW, o = k - i * db.OW;
+      const unsigned long long* am = assoc + (size_t)i * db.MW + 64 * o;
+      const int nw = min(db.MW - 64 * o, 64);
+      unsigned long long bits = 0ull;
+      for (int w = 0; w < nw; ++w)
+        if (am[w]) bits |= 1ull << w;
+      occ[k] = bits;
+    }
+  }
 }
 
 /* ------------------------------------------------------------------ unary terms of one pose (obstacles, dynamic
  * obstacles, via-points): accumulates U = sum kappa g g^T (xx,xy,yy,xt,yt,tt), ub = -sum beta g, chi2 by family */
-template <bool GEOM>
+template <bool GEOM, bool GT = false> /* GT: so is the scene's table in global memory, walk via the occupancy words */
 __device__ __forceinline__ void unary_terms(const KParams& kp, const DevBatch& db, int b, int sc, int i, int n, double px,
                                             double py, double cs, double sn, const TebObstacle* so, int M,
                                             bool want_grad, double U[6], double ub[3], double& chi_obst,
                                             double& chi_via) {
   if (i < 1 || i > n - 2) return;
   const double* pool = db.obst_vertices + (size_t)sc * db.PV_cap * 2; /* only dereferenced for vertex-list obstacles */
-  if (kp.has_obst) {
+  if (GT && kp.has_obst) {
+    walk_assoc_occ(db, (size_t)b * db.n_cap + i, [&](int w, int m) {
+      const TebObstacle ob = so[m];
+      double g[3], kappa, beta;
+      const double d = robot_obstacle_distance<GEOM>(kp, pool, px, py, cs, sn, ob, ob.x, ob.y, 0.0, 0.0, g);
+      double cterm = obstacle_terms(kp, d, kappa, beta);
+      if (kp.p.legacy_obstacle_association &&
+          ((db.assoc3[((size_t)b * db.n_cap + i) * db.MW + w] >> (m & 63)) & 1ull)) {
+        cterm *= 3; kappa *= 3; beta *= 3;
+      }
+      chi_obst += cterm;
+      if (want_grad && (kappa != 0 || beta != 0)) {
+        U[0] += kappa * g[0] * g[0]; U[1] += kappa * g[0] * g[1]; U[2] += kappa * g[1] * g[1];
+        U[3] += kappa * g[0] * g[2]; U[4] += kappa * g[1] * g[2]; U[5] += kappa * g[2] * g[2];
+        ub[0] -= beta * g[0]; ub[1] -= beta * g[1]; ub[2] -= beta * g[2];
+      }
+    });
+  } else if (kp.has_obst) {
     const unsigned long long* assoc = db.assoc + ((size_t)b * db.n_cap + i) * db.MW;
     for (int w = 0; w < db.MW; ++w) {
       unsigned long long mask = assoc[w];
@@ -1681,18 +1802,20 @@ __global__ void k_finalize(DevBatch db, KParams kp, TebOptimizeArgs args) {
  * optimal_planner.cpp:999-1021). One edge per obstacle associated with pose a over (pose a, pose a+1, dt_a); the
  * 7x7 J^T Omega J of every anchor is added to the band written by kernel A. Even anchors first, then odd ones, so
  * that overlapping rows are updated in a fixed order (deterministic, no atomics). */
-template <bool GEOM>
+template <bool GEOM, bool GT = false> /* GT: obstacle rows read from global memory, associations via the occupancy words */
 __global__ void __launch_bounds__(256) k_vor(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp) {
   extern __shared__ __align__(16) unsigned char vor_raw[];
-  TebObstacle* so = reinterpret_cast<TebObstacle*>(vor_raw);
+  TebObstacle* so_s = reinterpret_cast<TebObstacle*>(vor_raw);
   __shared__ double s_red[8];
   const int b = blockIdx.x;
   if (!db.state[b].active) return;
   const int n = db.n[b];
   const int sc = db.scene_id[b];
   const int M = db.obst_count[sc];
-  for (int m = threadIdx.x; m < M; m += blockDim.x) so[m] = db.obstacles[(size_t)sc * db.M_cap + m];
+  if constexpr (!GT)
+    for (int m = threadIdx.x; m < M; m += blockDim.x) so_s[m] = db.obstacles[(size_t)sc * db.M_cap + m];
   __syncthreads();
+  const TebObstacle* so = GT ? db.obstacles + (size_t)sc * db.M_cap : so_s;
   const double* P = db.poses + (size_t)b * db.n_cap * 4;
   const double* pool = db.obst_vertices + (size_t)sc * db.PV_cap * 2;
   double* H = db.Hb + (size_t)b * 4 * db.n_cap * HROW;
@@ -1713,7 +1836,17 @@ __global__ void __launch_bounds__(256) k_vor(const __grid_constant__ DevBatch db
 #pragma unroll
       for (int k = 0; k < 7; ++k) gb[k] = 0;
       const unsigned long long* am = db.assoc + ((size_t)b * db.n_cap + a) * db.MW;
-      for (int w = 0; w < db.MW; ++w) {
+      /* GT: one pass over the occupancy words yields the non-zero words in increasing order */
+      const unsigned long long* oc = db.occ + ((size_t)b * db.n_cap + a) * db.OW;
+      unsigned long long ow = 0ull;
+      int o = 0;
+      for (int w = 0; GT ? true : w < db.MW; ++w) {
+        if constexpr (GT) {
+          while (ow == 0ull && o < db.OW) ow = oc[o++];
+          if (ow == 0ull) break;
+          w = ((o - 1) << 6) + __ffsll((long long)ow) - 1;
+          ow &= ow - 1;
+        }
         unsigned long long mask = am[w];
         while (mask) {
           const int m = (w << 6) + __ffsll((long long)mask) - 1;

@@ -452,7 +452,9 @@ __device__ __forceinline__ void gram_start(const double* sStart, double (&acc)[4
 }
 
 /* unary terms of pose i with the first association word already in a register (prefetched before the TMA wait) */
-template <bool GEOM>
+/* GT (global-table path): so is the scene's table in global memory, mask0 the pose's first OCCUPANCY word, and only
+ * the association words it marks are read */
+template <bool GEOM, bool GT = false>
 __device__ __forceinline__ void unary_terms2(const KParams& kp, const DevBatch& db, int b, int sc, int i, int n, double px,
                                              double py, double cs, double sn, const TebObstacle* so, unsigned long long mask0,
                                              double U[6], double ub[3], double& chi_obst, double& chi_via) {
@@ -460,8 +462,17 @@ __device__ __forceinline__ void unary_terms2(const KParams& kp, const DevBatch& 
   const double* pool = db.obst_vertices + (size_t)sc * db.PV_cap * 2; /* only dereferenced for vertex-list obstacles */
   if (kp.has_obst) {
     const unsigned long long* assoc = db.assoc + ((size_t)b * db.n_cap + i) * db.MW;
-    for (int w = 0; w < db.MW; ++w) {
-      unsigned long long mask = (w == 0) ? mask0 : assoc[w];
+    const unsigned long long* oc = db.occ + ((size_t)b * db.n_cap + i) * db.OW;
+    unsigned long long ow = mask0;
+    int o = 1;
+    for (int w = 0; GT ? true : w < db.MW; ++w) {
+      if constexpr (GT) { /* next non-zero association word, in increasing order */
+        while (ow == 0ull && o < db.OW) ow = oc[o++];
+        if (ow == 0ull) break;
+        w = ((o - 1) << 6) + __ffsll((long long)ow) - 1;
+        ow &= ow - 1;
+      }
+      unsigned long long mask = GT ? assoc[w] : (w == 0) ? mask0 : assoc[w];
       while (mask) {
         const int m = (w << 6) + __ffsll((long long)mask) - 1;
         mask &= mask - 1;
@@ -520,7 +531,9 @@ __device__ __forceinline__ void unary_terms2(const KParams& kp, const DevBatch& 
 __device__ __forceinline__ double shfl_down1(double v) { return __shfl_down_sync(0xffffffffu, v, 1); }
 
 /* ------------------------------------------------------------------ k_linearize2 */
-template <bool HOLO, bool GEOM, bool OUT_DIRECT>
+/* GT = global-table path (M_cap > STAGED_MAX_OBST): no TMA copy of the scene's obstacle table, rows read from global
+ * memory, associations walked via the occupancy words */
+template <bool HOLO, bool GEOM, bool OUT_DIRECT, bool GT = false>
 __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   using L = JL<HOLO>;
@@ -529,7 +542,7 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
   double* sW = sP + KA2Smem::POSES + (size_t)warp * KA2Smem::warp_doubles<HOLO>(); /* this warp's records / output slots */
   double* sStart = sW + KA2Smem::rec_doubles<HOLO>();                    /* EdgeAccelerationStart rows (tile of anchor 0) */
   uint64_t* bar = reinterpret_cast<uint64_t*>(sP + KA2Smem::POSES + (size_t)KA2_W * KA2Smem::warp_doubles<HOLO>());
-  TebObstacle* so = reinterpret_cast<TebObstacle*>((reinterpret_cast<uintptr_t>(bar) + 16 + 15) & ~static_cast<uintptr_t>(15));
+  TebObstacle* so_s = reinterpret_cast<TebObstacle*>((reinterpret_cast<uintptr_t>(bar) + 16 + 15) & ~static_cast<uintptr_t>(15));
 
   /* everything the prologue needs is loaded at once: no chain of dependent global loads */
   const int y = blockIdx.y;
@@ -549,10 +562,10 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
   if (!active || P0 + 2 >= n) return;                                     /* uniform for the CTA, nothing in flight yet */
   if (tid == 0) {
     const uint32_t bytesP = (uint32_t)(hi - lo) * 32u;
-    const uint32_t bytesO = (uint32_t)db.M_cap * (uint32_t)sizeof(TebObstacle);
+    const uint32_t bytesO = GT ? 0u : (uint32_t)db.M_cap * (uint32_t)sizeof(TebObstacle);
     mbar_expect_tx(bar, bytesP + bytesO);
     tma_load_1d(sP + (size_t)(lo - P0) * 4, db.poses + ((size_t)b * db.n_cap + lo) * 4, bytesP, bar);
-    if (bytesO) tma_load_1d(so, db.obstacles + (size_t)s * db.M_cap, bytesO, bar);
+    if (bytesO) tma_load_1d(so_s, db.obstacles + (size_t)s * db.M_cap, bytesO, bar);
   }
   const int slot = warp * KA2_TP + lane;
   const int i = P0 + slot;                                                /* pose / anchor of this lane */
@@ -560,7 +573,8 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
   const bool out = (lane >= 2 && lane <= 30 && i < n);
   /* while the copies are in flight: association word of the own pose, zeroed record and start block */
   unsigned long long mask0 = 0ull;
-  if (out && kp.has_obst && i >= 1 && i <= n - 2) mask0 = db.assoc[((size_t)b * db.n_cap + i) * db.MW];
+  if (out && kp.has_obst && i >= 1 && i <= n - 2)
+    mask0 = GT ? db.occ[((size_t)b * db.n_cap + i) * db.OW] : db.assoc[((size_t)b * db.n_cap + i) * db.MW];
   {
     double* rec = sW + lane;
 #pragma unroll
@@ -584,7 +598,9 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
   if (have_pose) {
     sincos(pa[2], &sn, &cs);
     if (i <= n - 2) sd = seg_derivs(kp, pa[0], pa[1], pa[2], cs, sn, pa[4], pa[5], pa[6], pa[3]);
-    if (out) unary_terms2<GEOM>(kp, db, b, s, i, n, pa[0], pa[1], cs, sn, so, mask0, U, ub, chi[0], chi[1]);
+    if (out)
+      unary_terms2<GEOM, GT>(kp, db, b, s, i, n, pa[0], pa[1], cs, sn, GT ? db.obstacles + (size_t)s * db.M_cap : so_s, mask0, U, ub,
+                             chi[0], chi[1]);
   }
   /* the right neighbour's sin / cos and segment bundle (lane 31 receives nothing useful and anchors nothing) */
   SegDer sd2;

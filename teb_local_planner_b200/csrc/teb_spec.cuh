@@ -901,7 +901,7 @@ __host__ __device__ inline size_t eval2_smem_bytes(int n_cap, int M_cap, int K) 
 /* chi2 contributions of everything anchored at pose i of a trial state held in registers: chain edges of segment i,
  * time-optimal edge i, unary edges of pose i. (xa .. dta, ca, sa): pose i; (xb .. dtb, cb, sb): pose i+1; s1 / s2:
  * velocities of the segments i and i+1. Same arithmetic as pose_chi2 (teb_kernels.cuh). */
-template <bool GEOM>
+template <bool GEOM, bool GT = false>
 __device__ __forceinline__ void pose_chi2_lane(const KParams& kp, const DevBatch& db, int b, int sc, int i, int n, double xa,
                                                double ya, double tha, double dta, double ca, double sa, double xb, double yb,
                                                double thb, double dtb, double cb, double sb, const SegVal& s1, const SegVal& s2,
@@ -994,7 +994,17 @@ __device__ __forceinline__ void pose_chi2_lane(const KParams& kp, const DevBatch
     }
     if (kp.has_vor) { /* EdgeVelocityObstacleRatio: obstacles associated with pose i (pose 0 included) */
       const unsigned long long* am = db.assoc + ((size_t)b * db.n_cap + i) * db.MW;
-      for (int w = 0; w < db.MW; ++w) {
+      /* GT: one pass over the occupancy words yields the non-zero words in increasing order */
+      const unsigned long long* oc = db.occ + ((size_t)b * db.n_cap + i) * db.OW;
+      unsigned long long ow = 0ull;
+      int o = 0;
+      for (int w = 0; GT ? true : w < db.MW; ++w) {
+        if constexpr (GT) {
+          while (ow == 0ull && o < db.OW) ow = oc[o++];
+          if (ow == 0ull) break;
+          w = ((o - 1) << 6) + __ffsll((long long)ow) - 1;
+          ow &= ow - 1;
+        }
         unsigned long long mask = am[w];
         while (mask) {
           const int m = (w << 6) + __ffsll((long long)mask) - 1;
@@ -1014,13 +1024,13 @@ __device__ __forceinline__ void pose_chi2_lane(const KParams& kp, const DevBatch
     if (kp.has_time) chi[2] += kp.p.weight_optimaltime * dta * dta;
   }
   double U[6], ub[3];
-  unary_terms<GEOM>(kp, db, b, sc, i, n, xa, ya, ca, sa, so, M, false, U, ub, chi[0], chi[1]);
+  unary_terms<GEOM, GT>(kp, db, b, sc, i, n, xa, ya, ca, sa, so, M, false, U, ub, chi[0], chi[1]);
 }
 
 /* One (trial, 30-pose tile) task of a warp: lane -> pose i = tile * 30 + lane (lanes 30, 31 are the halo). Forms the trial
  * state x [+] dx of its pose, gets the right neighbour's by shuffles, evaluates every cost term anchored at the pose and
  * returns the warp sums: chi2 by family and the computeScale() part of the owned rows. Shared by k_trial_eval2 / 3. */
-template <bool GEOM>
+template <bool GEOM, bool GT = false>
 __device__ __forceinline__ void eval_tile_task(const KParams& kp, const DevBatch& db, int b, int sc, int n, int tile, int lane, bool ok,
                                                double lambda, const double* mydx, const double* sP0, const double* sB,
                                                const TebObstacle* so, int M, const double* vs, const double* vg, double (&chi)[4],
@@ -1058,13 +1068,15 @@ __device__ __forceinline__ void eval_tile_task(const KParams& kp, const DevBatch
   SegVal s2;
   s2.v = __shfl_down_sync(0xffffffffu, s1.v, 1); s2.w = __shfl_down_sync(0xffffffffu, s1.w, 1);
   s2.vx = __shfl_down_sync(0xffffffffu, s1.vx, 1); s2.vy = __shfl_down_sync(0xffffffffu, s1.vy, 1);
-  if (own) pose_chi2_lane<GEOM>(kp, db, b, sc, i, n, x, y, th, dt, ca, sa, xb, yb, thb, dtb, cb, sb, s1, s2, so, M, vs, vg, chi);
+  if (own) pose_chi2_lane<GEOM, GT>(kp, db, b, sc, i, n, x, y, th, dt, ca, sa, xb, yb, thb, dtb, cb, sb, s1, s2, so, M, vs, vg, chi);
 #pragma unroll
   for (int c = 0; c < 4; ++c) chi[c] = warp_sum(chi[c]);
   scl = warp_sum(scl);
 }
 
-template <bool GEOM, int NT> /* NT = 256 (throughput regime, 2 CTAs per SM) or 512 (latency regime: more warps per band) */
+/* NT = 256 (throughput regime, 2 CTAs per SM) or 512 (latency regime: more warps per band). GT = global-table path
+ * (M_cap > STAGED_MAX_OBST): no copy of the scene's obstacle table, rows read from global memory. */
+template <bool GEOM, int NT, bool GT = false>
 __global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_trial_eval2(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp,
                                                              const __grid_constant__ SpecBufs sp, int iteration, int round,
                                                              int g, int tag) {
@@ -1087,12 +1099,14 @@ __global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_t
   double* sPart = sB + (size_t)4 * db.n_cap;                   /* [K][tiles(n_cap)][5] tile partials: chi by family, scale */
   double* sRes = sPart + (size_t)SPEC_K * ev2_tiles(db.n_cap) * 5; /* [K][RES_STRIDE] */
   int* sAcc = reinterpret_cast<int*>(sRes + (size_t)SPEC_K * RES_STRIDE);
-  TebObstacle* so = reinterpret_cast<TebObstacle*>(sAcc + 4);
+  TebObstacle* so_s = reinterpret_cast<TebObstacle*>(sAcc + 4);
   const int sc = db.scene_id[b];
   const int M = db.obst_count[sc];
+  const TebObstacle* so = GT ? db.obstacles + (size_t)sc * db.M_cap : so_s;
   {
     const TebObstacle* go = db.obstacles + (size_t)sc * db.M_cap;
-    for (int m = tid; m < M; m += nthreads) so[m] = go[m];
+    if constexpr (!GT)
+      for (int m = tid; m < M; m += nthreads) so_s[m] = go[m];
     const double* gP = db.poses + (size_t)b * db.n_cap * 4;
     const double* grhs = db.rhs + (size_t)b * 4 * db.n_cap;
     /* the K trial solutions of a band sit in adjacent lanes of the solver's interleaved scratch (K even) */
@@ -1115,7 +1129,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_t
     const int k = task / tiles, tile = task - k * tiles;
     const double* res = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
     double chi[4], scl;
-    eval_tile_task<GEOM>(kp, db, b, sc, n, tile, lane, res[5] != 0.0, res[6], sdx + (size_t)k * 4 * db.n_cap, sP0, sB, so, M, vs, vg,
+    eval_tile_task<GEOM, GT>(kp, db, b, sc, n, tile, lane, res[5] != 0.0, res[6], sdx + (size_t)k * 4 * db.n_cap, sP0, sB, so, M, vs, vg,
                          chi, scl);
     if (lane == 0) {
       double* pp = sPart + ((size_t)k * ev2_tiles(db.n_cap) + tile) * 5;
@@ -1174,7 +1188,7 @@ __host__ __device__ inline size_t eval3_smem_bytes(int n_cap, int M_cap, int K) 
          ((size_t)ev2_tiles(n_cap) * 5 + (size_t)K * RES_STRIDE) * sizeof(double) + 64;
 }
 
-template <bool GEOM>
+template <bool GEOM, bool GT = false> /* GT: as k_trial_eval2 */
 __global__ void __launch_bounds__(512, 1) k_trial_eval3(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp,
                                                         const __grid_constant__ SpecBufs sp, int iteration, int round, int g,
                                                         int tag, int32_t* arrive) {
@@ -1199,9 +1213,10 @@ __global__ void __launch_bounds__(512, 1) k_trial_eval3(const __grid_constant__ 
   double* sPart = sB + (size_t)4 * db.n_cap;                   /* [tiles(n_cap)][5] tile partials: chi by family, scale */
   double* sRes = sPart + (size_t)ev2_tiles(db.n_cap) * 5;      /* [K][RES_STRIDE], filled by the deciding CTA */
   int* sAcc = reinterpret_cast<int*>(sRes + (size_t)SPEC_K * RES_STRIDE);
-  TebObstacle* so = reinterpret_cast<TebObstacle*>(sAcc + 4);
+  TebObstacle* so_s = reinterpret_cast<TebObstacle*>(sAcc + 4);
   const int sc = db.scene_id[b];
   const int M = db.obst_count[sc];
+  const TebObstacle* so = GT ? db.obstacles + (size_t)sc * db.M_cap : so_s;
   double* gP = db.poses + (size_t)b * db.n_cap * 4;
   auto dx_of = [&](int kk) { /* trial kk's solution in the solver's interleaved scratch: + r * 32 */
     const int tsys = slot * SPEC_K + kk;
@@ -1209,7 +1224,8 @@ __global__ void __launch_bounds__(512, 1) k_trial_eval3(const __grid_constant__ 
   };
   {
     const TebObstacle* go = db.obstacles + (size_t)sc * db.M_cap;
-    for (int m = tid; m < M; m += nthreads) so[m] = go[m];
+    if constexpr (!GT)
+      for (int m = tid; m < M; m += nthreads) so_s[m] = go[m];
     const double* grhs = db.rhs + (size_t)b * 4 * db.n_cap;
     const double* gdx = dx_of(k);
     for (int r = tid; r < N; r += nthreads) {
@@ -1227,7 +1243,7 @@ __global__ void __launch_bounds__(512, 1) k_trial_eval3(const __grid_constant__ 
     const double lambda = res[6];
     for (int tile = warp; tile < tiles; tile += nthreads / 32) {
       double chi[4], scl;
-      eval_tile_task<GEOM>(kp, db, b, sc, n, tile, lane, ok, lambda, sdx, sP0, sB, so, M, vs, vg, chi, scl);
+      eval_tile_task<GEOM, GT>(kp, db, b, sc, n, tile, lane, ok, lambda, sdx, sP0, sB, so, M, vs, vg, chi, scl);
       if (lane == 0) {
         double* pp = sPart + (size_t)tile * 5;
         pp[0] = chi[0]; pp[1] = chi[1]; pp[2] = chi[2]; pp[3] = chi[3]; pp[4] = scl;

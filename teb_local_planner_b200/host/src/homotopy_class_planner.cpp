@@ -48,6 +48,10 @@ bool HomotopyClassPlanner::plan(const tf::Pose& start, const tf::Pose& goal, con
 /* :107-125 */
 bool HomotopyClassPlanner::plan(const PoseSE2& start, const PoseSE2& goal, const geometry_msgs::Twist* start_vel, bool free_goal_vel) {
   if (!initialized_) return false;
+  if (obstacles_ && obstacles_->size() > 1024) { /* the H-signature's product over the obstacles leaves the double range */
+    std::fprintf(stderr, "HomotopyClassPlanner: more than 1024 obstacles per scene is not supported (H-signature)\n");
+    return false;
+  }
   updateAllTEBs(&start, &goal, start_vel);
   exploreEquivalenceClassesAndInitTebs(start, goal, cfg_->obstacles.min_obstacle_dist, start_vel, free_goal_vel);
   updateReferenceTrajectoryViaPoints(cfg_->hcp.viapoints_all_candidates);

@@ -188,7 +188,13 @@ bool TebOptimalPlanner::runBatch(const TebConfig& cfg, const std::vector<TebOpti
   int M_cap = 1;
   for (auto* oc : scenes)
     if (oc) M_cap = std::max(M_cap, (int)oc->size());
-  if (M_cap > 1024) { std::fprintf(stderr, "optimizeTEB: more than 1024 obstacles per scene is not supported\n"); return false; }
+  if (M_cap > 16384) { std::fprintf(stderr, "optimizeTEB: more than 16384 obstacles per scene is not supported\n"); return false; }
+  /* the 2-D H-signature multiplies M - 1 obstacle differences: beyond 1024 obstacles the product leaves the fp64 range */
+  if (hsig_out && M_cap > 1024) {
+    std::fprintf(stderr, "H-signature: more than 1024 obstacles per scene is not supported (the product over the obstacles "
+                         "leaves the double range)\n");
+    return false;
+  }
   std::vector<TebObstacle> obst((size_t)S * M_cap);
   std::vector<int32_t> obst_count(S, 0);
   std::vector<std::vector<double>> pools(S);

@@ -181,3 +181,48 @@ def set_polygon_footprint(p, vertices=((-0.25, -0.2), (0.35, -0.2), (0.35, 0.2),
     for k, (x, y) in enumerate(vertices):
         p.footprint_vertices[2 * k], p.footprint_vertices[2 * k + 1] = x, y
     return p
+
+
+def costmap_scene(M, n=100, candidates=3, seed=0, amp=0.6, shapes=True):
+    """A scene the way a local costmap produces it: one point obstacle per occupied 5 cm cell (two walls along the
+    corridor and blobs of cells near the band), plus a few circular, line and moving obstacles. Exactly M rows.
+    -> (TebParams, HostBatch) with C3's parameters, moving obstacles switched on and autoResize off."""
+    p = config_params("C3")
+    p.include_dynamic_obstacles = 1
+    p.teb_autosize = 0
+    rng = np.random.default_rng(seed)
+    L = 0.4 * 0.3 * (n - 1)
+    cells = set()
+    res = 0.05
+    for y in (-1.6, 1.6):                              # walls of the corridor
+        for x in np.arange(-L / 2, L / 2, res):
+            cells.add((round(x / res), round(y / res)))
+    while len(cells) < M:                              # blobs of occupied cells beside the band
+        cx, cy = rng.uniform(-L / 2 + 1, L / 2 - 1), rng.choice([-1, 1]) * rng.uniform(0.8, 3.0)
+        r = rng.uniform(0.05, 0.4)
+        for gx in range(round((cx - r) / res), round((cx + r) / res) + 1):
+            for gy in range(round((cy - r) / res), round((cy + r) / res) + 1):
+                if (gx * res - cx) ** 2 + (gy * res - cy) ** 2 <= r * r:
+                    cells.add((gx, gy))
+    cells = sorted(cells, key=lambda c: rng.random())[:M]
+    o = np.zeros(M, abi.OBST_DTYPE)
+    o["x"] = [c[0] * res for c in cells]
+    o["y"] = [c[1] * res for c in cells]
+    pool = np.zeros((0, 2))
+    if shapes:
+        k = rng.choice(M, 12, replace=False)
+        o["type"][k[:4]], o["radius"][k[:4]] = abi.TEB_OBST_CIRCULAR, 0.1
+        o["dynamic"][k[4:8]] = 1                       # moving points
+        o["vx"][k[4:8]], o["vy"][k[4:8]] = rng.uniform(-0.3, 0.3, 4), rng.uniform(-0.3, 0.3, 4)
+        pool = np.zeros((8, 2))
+        for j, m in enumerate(k[8:]):                  # short line segments centred on their cell
+            pool[2 * j] = (o["x"][m] - 0.1, o["y"][m] - 0.05)
+            pool[2 * j + 1] = (o["x"][m] + 0.1, o["y"][m] + 0.05)
+            o["type"][m], o["vertex_begin"][m], o["vertex_count"][m] = abi.TEB_OBST_LINE, 2 * j, 2
+    poses = np.zeros((candidates, n, 4))
+    brng = np.random.default_rng(seed + 1)
+    for b in range(candidates):
+        poses[b] = make_band(n, brng.uniform(-amp, amp), 0.4, 0.3)
+    hb = abi.HostBatch(poses, np.full(candidates, n, np.int32), o, np.array([M], np.int32),
+                       obst_vertices=pool[None] if shapes else None)
+    return p, hb
