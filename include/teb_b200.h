@@ -346,6 +346,29 @@ int32_t tebgpu_solve_system(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, const dou
                             const int32_t* list, int32_t list_len, int32_t lat_cap, double* dx_out, double* ok_out,
                             double* lambda_out);
 
+/* Trial evaluation only: one round of the speculative LM step's trial evaluation and accept / reject chain, launched by
+ * the same code as in tebgpu_optimize_batch (the kernel TEBGPU_EVAL_V1 / TEBGPU_EVAL3 and the batch size select). Test /
+ * profiling entry point of the trial-evaluation kernels. The graph, right-hand side and kernel A's chi2 / max-diagonal
+ * partials are made as tebgpu_build_system makes them for outer_index. HOST buffers:
+ *   bt                   the batch; bt->poses is the band state before the round and receives the state after it;
+ *   iteration            LM iteration (0: round 0 takes lambda = 1e-5 max |H_rr| from kernel A, nu = 2), K: 2 .. 8 even;
+ *   dx [B][K][4 n_cap], ok [B][K], lambda_k [B][K]   the trials as the solve left them (ok 0: failed factorisation,
+ *                        the trial is x + b); a retry round reads the trials of band list[s] from row list[s];
+ *   state [B][TEBGPU_EVAL_STATE]   band state before the round: lambda, nu, currentChi, chi2 by family at the current
+ *                        state (4), at the last evaluated trial (4), status bits, active (1 / 0), LM iterations;
+ *   qmax [B], list       NULL / 0: round 0 over all bands. Otherwise a retry round over the list_len bands of `list`
+ *                        whose first qmax[b] trials were already used.
+ * Outputs (any may be NULL): res_out [B][K][5] each trial's chi2 by family (obstacles, via, time-optimal, other) and
+ * computeScale() sum, all-ones bytes (a NaN) where no trial was evaluated; chi_lin [B][4] kernel A's chi2 by family
+ * (the sum of the band's tile partials); state_out [B][TEBGPU_EVAL_STATE]; qmax_out [B] trials of the iteration;
+ * need_out [B] 1 when the band is queued for another round, 0 when its iteration ended, -1 where no band decided;
+ * next_list [B] and *next_len the bands queued, in queue order. */
+#define TEBGPU_EVAL_STATE 14
+int32_t tebgpu_eval_trials(tebgpu_ctx* ctx, TebBatch* bt, int32_t outer_index, int32_t iteration, int32_t K, const double* dx,
+                           const double* ok, const double* lambda_k, const double* state, const int32_t* qmax,
+                           const int32_t* list, int32_t list_len, double* res_out, double* chi_lin, double* state_out,
+                           int32_t* qmax_out, int32_t* need_out, int32_t* next_list, int32_t* next_len);
+
 /* TebOptimalPlanner::computeCurrentCost called OUTSIDE optimizeTEB (optimal_planner.cpp:1041-1094, graph rebuilt with
  * weight multiplier 1, errors evaluated at the current state): HOST buffers; writes cost[], chi2[], status[]. */
 int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* batch, const TebOptimizeArgs* args);

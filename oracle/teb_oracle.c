@@ -1492,6 +1492,58 @@ static void apply_update(Graph* g) {
 /* ------------------------------------------------------------------ Levenberg-Marquardt (App. A.4/A.5) */
 typedef struct LMState { double lambda, ni; } LMState;
 
+/* The decision on one trial, the body of g2o's do-while after update(x) and computeActiveErrors: rho from the trial's
+ * chi2 and computeScale() sum (scale_sum, without the 1e-3), the lambda / nu update, the status bits. A failed
+ * factorisation counts as tempChi = DBL_MAX. *q counts the trials of the iteration; *stop is set when the loop ends
+ * after this trial. Returns 1 when the trial is accepted. */
+static int lm_decide_trial(double* currentChi, LMState* lm, double tempChi, double scale_sum, int ok, int* q, double* rho,
+                           int32_t* status, int* stop) {
+  if (!ok) { *status |= TEB_STATUS_CHOL_FAILED; tempChi = DBL_MAX; }
+  *rho = (*currentChi - tempChi);
+  *rho /= scale_sum + 1e-3;
+  int accepted = 0;
+  *stop = 0;
+  if (*rho > 0 && isfinite(tempChi)) {
+    double alpha = 1. - pow((2 * *rho - 1), 3);
+    alpha = alpha < (2. / 3.) ? alpha : (2. / 3.);
+    double scaleFactor = (1. / 3.) > alpha ? (1. / 3.) : alpha;
+    lm->lambda *= scaleFactor;
+    lm->ni = 2;
+    *currentChi = tempChi;
+    accepted = 1;
+  } else {
+    lm->lambda *= lm->ni;
+    lm->ni *= 2;
+    if (!isfinite(lm->lambda)) { *status |= TEB_STATUS_NONFINITE; *stop = 1; return 0; }
+  }
+  (*q)++;
+  *stop = !(*rho < 0 && *q < 10);
+  return accepted;
+}
+/* the iteration's Terminate verdict once its trial loop has ended (optimization_algorithm_levenberg.cpp) */
+static int lm_terminates(int q, double rho, const LMState* lm) { return q == 10 || rho == 0 || !isfinite(lm->lambda); }
+
+int32_t teb_oracle_lm_decide(double current_chi, double lambda, double nu, int32_t q0, int32_t count, const double* temp_chi,
+                             const double* scale_sum, const int32_t* ok, int32_t* out_i, double* out_d) {
+  if (!out_i || !out_d || count < 0 || q0 < 0 || (count > 0 && (!temp_chi || !scale_sum || !ok))) return -1;
+  LMState lm = {lambda, nu};
+  int q = q0, stop = 0, accepted = -1, used = 0;
+  int32_t status = 0;
+  double rho = 0;
+  for (int k = 0; k < count && q < 10 && !stop; ++k, ++used)
+    if (lm_decide_trial(&current_chi, &lm, temp_chi[k], scale_sum[k], ok[k] != 0, &q, &rho, &status, &stop)) accepted = k;
+  out_i[0] = accepted;
+  out_i[1] = used;
+  out_i[2] = stop && lm_terminates(q, rho, &lm);
+  out_i[3] = status;
+  out_i[4] = !stop; /* the iteration needs more trials than the sequence holds */
+  out_i[5] = q;
+  out_d[0] = lm.lambda;
+  out_d[1] = lm.ni;
+  out_d[2] = current_chi;
+  return 0;
+}
+
 /* returns 1 = OK, 0 = Terminate */
 static int lm_solve(Graph* g, int iteration, LMState* lm, const OracleOptions* opt, OracleStats* st) {
   double currentChi = compute_active_errors(g);
@@ -1507,12 +1559,11 @@ static int lm_solve(Graph* g, int iteration, LMState* lm, const OracleOptions* o
     lm->ni = 2;
   }
   double rho = 0;
-  int qmax = 0;
+  int qmax = 0, stop = 0;
   do {
     memcpy(g->backup, g->rec, sizeof(double) * 4 * (size_t)g->n); /* _optimizer->push() */
     int ok2 = (opt->solver == ORACLE_SOLVER_DENSE) ? solve_dense(g, lm->lambda) : solve_banded(g, lm->lambda);
     if (!ok2) {
-      st->status |= TEB_STATUS_CHOL_FAILED;
       /* g2o still calls update(x) with whatever the solver left in x; CSparse leaves x = b on failure.
        * The state is restored below (tempChi = DBL_MAX -> reject), so only the cached errors differ. */
       memcpy(g->x, g->b, sizeof(double) * (size_t)g->N);
@@ -1520,33 +1571,17 @@ static int lm_solve(Graph* g, int iteration, LMState* lm, const OracleOptions* o
     st->lm_trials++;
     apply_update(g);
     tempChi = compute_active_errors(g);
-    if (!ok2) tempChi = DBL_MAX;
-    rho = (currentChi - tempChi);
     double scale = 0;
     for (int j = 0; j < g->N; ++j) scale += g->x[j] * (lm->lambda * g->x[j] + g->b[j]);
-    scale += 1e-3;
-    rho /= scale;
-    if (rho > 0 && isfinite(tempChi)) {
-      double alpha = 1. - pow((2 * rho - 1), 3);
-      alpha = alpha < (2. / 3.) ? alpha : (2. / 3.);
-      double scaleFactor = (1. / 3.) > alpha ? (1. / 3.) : alpha;
-      lm->lambda *= scaleFactor;
-      lm->ni = 2;
-      currentChi = tempChi;
-    } else {
-      lm->lambda *= lm->ni;
-      lm->ni *= 2;
+    if (!lm_decide_trial(&currentChi, lm, tempChi, scale, ok2, &qmax, &rho, &st->status, &stop)) {
       memcpy(g->rec, g->backup, sizeof(double) * 4 * (size_t)g->n); /* pop() */
       st->rejected++;
-      if (!isfinite(lm->lambda)) { st->status |= TEB_STATUS_NONFINITE; break; }
     }
-    qmax++;
-  } while (rho < 0 && qmax < 10);
+  } while (!stop);
   st->chi2_final = currentChi;
   st->lambda_final = lm->lambda;
   if (opt->verbose) fprintf(stderr, "LMTRIALS %d %d %.6g %.6g\n", iteration, qmax, currentChi, lm->lambda);
-  if (qmax == 10 || rho == 0 || !isfinite(lm->lambda)) return 0;
-  return 1;
+  return !lm_terminates(qmax, rho, lm);
 }
 
 /* SparseOptimizer::optimize(iterations) */
@@ -1882,6 +1917,42 @@ int32_t teb_oracle_build_system(const TebParams* cfg, const double* rec_in, int3
   graph_free(&g);
   free(rec);
   return N;
+}
+
+int32_t teb_oracle_trial_chi2(const TebParams* cfg, const double* rec_graph, int32_t n, const TebObstacle* obst, int32_t M,
+                              const double* via, int32_t V, const double* vel_start4, const double* vel_goal4,
+                              int32_t prefer_rotdir, double weight_multiplier, const double* rec_trials, int32_t T,
+                              double* chi_out, const double* obst_vertices) {
+  if (!cfg || !rec_graph || !chi_out || n < 3 || T < 0 || (T > 0 && !rec_trials)) return -1;
+  Graph g;
+  memset(&g, 0, sizeof(g));
+  double* rec = (double*)malloc(sizeof(double) * 4 * (size_t)n);
+  memcpy(rec, rec_graph, sizeof(double) * 4 * (size_t)n);
+  g.cfg = cfg; g.rec = rec; g.n = n; g.obst = obst; g.M = M; g.via = via; g.V = V; g.pverts = obst_vertices;
+  memcpy(g.vel_start, vel_start4, sizeof(double) * 4);
+  memcpy(g.vel_goal, vel_goal4, sizeof(double) * 4);
+  g.rotdir = prefer_rotdir;
+  graph_alloc(&g, n);
+  int rc = build_graph(&g, weight_multiplier);
+  if (rc) { graph_free(&g); free(rec); return rc; }
+  for (int t = 0; t < T; ++t) {
+    memcpy(rec, rec_trials + (size_t)t * 4 * n, sizeof(double) * 4 * (size_t)n);
+    long double fam[4] = {0, 0, 0, 0};
+    for (int k = 0; k < g.n_edges; ++k) {
+      Edge* e = g.edges[k];
+      e->compute_error(e, &g);
+      /* compute_current_cost's classification; the velocity-obstacle-ratio edge is one of the others */
+      const int f = (e->type == E_OBST || e->type == E_INFL || e->type == E_DYN) ? 0
+                    : e->type == E_VIA                                         ? 1
+                    : e->type == E_TIMEOPT                                     ? 2
+                                                                               : 3;
+      for (int d = 0; d < e->dim; ++d) fam[f] += (long double)e->err[d] * e->info[d] * e->err[d];
+    }
+    for (int f = 0; f < 4; ++f) chi_out[4 * (size_t)t + f] = (double)fam[f];
+  }
+  graph_free(&g);
+  free(rec);
+  return 0;
 }
 
 /* Per-edge dump of the graph buildGraph() produces at the given state, in insertion order, after computeActiveErrors

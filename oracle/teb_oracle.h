@@ -75,6 +75,25 @@ int32_t teb_oracle_dump_edges(const TebParams* cfg, const double* rec, int32_t n
                               int32_t prefer_rotdir, double weight_multiplier, int32_t jac_mode, double* rows,
                               int32_t max_rows, const double* obst_vertices);
 
+/* chi2 of LM trial states by the device's four families (obstacle / inflated / dynamic-obstacle edges, via-points,
+ * time-optimal, every other edge including the velocity-obstacle ratio), accumulated in long double. The graph is built
+ * once at rec_graph with the weight multiplier, which freezes the obstacle association, the dynamic-obstacle times and
+ * the via-point assignment; every edge's error is then evaluated at each of the T states rec_trials [T][n][4].
+ * chi_out [T][4]. Returns 0, or <0. */
+int32_t teb_oracle_trial_chi2(const TebParams* cfg, const double* rec_graph, int32_t n, const TebObstacle* obst, int32_t M,
+                              const double* via, int32_t V, const double* vel_start4, const double* vel_goal4,
+                              int32_t prefer_rotdir, double weight_multiplier, const double* rec_trials, int32_t T,
+                              double* chi_out, const double* obst_vertices);
+
+/* g2o's accept / reject chain of one LM iteration, the function teb_oracle_optimize's LM loop runs for every trial.
+ * From currentChi, lambda, nu and q0 trials already consumed in the iteration, it takes the trials k = 0 .. count-1
+ * (trial chi2 temp_chi[k], computeScale() sum scale_sum[k] without the 1e-3, ok[k] == 0: failed factorisation) while
+ * the iteration goes on. out_i: [0] accepted trial (last accepted k, or -1), [1] trials consumed, [2] Terminate,
+ * [3] TEB_STATUS_* bits added, [4] 1 when the iteration needs more trials than given, [5] trials of the iteration
+ * after these (q). out_d: lambda, nu, currentChi after them. Returns 0, or <0. */
+int32_t teb_oracle_lm_decide(double current_chi, double lambda, double nu, int32_t q0, int32_t count, const double* temp_chi,
+                             const double* scale_sum, const int32_t* ok, int32_t* out_i, double* out_d);
+
 /* TimedElasticBand::autoResize (timed_elastic_band.cpp:227-286). Returns new n. */
 int32_t teb_oracle_auto_resize(double* rec, int32_t n, int32_t n_cap, double dt_ref, double dt_hysteresis,
                                int32_t min_samples, int32_t max_samples, int32_t fast_mode);

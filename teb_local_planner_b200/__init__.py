@@ -85,6 +85,9 @@ def load_library(build_if_missing=False):
     L.tebgpu_solve_system.restype = C.c_int32
     L.tebgpu_solve_system.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32,
                                       vp, vp, vp]
+    L.tebgpu_eval_trials.restype = C.c_int32
+    L.tebgpu_eval_trials.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp,
+                                     C.c_int32, vp, vp, vp, vp, vp, vp, vp]
     L.tebgpu_select_best.restype = C.c_int32
     L.tebgpu_select_best.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double]
     L.tebgpu_auto_resize_host.restype = C.c_int32
@@ -265,6 +268,37 @@ class TebGpu:
                                                  0 if order is None else order.size, int(lat_cap), dx.ctypes.data,
                                                  ok.ctypes.data, lam_used.ctypes.data), "tebgpu_solve_system")
         return dx, ok, lam_used
+
+    EVAL_STATE = 14   # band state columns: lambda, nu, currentChi, chi2 by family (current 4, last trial 4), status,
+                      # active, LM iterations
+
+    def eval_trials(self, hb, K, dx, ok, lam, state, outer_index=0, iteration=1, qmax=None, order=None):
+        """One round of trial evaluation and g2o's accept / reject chain (tebgpu_eval_trials) on the graph and system
+        that build_system(hb, outer_index) makes. dx [B][K][4 n_cap], ok [B][K], lam [B][K]: the trials; state
+        [B][EVAL_STATE]: the band state before the round; qmax [B] + order (list of bands): a retry round over `order`.
+        hb.poses receives the state after the round. Returns dict(res [B][K][5], chi_lin [B][4], state [B][EVAL_STATE],
+        qmax [B], need [B], next_list)."""
+        import numpy as np
+        B, n_cap = hb.B, hb.n_cap
+        f64 = lambda a, shape: np.ascontiguousarray(np.broadcast_to(a, shape), dtype=np.float64)
+        dx, ok, lam = f64(dx, (B, K, 4 * n_cap)), f64(ok, (B, K)), f64(lam, (B, K))
+        state = f64(state, (B, self.EVAL_STATE))
+        qmax = None if qmax is None else np.ascontiguousarray(qmax, dtype=np.int32)
+        order = None if order is None else np.ascontiguousarray(order, dtype=np.int32)
+        res = np.empty((B, K, 5))
+        chi_lin = np.empty((B, 4))
+        st_out = np.empty((B, self.EVAL_STATE))
+        q_out = np.empty(B, np.int32)
+        need = np.empty(B, np.int32)
+        nxt = np.empty(B, np.int32)
+        nlen = C.c_int32(0)
+        bs = hb.struct()
+        self._check(self.lib.tebgpu_eval_trials(self.ctx, C.byref(bs), int(outer_index), int(iteration), int(K), dx.ctypes.data,
+                                                ok.ctypes.data, lam.ctypes.data, state.ctypes.data, abi.ptr(qmax),
+                                                abi.ptr(order), 0 if order is None else order.size, res.ctypes.data,
+                                                chi_lin.ctypes.data, st_out.ctypes.data, q_out.ctypes.data, need.ctypes.data,
+                                                nxt.ctypes.data, C.byref(nlen)), "tebgpu_eval_trials")
+        return dict(res=res, chi_lin=chi_lin, state=st_out, qmax=q_out, need=need, next_list=nxt[:nlen.value].copy())
 
     def close(self):
         if self.ctx:

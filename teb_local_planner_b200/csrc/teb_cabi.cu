@@ -1320,6 +1320,140 @@ int32_t tebgpu_solve_system(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, const dou
   return TEBGPU_OK;
 }
 
+int32_t tebgpu_eval_trials(tebgpu_ctx* ctx, TebBatch* bt, int32_t outer_index, int32_t iteration, int32_t K, const double* dx,
+                           const double* ok, const double* lambda_k, const double* state, const int32_t* qmax,
+                           const int32_t* list, int32_t list_len, double* res_out, double* chi_lin, double* state_out,
+                           int32_t* qmax_out, int32_t* need_out, int32_t* next_list, int32_t* next_len) {
+  int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  if (!dx || !ok || !lambda_k || !state || outer_index < 0 || iteration < 0) return TEBGPU_ERR_INVALID_ARG;
+  if (!(K == 2 || K == 4 || K == 6 || K == 8)) { ctx->err = "bad speculation width"; return TEBGPU_ERR_INVALID_ARG; }
+  rc = check_path(ctx, bt, true);
+  if (rc) return rc;
+  const int B = bt->B, n_cap = bt->n_cap;
+  const bool retry = qmax != nullptr;
+  for (int b = 0; b < B; ++b)
+    if (bt->n[b] < 3 || bt->n[b] > n_cap) { ctx->err = "n[b] outside 3 .. n_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  if (retry) {
+    if (!list || list_len < 0 || list_len > B) { ctx->err = "a retry round needs its list"; return TEBGPU_ERR_INVALID_ARG; }
+    std::vector<char> seen((size_t)B, 0);
+    for (int s = 0; s < list_len; ++s) {
+      const int b = list[s];
+      if (b < 0 || b >= B || seen[b] || qmax[b] < 0 || qmax[b] > 10) { ctx->err = "bad retry list"; return TEBGPU_ERR_INVALID_ARG; }
+      seen[b] = 1;
+    }
+  }
+  const size_t smem = eval_bytes(ctx, n_cap, bt->M_cap, K);
+  if (smem > 232448) { ctx->err = "trial-evaluation staging exceeds shared memory"; return TEBGPU_ERR_CAPACITY; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  rc = upload_batch(ctx, bt);
+  if (rc) return rc;
+  TebBatch d = mirror_batch(ctx, bt);
+  cudaStream_t st = ctx->stream;
+  DevBatch db = make_devbatch(ctx, &d);
+  double mult = 1.0;
+  for (int o = 0; o < outer_index; ++o) mult *= ctx->params.weight_adapt_factor;
+  KParams kp = make_kparams(ctx, bt, mult);
+  const int tb = 128, gb = ((B > bt->S ? B : bt->S) + tb - 1) / tb;
+  const size_t smem_g = (size_t)(bt->M_cap > 0 ? bt->M_cap : 1) * sizeof(TebObstacle);
+  k_begin<<<gb, tb, 0, st>>>(db, kp);
+  launch_build_graph(db, kp, B, smem_g, st);
+  launch_linearize(ctx, db, kp, B, bt->M_cap, st);
+  if (kp.has_vor) launch_vor(db, kp, B, smem_g, st);
+  /* the band state before the round replaces what buildGraph set (kernel A above ran for every band) */
+  std::vector<BandState> bs((size_t)B);
+  for (int b = 0; b < B; ++b) {
+    const double* s = state + (size_t)b * TEBGPU_EVAL_STATE;
+    BandState& x = bs[b];
+    std::memset(&x, 0, sizeof(x));
+    x.lambda = s[0]; x.ni = s[1]; x.current_chi = s[2]; x.chi2_final = s[2];
+    for (int c = 0; c < 4; ++c) { x.parts_cur[c] = s[3 + c]; x.parts_last[c] = s[7 + c]; }
+    x.status = (int32_t)s[11]; x.active = s[12] != 0; x.lm_iters = (int32_t)s[13];
+  }
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->state, bs.data(), (size_t)B * sizeof(BandState), cudaMemcpyHostToDevice, st));
+  /* the trials, in the solver's interleaved scratch: system K slot + k in lane & 31 of warp >> 5, row r at r * 32, slot =
+   * band (round 0) or list position; res rows 0 .. 4 all-ones (a NaN), res[5] / res[6] what the solve wrote */
+  SpecBufs spec = ctx->spec;
+  spec.K = K; spec.sel_list = nullptr; spec.sel_cnt = nullptr; spec.defer = nullptr; spec.skip_tag = 0; spec.lat_cap = 0;
+  const int round = retry ? 1 : 0, g = retry ? 1 : 0; /* retry rounds read list g % SPEC_LISTS and its length cnt[g] */
+  const int slots = retry ? list_len : B;
+  const size_t rows = (size_t)4 * n_cap;
+  const size_t sys = (((size_t)B * K + 31) / 32) * 32;
+  std::vector<double> hdx(sys * rows), hres((size_t)B * SPEC_K_MAX * RES_STRIDE);
+  std::memset(hdx.data(), 0xff, hdx.size() * sizeof(double));
+  std::memset(hres.data(), 0xff, hres.size() * sizeof(double));
+  for (int s = 0; s < slots; ++s) {
+    const int b = retry ? list[s] : s;
+    for (int k = 0; k < K; ++k) {
+      const size_t t = (size_t)K * s + k;
+      const double* src = dx + ((size_t)b * K + k) * rows;
+      double* dst = hdx.data() + (t >> 5) * 32 * rows + (t & 31);
+      for (size_t r = 0; r < rows; ++r) dst[r * 32] = src[r];
+    }
+  }
+  for (int b = 0; b < B; ++b)
+    for (int k = 0; k < K; ++k) {
+      hres[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + 5] = ok[(size_t)b * K + k];
+      hres[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + 6] = lambda_k[(size_t)b * K + k];
+    }
+  CUDA_TRY(ctx, cudaMemcpyAsync(spec.dx, hdx.data(), hdx.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(spec.res, hres.data(), hres.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemsetAsync(spec.need, 0xff, (size_t)B * sizeof(int32_t), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(spec.cnt, 0, 3 * sizeof(int32_t), st)); /* list lengths of rounds 0 .. 2 */
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->defer, 0, (size_t)B * sizeof(int32_t), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->arrive, 0, (size_t)B * sizeof(int32_t), st));
+  if (retry) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(spec.qmax, qmax, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (list_len > 0)
+      CUDA_TRY(ctx, cudaMemcpyAsync(spec.list + (size_t)(g % SPEC_LISTS) * B, list, (size_t)list_len * sizeof(int32_t),
+                                    cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(spec.cnt + g, &list_len, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  } else {
+    CUDA_TRY(ctx, cudaMemsetAsync(spec.qmax, 0xff, (size_t)B * sizeof(int32_t), st));
+  }
+  launch_trial_eval(ctx, spec, db, kp, B, K, smem, iteration, round, g, 1, st);
+  ctx->launches = 4 + (kp.has_vor ? 1 : 0);
+  CUDA_TRY(ctx, cudaGetLastError());
+  std::vector<double> parts((size_t)B * db.chunks * 4);
+  std::vector<int32_t> hq((size_t)B), hneed((size_t)B), hlist((size_t)B);
+  int32_t hcnt = 0;
+  CUDA_TRY(ctx, cudaMemcpyAsync(hres.data(), spec.res, hres.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(parts.data(), ctx->chi_parts, parts.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(bs.data(), ctx->state, (size_t)B * sizeof(BandState), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(hq.data(), spec.qmax, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(hneed.data(), spec.need, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(hlist.data(), spec.list + (size_t)((g + 1) % SPEC_LISTS) * B, (size_t)B * sizeof(int32_t),
+                                cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(&hcnt, spec.cnt + g + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(bt->poses, ctx->d_poses, (size_t)B * n_cap * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  for (int b = 0; b < B; ++b) {
+    if (res_out)
+      for (int k = 0; k < K; ++k)
+        for (int c = 0; c < 5; ++c) res_out[((size_t)b * K + k) * 5 + c] = hres[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + c];
+    if (chi_lin) { /* spec_decide's sum: the used tiles in order, family by family */
+      double cur[4] = {0, 0, 0, 0};
+      const int used = (bt->n[b] + db.tile - 1) / db.tile;
+      for (int ch = 0; ch < used; ++ch)
+        for (int c = 0; c < 4; ++c) cur[c] += parts[((size_t)b * db.chunks + ch) * 4 + c];
+      for (int c = 0; c < 4; ++c) chi_lin[(size_t)b * 4 + c] = cur[c];
+    }
+    if (state_out) {
+      double* s = state_out + (size_t)b * TEBGPU_EVAL_STATE;
+      const BandState& x = bs[b];
+      s[0] = x.lambda; s[1] = x.ni; s[2] = x.current_chi;
+      for (int c = 0; c < 4; ++c) { s[3 + c] = x.parts_cur[c]; s[7 + c] = x.parts_last[c]; }
+      s[11] = x.status; s[12] = x.active; s[13] = x.lm_iters;
+    }
+    if (qmax_out) qmax_out[b] = hq[b];
+    if (need_out) need_out[b] = hneed[b];
+  }
+  if (next_len) *next_len = hcnt;
+  if (next_list)
+    for (int s = 0; s < hcnt && s < B; ++s) next_list[s] = hlist[s];
+  return TEBGPU_OK;
+}
+
 /* ------------------------------------------------------------------ the one collective: all-gather of the costs */
 #define NCCL_TRY(ctx, expr)                                                                              \
   do {                                                                                                   \

@@ -855,6 +855,9 @@ __global__ void __launch_bounds__(32 * SPEC_K_MAX, MINB) k_trial_eval(DevBatch d
     r[0] = chi[0]; r[1] = chi[1]; r[2] = chi[2]; r[3] = chi[3];
     r[4] = scl;
     r[5] = ok ? 1.0 : 0.0;
+    /* the trial's row is published as k_trial_eval3 publishes it (read by tebgpu_eval_trials only) */
+    double* gr = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
+    gr[0] = chi[0]; gr[1] = chi[1]; gr[2] = chi[2]; gr[3] = chi[3]; gr[4] = scl;
   }
   __syncthreads();
 
@@ -1138,6 +1141,8 @@ __global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_t
   }
   __syncthreads();
   if (tid < kact) { /* fold the tile partials of trial tid in tile order */
+    double* gr = sp.res + ((size_t)b * SPEC_K_MAX + tid) * RES_STRIDE;
+    const double okv = gr[5];
     double a[5] = {0, 0, 0, 0, 0};
     for (int t = 0; t < tiles; ++t) {
       const double* pp = sPart + ((size_t)tid * ev2_tiles(db.n_cap) + t) * 5;
@@ -1146,7 +1151,10 @@ __global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_t
     }
     double* r = sRes + tid * RES_STRIDE;
     r[0] = a[0]; r[1] = a[1]; r[2] = a[2]; r[3] = a[3]; r[4] = a[4];
-    r[5] = sp.res[((size_t)b * SPEC_K_MAX + tid) * RES_STRIDE + 5];
+    r[5] = okv;
+    /* the trial's row is published as k_trial_eval3 publishes it (read by tebgpu_eval_trials only) */
+#pragma unroll
+    for (int c = 0; c < 5; ++c) gr[c] = a[c];
   }
   __syncthreads();
   /* ---- accept / reject replay, sequential over the K trials */

@@ -193,6 +193,51 @@ def dump_edges(params, rec, n, obstacles, via=None, vel_start=None, vel_goal=Non
     return rows[:ne]
 
 
+def trial_chi2(params, rec_graph, n, trials, obstacles, via=None, vel_start=None, vel_goal=None, rotdir=0,
+               weight_multiplier=1.0, obst_vertices=None):
+    """chi2 by family (obstacles, via, time-optimal, other) [T][4] of the trial states trials [T][>= n][4], with the graph
+    built at rec_graph (association, dynamic-obstacle times and via-points frozen there)"""
+    L = lib()
+    L.teb_oracle_trial_chi2.restype = C.c_int32
+    L.teb_oracle_trial_chi2.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                        C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_int32, C.c_void_p,
+                                        C.c_void_p]
+    rec = np.ascontiguousarray(rec_graph[:n], dtype=np.float64)
+    tr = np.ascontiguousarray(np.asarray(trials, dtype=np.float64)[:, :n])
+    obstacles = np.ascontiguousarray(obstacles, dtype=abi.OBST_DTYPE)
+    via = np.zeros((0, 2)) if via is None else np.ascontiguousarray(via, dtype=np.float64)
+    vs = np.array([0, 0, 0, 1.0]) if vel_start is None else np.ascontiguousarray(vel_start, dtype=np.float64)
+    vg = np.array([0, 0, 0, 1.0]) if vel_goal is None else np.ascontiguousarray(vel_goal, dtype=np.float64)
+    out = np.zeros((tr.shape[0], 4))
+    rc = L.teb_oracle_trial_chi2(C.addressof(params), rec.ctypes.data, n, obstacles.ctypes.data if len(obstacles) else None,
+                                 len(obstacles), via.ctypes.data if len(via) else None, len(via), vs.ctypes.data,
+                                 vg.ctypes.data, int(rotdir), float(weight_multiplier), tr.ctypes.data, tr.shape[0],
+                                 out.ctypes.data, _verts(obst_vertices)[1])
+    if rc != 0:
+        raise RuntimeError(f"teb_oracle_trial_chi2 rc={rc}")
+    return out
+
+
+def lm_decide(current_chi, lam, nu, q0, temp_chi, scale_sum, ok):
+    """g2o's accept / reject chain over a sequence of trials -> dict(accepted, used, terminate, status, need, q, lambda,
+    nu, current_chi)"""
+    L = lib()
+    L.teb_oracle_lm_decide.restype = C.c_int32
+    L.teb_oracle_lm_decide.argtypes = [C.c_double, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]
+    tc = np.ascontiguousarray(temp_chi, dtype=np.float64)
+    sc = np.ascontiguousarray(scale_sum, dtype=np.float64)
+    okk = np.ascontiguousarray(ok, dtype=np.int32)
+    oi = np.zeros(6, np.int32)
+    od = np.zeros(3)
+    rc = L.teb_oracle_lm_decide(float(current_chi), float(lam), float(nu), int(q0), tc.size, tc.ctypes.data, sc.ctypes.data,
+                                okk.ctypes.data, oi.ctypes.data, od.ctypes.data)
+    if rc != 0:
+        raise RuntimeError(f"teb_oracle_lm_decide rc={rc}")
+    return dict(accepted=int(oi[0]), used=int(oi[1]), terminate=bool(oi[2]), status=int(oi[3]), need=bool(oi[4]),
+                q=int(oi[5]), lam=float(od[0]), nu=float(od[1]), current_chi=float(od[2]))
+
+
 def auto_resize(rec, n, dt_ref, dt_hyst, min_samples, max_samples, fast_mode, n_cap=None):
     L = lib()
     n_cap = max(rec.shape[0], 4 * n) if n_cap is None else n_cap
