@@ -346,6 +346,23 @@ int32_t tebgpu_solve_system(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, const dou
                             const int32_t* list, int32_t list_len, int32_t lat_cap, double* dx_out, double* ok_out,
                             double* lambda_out);
 
+/* Graph build + kernel A readout: the launches of tebgpu_build_system (k_begin, k_build_graph, kernel A, k_vor) with
+ * the graph structure exposed. Test / profiling entry point of the graph build and of kernel A. HOST buffers.
+ *   list, list_len       NULL: every band. Otherwise k_build_graph and kernel A run over the bands of `list` as the
+ *                        retry side stream launches them (DevBatch::a_list / a_cnt, grids over the whole batch);
+ *                        k_begin still runs for every band. Refused with a velocity-obstacle ratio weight (k_vor has no
+ *                        list form).
+ * Before the launches, Hb, rhs, the association, multiplicity-3 and occupancy words, via_idx, dyn_t and the tile
+ * partials are filled with all-ones bytes (a NaN); what no kernel wrote comes back as that pattern.
+ * Outputs (any may be NULL): Hb_out [B][4 n_cap][12]; chi_fam_out [B][4] kernel A's chi2 by family (obstacles, via,
+ * time-optimal, other) folded as tebgpu_eval_trials folds its chi_lin, all-ones for a band not listed;
+ * assoc_out, assoc3_out [B][n_cap][MW] (MW = max(1, ceil(M_cap / 64))); occ_out [B][n_cap][ceil(MW / 64)] (written
+ * on the global-table path only, M_cap > 1024); via_idx_out [B][V_cap] (pose of each via-point, -1 skipped);
+ * dyn_t_out [B][n_cap] (frozen dynamic-obstacle time of each pose). */
+int32_t tebgpu_build_system_graph(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_index, const int32_t* list,
+                                  int32_t list_len, double* Hb_out, double* chi_fam_out, uint64_t* assoc_out,
+                                  uint64_t* assoc3_out, uint64_t* occ_out, int32_t* via_idx_out, double* dyn_t_out);
+
 /* Trial evaluation only: one round of the speculative LM step's trial evaluation and accept / reject chain, launched by
  * the same code as in tebgpu_optimize_batch (the kernel TEBGPU_EVAL_V1 / TEBGPU_EVAL3 and the batch size select). Test /
  * profiling entry point of the trial-evaluation kernels. The graph, right-hand side and kernel A's chi2 / max-diagonal

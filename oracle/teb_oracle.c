@@ -1955,6 +1955,53 @@ int32_t teb_oracle_trial_chi2(const TebParams* cfg, const double* rec_graph, int
   return 0;
 }
 
+int32_t teb_oracle_graph(const TebParams* cfg, const double* rec_in, int32_t n, const TebObstacle* obst, int32_t M,
+                         const double* via, int32_t V, const double* vel_start4, const double* vel_goal4,
+                         int32_t prefer_rotdir, double weight_multiplier, int32_t MW, uint64_t* assoc_out,
+                         uint64_t* assoc3_out, int32_t* via_idx_out, double* dyn_t_out, const double* obst_vertices) {
+  if (!cfg || !rec_in || n < 3 || M < 0 || MW < (M + 63) / 64 || MW < 1) return -1;
+  Graph g;
+  memset(&g, 0, sizeof(g));
+  double* rec = (double*)malloc(sizeof(double) * 4 * (size_t)n);
+  memcpy(rec, rec_in, sizeof(double) * 4 * (size_t)n);
+  g.cfg = cfg; g.rec = rec; g.n = n; g.obst = obst; g.M = M; g.via = via; g.V = V; g.pverts = obst_vertices;
+  memcpy(g.vel_start, vel_start4, sizeof(double) * 4);
+  memcpy(g.vel_goal, vel_goal4, sizeof(double) * 4);
+  g.rotdir = prefer_rotdir;
+  graph_alloc(&g, n);
+  int rc = build_graph(&g, weight_multiplier);
+  if (rc) { graph_free(&g); free(rec); return rc; }
+  /* obstacle / inflated edges per (pose, obstacle): 1, or 3 on the legacy centre pose */
+  int* cnt = (int*)calloc((size_t)n * (M > 0 ? M : 1), sizeof(int));
+  if (assoc_out) memset(assoc_out, 0, sizeof(uint64_t) * (size_t)n * MW);
+  if (assoc3_out) memset(assoc3_out, 0, sizeof(uint64_t) * (size_t)n * MW);
+  if (via_idx_out)
+    for (int v = 0; v < V; ++v) via_idx_out[v] = -1;
+  if (dyn_t_out)
+    for (int i = 0; i < n; ++i) dyn_t_out[i] = NAN;
+  for (int k = 0; k < g.n_edges; ++k) {
+    const Edge* e = g.edges[k];
+    const int i = e->vidx[0];
+    if (e->type == E_OBST || e->type == E_INFL || e->type == E_VEL_OBST_RATIO) {
+      const int m = (int)(e->ob - obst);
+      if (assoc_out) assoc_out[(size_t)i * MW + (m >> 6)] |= 1ull << (m & 63);
+      if (e->type != E_VEL_OBST_RATIO) ++cnt[(size_t)i * M + m];
+    } else if (e->type == E_VIA) {
+      if (via_idx_out) via_idx_out[(e->via - via) / 2] = i;
+    } else if (e->type == E_DYN) {
+      if (dyn_t_out) dyn_t_out[i] = e->t;
+    }
+  }
+  if (assoc3_out)
+    for (int i = 0; i < n; ++i)
+      for (int m = 0; m < M; ++m)
+        if (cnt[(size_t)i * M + m] == 3) assoc3_out[(size_t)i * MW + (m >> 6)] |= 1ull << (m & 63);
+  free(cnt);
+  graph_free(&g);
+  free(rec);
+  return 0;
+}
+
 /* Per-edge dump of the graph buildGraph() produces at the given state, in insertion order, after computeActiveErrors
  * and linearisation: rows of 64 doubles, same layout as oracle/ref_driver.cpp's teb_ref_build_system(edges_out):
  * [0] error dimension, [1] vertex count, [2..4] error, [5..7] information diagonal, [8 + 9 k ...] Jacobian of vertex k

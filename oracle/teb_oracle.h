@@ -85,6 +85,17 @@ int32_t teb_oracle_trial_chi2(const TebParams* cfg, const double* rec_graph, int
                               int32_t prefer_rotdir, double weight_multiplier, const double* rec_trials, int32_t T,
                               double* chi_out, const double* obst_vertices);
 
+/* The structure buildGraph() gives the band at rec with the weight multiplier, read off the active edges:
+ * assoc_out [n][MW] bit m of pose i for an obstacle / inflated-obstacle edge on pose i whose obstacle is obst[m] (and,
+ * with the velocity-obstacle ratio, for the ratio edges anchored at pose i, which carry pose 0's association);
+ * assoc3_out [n][MW] bit m where pose i carries three such edges (the legacy centre pose); via_idx_out [V] the pose of
+ * each via-point's edge, -1 where it has none; dyn_t_out [n] the frozen time t of pose i's dynamic-obstacle edges, NaN
+ * where it has none. MW >= ceil(M / 64). Returns 0, or <0. */
+int32_t teb_oracle_graph(const TebParams* cfg, const double* rec, int32_t n, const TebObstacle* obst, int32_t M,
+                         const double* via, int32_t V, const double* vel_start4, const double* vel_goal4,
+                         int32_t prefer_rotdir, double weight_multiplier, int32_t MW, uint64_t* assoc_out,
+                         uint64_t* assoc3_out, int32_t* via_idx_out, double* dyn_t_out, const double* obst_vertices);
+
 /* g2o's accept / reject chain of one LM iteration, the function teb_oracle_optimize's LM loop runs for every trial.
  * From currentChi, lambda, nu and q0 trials already consumed in the iteration, it takes the trials k = 0 .. count-1
  * (trial chi2 temp_chi[k], computeScale() sum scale_sum[k] without the 1e-3, ok[k] == 0: failed factorisation) while

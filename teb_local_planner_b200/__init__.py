@@ -82,6 +82,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_h_signature.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, C.c_int32]
     L.tebgpu_build_system.restype = C.c_int32
     L.tebgpu_build_system.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, vp, C.c_int32]
+    L.tebgpu_build_system_graph.restype = C.c_int32
+    L.tebgpu_build_system_graph.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp]
     L.tebgpu_solve_system.restype = C.c_int32
     L.tebgpu_solve_system.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32,
                                       vp, vp, vp]
@@ -233,9 +235,29 @@ class TebGpu:
     def launch_count(self):
         return int(self.lib.tebgpu_last_launch_count(self.ctx))
 
-    def build_system(self, hb, outer_index=0):
-        """Returns (Hb [B][4*n_cap][12], chi2 [B]) as numpy arrays (host-buffer path)."""
+    def build_system(self, hb, outer_index=0, bands=None, graph=False):
+        """Returns (Hb [B][4*n_cap][12], chi2 [B]) as numpy arrays (host-buffer path).
+
+        With bands (a list of band indices: k_build_graph and kernel A run over that list as the retry side stream runs
+        them) or graph=True, runs tebgpu_build_system_graph instead and returns dict(Hb, chi_fam [B][4] (obstacles, via,
+        time-optimal, other), assoc, assoc3 [B][n_cap][MW] uint64, occ [B][n_cap][OW] uint64, via_idx [B][V_cap],
+        dyn_t [B][n_cap]); everything starts as all-ones bytes, so what no kernel wrote keeps that pattern."""
         import numpy as np
+        if bands is not None or graph:
+            B, n_cap = hb.B, hb.n_cap
+            MW = max(1, (hb.M_cap + 63) // 64)
+            OW = (MW + 63) // 64
+            order = None if bands is None else np.ascontiguousarray(bands, dtype=np.int32)
+            out = dict(Hb=np.empty((B, 4 * n_cap, 12)), chi_fam=np.empty((B, 4)),
+                       assoc=np.empty((B, n_cap, MW), np.uint64), assoc3=np.empty((B, n_cap, MW), np.uint64),
+                       occ=np.empty((B, n_cap, OW), np.uint64), via_idx=np.empty((B, hb.V_cap), np.int32),
+                       dyn_t=np.empty((B, n_cap)))
+            bs = hb.struct()
+            self._check(self.lib.tebgpu_build_system_graph(
+                self.ctx, C.byref(bs), int(outer_index), abi.ptr(order), 0 if order is None else order.size,
+                *(out[k].ctypes.data for k in ("Hb", "chi_fam", "assoc", "assoc3", "occ", "via_idx", "dyn_t"))),
+                "tebgpu_build_system_graph")
+            return out
         Hb = np.zeros((hb.B, 4 * hb.n_cap, 12))
         chi2 = np.zeros(hb.B)
         bs = hb.struct()

@@ -1223,6 +1223,95 @@ int32_t tebgpu_build_system(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_i
   return TEBGPU_OK;
 }
 
+/* kernel A's chi2 by family of band b (obstacles, via, time-optimal, other): spec_decide's sum, the used tiles in
+ * order, family by family, over the host copy of the tile partials */
+static void fold_chi_parts(const double* parts, const DevBatch& db, int b, int n, double* out4) {
+  double cur[4] = {0, 0, 0, 0};
+  const int used = (n + db.tile - 1) / db.tile;
+  for (int ch = 0; ch < used; ++ch)
+    for (int c = 0; c < 4; ++c) cur[c] += parts[((size_t)b * db.chunks + ch) * 4 + c];
+  for (int c = 0; c < 4; ++c) out4[c] = cur[c];
+}
+
+int32_t tebgpu_build_system_graph(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_index, const int32_t* list,
+                                  int32_t list_len, double* Hb_out, double* chi_fam_out, uint64_t* assoc_out,
+                                  uint64_t* assoc3_out, uint64_t* occ_out, int32_t* via_idx_out, double* dyn_t_out) {
+  int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  if (outer_index < 0) return TEBGPU_ERR_INVALID_ARG;
+  rc = check_path(ctx, bt, false);
+  if (rc) return rc;
+  const int B = bt->B, n_cap = bt->n_cap;
+  if (list) {
+    if (list_len < 0 || list_len > B) { ctx->err = "bad band list"; return TEBGPU_ERR_INVALID_ARG; }
+    std::vector<char> seen((size_t)B, 0);
+    for (int s = 0; s < list_len; ++s) {
+      const int b = list[s];
+      if (b < 0 || b >= B || seen[b]) { ctx->err = "bad band list"; return TEBGPU_ERR_INVALID_ARG; }
+      seen[b] = 1;
+    }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  rc = upload_batch(ctx, bt);
+  if (rc) return rc;
+  TebBatch d = mirror_batch(ctx, bt);
+  cudaStream_t st = ctx->stream;
+  DevBatch db = make_devbatch(ctx, &d);
+  double mult = 1.0;
+  for (int o = 0; o < outer_index; ++o) mult *= ctx->params.weight_adapt_factor;
+  KParams kp = make_kparams(ctx, bt, mult);
+  /* k_vor takes blockIdx.x as the band and has no list form; optimize never forks the side stream when it runs */
+  if (list && kp.has_vor) { ctx->err = "a band list cannot be combined with the velocity-obstacle ratio"; return TEBGPU_ERR_INVALID_ARG; }
+  /* everything the graph build and kernel A write starts as all-ones bytes (a NaN), so what no kernel wrote shows */
+  const size_t hb_len = (size_t)B * 4 * n_cap * HROW, aw = (size_t)B * n_cap * db.MW, ow = (size_t)B * n_cap * db.OW;
+  const size_t vl = (size_t)B * (bt->V_cap > 0 ? bt->V_cap : 0), parts_len = (size_t)B * db.chunks * 4;
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->Hb, 0xff, hb_len * sizeof(double), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->rhs, 0xff, (size_t)B * 4 * n_cap * sizeof(double), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->assoc, 0xff, aw * sizeof(uint64_t), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->assoc3, 0xff, aw * sizeof(uint64_t), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->occ, 0xff, ow * sizeof(uint64_t), st));
+  if (vl) CUDA_TRY(ctx, cudaMemsetAsync(ctx->via_idx, 0xff, vl * sizeof(int32_t), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->dyn_t, 0xff, (size_t)B * n_cap * sizeof(double), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->chi_parts, 0xff, parts_len * sizeof(double), st));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->dmax_parts, 0xff, (size_t)B * db.chunks * sizeof(double), st));
+  const int tb = 128, gb = ((B > bt->S ? B : bt->S) + tb - 1) / tb;
+  const size_t smem_g = (size_t)(bt->M_cap > 0 ? bt->M_cap : 1) * sizeof(TebObstacle);
+  k_begin<<<gb, tb, 0, st>>>(db, kp);
+  DevBatch dl = db;
+  if (list) { /* the side stream's form: the list and its length in device memory, grids over the whole batch */
+    if (list_len > 0)
+      CUDA_TRY(ctx, cudaMemcpyAsync(ctx->spec.list, list, (size_t)list_len * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->spec.cnt, &list_len, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    dl.a_list = ctx->spec.list;
+    dl.a_cnt = ctx->spec.cnt;
+  }
+  launch_build_graph(dl, kp, B, smem_g, st);
+  launch_linearize(ctx, dl, kp, B, bt->M_cap, st);
+  if (kp.has_vor) launch_vor(db, kp, B, smem_g, st);
+  ctx->launches = 3 + (kp.has_vor ? 1 : 0);
+  CUDA_TRY(ctx, cudaGetLastError());
+  std::vector<double> parts(parts_len);
+  CUDA_TRY(ctx, cudaMemcpyAsync(parts.data(), ctx->chi_parts, parts_len * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (Hb_out) CUDA_TRY(ctx, cudaMemcpyAsync(Hb_out, ctx->Hb, hb_len * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (assoc_out) CUDA_TRY(ctx, cudaMemcpyAsync(assoc_out, ctx->assoc, aw * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  if (assoc3_out) CUDA_TRY(ctx, cudaMemcpyAsync(assoc3_out, ctx->assoc3, aw * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  if (occ_out) CUDA_TRY(ctx, cudaMemcpyAsync(occ_out, ctx->occ, ow * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  if (via_idx_out && vl) CUDA_TRY(ctx, cudaMemcpyAsync(via_idx_out, ctx->via_idx, vl * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (dyn_t_out) CUDA_TRY(ctx, cudaMemcpyAsync(dyn_t_out, ctx->dyn_t, (size_t)B * n_cap * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  if (chi_fam_out) {
+    /* a band no kernel linearised (not listed, or not active) keeps the all-ones pattern */
+    std::vector<char> ran((size_t)B, list ? 0 : 1);
+    if (list)
+      for (int s = 0; s < list_len; ++s) ran[list[s]] = 1;
+    for (int b = 0; b < B; ++b) {
+      if (ran[b]) fold_chi_parts(parts.data(), db, b, bt->n[b], chi_fam_out + (size_t)b * 4);
+      else std::memset(chi_fam_out + (size_t)b * 4, 0xff, 4 * sizeof(double));
+    }
+  }
+  return TEBGPU_OK;
+}
+
 int32_t tebgpu_solve_system(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, const double* Hb, const int32_t* n,
                             const double* lambda, const double* nu, const int32_t* active, int32_t K, const int32_t* qmax,
                             const int32_t* list, int32_t list_len, int32_t lat_cap, double* dx_out, double* ok_out,
@@ -1431,13 +1520,7 @@ int32_t tebgpu_eval_trials(tebgpu_ctx* ctx, TebBatch* bt, int32_t outer_index, i
     if (res_out)
       for (int k = 0; k < K; ++k)
         for (int c = 0; c < 5; ++c) res_out[((size_t)b * K + k) * 5 + c] = hres[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + c];
-    if (chi_lin) { /* spec_decide's sum: the used tiles in order, family by family */
-      double cur[4] = {0, 0, 0, 0};
-      const int used = (bt->n[b] + db.tile - 1) / db.tile;
-      for (int ch = 0; ch < used; ++ch)
-        for (int c = 0; c < 4; ++c) cur[c] += parts[((size_t)b * db.chunks + ch) * 4 + c];
-      for (int c = 0; c < 4; ++c) chi_lin[(size_t)b * 4 + c] = cur[c];
-    }
+    if (chi_lin) fold_chi_parts(parts.data(), db, b, bt->n[b], chi_lin + (size_t)b * 4);
     if (state_out) {
       double* s = state_out + (size_t)b * TEBGPU_EVAL_STATE;
       const BandState& x = bs[b];

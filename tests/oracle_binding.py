@@ -218,6 +218,33 @@ def trial_chi2(params, rec_graph, n, trials, obstacles, via=None, vel_start=None
     return out
 
 
+def graph(params, rec, n, obstacles, via=None, vel_start=None, vel_goal=None, rotdir=0, weight_multiplier=1.0,
+          obst_vertices=None, MW=None):
+    """the structure buildGraph() gives the band (teb_oracle_graph) -> dict(assoc [n][MW] uint64, assoc3 [n][MW] uint64,
+    via_idx [V] (-1: no edge), dyn_t [n] (NaN: no dynamic-obstacle edge on the pose))"""
+    L = lib()
+    L.teb_oracle_graph.restype = C.c_int32
+    L.teb_oracle_graph.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                   C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p]
+    rec = np.ascontiguousarray(rec[:n], dtype=np.float64)
+    obstacles = np.ascontiguousarray(obstacles, dtype=abi.OBST_DTYPE)
+    via = np.zeros((0, 2)) if via is None else np.ascontiguousarray(via, dtype=np.float64)
+    vs = np.array([0, 0, 0, 1.0]) if vel_start is None else np.ascontiguousarray(vel_start, dtype=np.float64)
+    vg = np.array([0, 0, 0, 1.0]) if vel_goal is None else np.ascontiguousarray(vel_goal, dtype=np.float64)
+    MW = max(1, (len(obstacles) + 63) // 64) if MW is None else MW
+    out = dict(assoc=np.zeros((n, MW), np.uint64), assoc3=np.zeros((n, MW), np.uint64),
+               via_idx=np.zeros(len(via), np.int32), dyn_t=np.zeros(n))
+    rc = L.teb_oracle_graph(C.addressof(params), rec.ctypes.data, n, obstacles.ctypes.data if len(obstacles) else None,
+                            len(obstacles), via.ctypes.data if len(via) else None, len(via), vs.ctypes.data, vg.ctypes.data,
+                            int(rotdir), float(weight_multiplier), int(MW), out["assoc"].ctypes.data,
+                            out["assoc3"].ctypes.data, out["via_idx"].ctypes.data, out["dyn_t"].ctypes.data,
+                            _verts(obst_vertices)[1])
+    if rc != 0:
+        raise RuntimeError(f"teb_oracle_graph rc={rc}")
+    return out
+
+
 def lm_decide(current_chi, lam, nu, q0, temp_chi, scale_sum, ok):
     """g2o's accept / reject chain over a sequence of trials -> dict(accepted, used, terminate, status, need, q, lambda,
     nu, current_chi)"""
