@@ -269,18 +269,24 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
     if (const char* e = std::getenv("TEBGPU_EVAL_V1")) c->eval_v1 = std::atoi(e) != 0;
     size_t ev2 = eval2_smem_bytes((int)nc, (int)Ms, SPEC_K_MAX);
     if (ev2 > 232448) ev2 = 232448;
-#define EV2_ATTR(G, T)                                                                                                  \
-  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev2));          \
-  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    EV2_ATTR(false, 256) EV2_ATTR(true, 256) EV2_ATTR(false, 512) EV2_ATTR(true, 512)
+#define EV2_ATTR(G)                                                                                                  \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev2));          \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    EV2_ATTR(false) EV2_ATTR(true)
     size_t ev2g = eval2_smem_bytes((int)nc, 0, SPEC_K_MAX);
     if (ev2g > 232448) ev2g = 232448;
-#define EV2G_ATTR(G, T)                                                                                                 \
-  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev2g));   \
-  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, T, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    EV2G_ATTR(false, 256) EV2G_ATTR(true, 256) EV2G_ATTR(false, 512) EV2G_ATTR(true, 512)
+#define EV2G_ATTR(G)                                                                                                 \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev2g));   \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2<G, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    EV2G_ATTR(false) EV2G_ATTR(true)
 #undef EV2G_ATTR
 #undef EV2_ATTR
+    /* the persistent build: the same shared memory as k_trial_eval2 */
+#define EVP_ATTR(G, T, BYTES)                                                                                           \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2p<G, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(BYTES)));      \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval2p<G, T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    EVP_ATTR(false, false, ev2) EVP_ATTR(true, false, ev2) EVP_ATTR(false, true, ev2g) EVP_ATTR(true, true, ev2g)
+#undef EVP_ATTR
     size_t ev3 = eval3_smem_bytes((int)nc, (int)Ms, SPEC_K_MAX);
     if (ev3 > 232448) ev3 = 232448;
     CUDA_TRY(c, cudaFuncSetAttribute(k_trial_eval3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ev3));
@@ -545,29 +551,32 @@ static void launch_trial_eval(tebgpu_ctx* ctx, const SpecBufs& spec, const DevBa
     return;
   }
   if (!ctx->eval_v1) { /* second generation: one lane per pose */
-    const bool wide = (long long)B * 2 <= ctx->sms; /* a CTA per band leaves SMs idle: give each band up to 16 warps */
-    /* two compilations: <., 256> is built for 4 CTAs per SM (64 registers, a few spills) - what a full machine wants;
-     * <., 512> keeps all 116 registers - faster per thread, right while every CTA is resident at 2 per SM anyway
-     * (on C4 the 512-thread build wins up to 2 CTAs per SM worth of bands, the 256-thread one beyond) */
-    const bool relaxed = wide || B <= 2 * ctx->sms;
     /* one warp per 30-pose tile of the longest band (2 .. 8 warps; 4 .. 16 in the wide variant: two trials side by side),
      * so that the K x tiles warp tasks split evenly and nobody idles at the barrier */
     int warps = ev2_tiles(db.n_cap);
     warps = warps < 2 ? 2 : (warps > 8 ? 8 : warps);
-    if (wide) warps = 2 * warps;
-    const int nt = 32 * warps;
-    if (gt) {
-      if (kp.generic && relaxed) k_trial_eval2<true, 512, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
-      else if (kp.generic) k_trial_eval2<true, 256, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
-      else if (relaxed) k_trial_eval2<false, 512, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
-      else k_trial_eval2<false, 256, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
-    } else if (kp.generic) {
-      if (relaxed) k_trial_eval2<true, 512><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
-      else k_trial_eval2<true, 256><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
-    } else {
-      if (relaxed) k_trial_eval2<false, 512><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
-      else k_trial_eval2<false, 256><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+    const bool wide = (long long)B * 2 <= ctx->sms; /* a CTA per band leaves SMs idle: give each band up to 16 warps */
+    if (wide || B <= 2 * ctx->sms) {
+      /* a CTA per band, compiled for 1 CTA per SM (all registers): right while every CTA is resident anyway */
+      if (wide) warps = 2 * warps;
+      const int nt = 32 * warps;
+      if (gt && kp.generic) k_trial_eval2<true, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+      else if (gt) k_trial_eval2<false, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+      else if (kp.generic) k_trial_eval2<true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+      else k_trial_eval2<false><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+      return;
     }
+    /* throughput regime: the persistent build, as many CTAs as are resident (same shared memory as k_trial_eval2) */
+    const int nt = 32 * warps;
+    auto go = [&](auto kern) {
+      int per_sm = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, nt, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+      kern<<<per_sm * ctx->sms, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
+    };
+    if (gt && kp.generic) go(k_trial_eval2p<true, true>);
+    else if (gt) go(k_trial_eval2p<false, true>);
+    else if (kp.generic) go(k_trial_eval2p<true, false>);
+    else go(k_trial_eval2p<false, false>);
     return;
   }
   if (kp.generic) k_trial_eval<2, true><<<B, 32 * K, smem, st>>>(db, kp, spec, it, round, g, tag);

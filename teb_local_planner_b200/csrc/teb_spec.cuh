@@ -892,8 +892,7 @@ __global__ void __launch_bounds__(32 * SPEC_K_MAX, MINB) k_trial_eval(DevBatch d
  * and the lane evaluates all cost terms anchored at its pose. Tile partials are folded in a fixed order, then one thread
  * replays g2o's accept / reject chain (spec_decide) and the CTA commits the accepted trial state.
  * ==================================================================================================================== */
-constexpr int EV2_THREADS = 256;
-constexpr int EV2_MINB = 4;       /* CTAs per SM the throughput variant is compiled for (register cap 85) */
+constexpr int EV2_THREADS = 256;  /* the most threads k_trial_eval2p runs: 8 warps */
 constexpr int EV2_TILE = 30;      /* poses evaluated per warp task: lanes 0 .. 29 (lanes 30, 31: halo) */
 __host__ __device__ inline int ev2_tiles(int n_cap) { return (n_cap + EV2_TILE - 1) / EV2_TILE; }
 __host__ __device__ inline size_t eval2_smem_bytes(int n_cap, int M_cap, int K) {
@@ -1077,10 +1076,11 @@ __device__ __forceinline__ void eval_tile_task(const KParams& kp, const DevBatch
   scl = warp_sum(scl);
 }
 
-/* NT = 256 (throughput regime, 2 CTAs per SM) or 512 (latency regime: more warps per band). GT = global-table path
+/* A CTA per band, compiled for one CTA per SM (up to 512 threads, all registers): the build of batches whose CTAs are
+ * all resident at once (B <= 2 x SMs); larger batches run k_trial_eval2p. GT = global-table path
  * (M_cap > STAGED_MAX_OBST): no copy of the scene's obstacle table, rows read from global memory. */
-template <bool GEOM, int NT, bool GT = false>
-__global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_trial_eval2(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp,
+template <bool GEOM, bool GT = false>
+__global__ void __launch_bounds__(512, 1) k_trial_eval2(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp,
                                                              const __grid_constant__ SpecBufs sp, int iteration, int round,
                                                              int g, int tag) {
   extern __shared__ __align__(16) unsigned char ev_raw[];
@@ -1089,7 +1089,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_t
   const int b = spec_band(db, sp, round, g, slot);
   if (b < 0) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int nthreads = blockDim.x; /* <= NT: as many warps as the band has 30-pose tiles, so that the K x tiles tasks split evenly */
+  const int nthreads = blockDim.x; /* <= 512: as many warps as the band has 30-pose tiles, so that the K x tiles tasks split evenly */
   BandState* st = &db.state[b];
   if (!st->active) return;
   const int q0 = (round == 0) ? 0 : sp.qmax[b];
@@ -1184,12 +1184,179 @@ __global__ void __launch_bounds__(NT, NT == 256 ? (GEOM ? 2 : EV2_MINB) : 1) k_t
 }
 
 /* ====================================================================================================================
+ * k_trial_eval2p — the trial evaluation of the THROUGHPUT regime (B > 2 x SMs): k_trial_eval2's band evaluation in a
+ * PERSISTENT grid. As many CTAs as are resident; CTA c takes the slots c, c + G, c + 2G, ... of the launch (G CTAs; the
+ * slots are every band in round 0 and the retry list of round g in retry rounds, its length read on the device). Per band
+ * it runs k_trial_eval2's tile tasks, fold, spec_decide and commit on the same layout with the same pointers, so the
+ * results are the same bits. What differs:
+ *   - the band's current state, right-hand side and K trial solutions reach shared memory by cp.async (LDGSTS): the
+ *     state and rhs in 16-byte pieces, the solutions in 8-byte pieces straight into their per-trial rows. No registers
+ *     hold the copies, so every piece of a band is in flight at once; they are issued right after the previous band's
+ *     commit;
+ *   - the scene's obstacle table is copied only when the scene changes; the GT build reads rows from global memory as
+ *     k_trial_eval2<., ., true> does;
+ *   - no grid of B CTAs: a retry round's CTAs split its list instead of B CTAs reading cnt[g] and leaving.
+ * The slots are dealt out round robin, not in contiguous ranges: neighbouring bands belong to the same scene and cost
+ * alike, so contiguous ranges left some CTAs with the expensive scenes and measured slower than one CTA per band.
+ * One staging buffer: a second one (band j + 1 copied while band j is evaluated) costs a resident CTA per SM and
+ * measured slower at every width (DESIGN §8).
+ * ==================================================================================================================== */
+constexpr int EVP_MINB = 4; /* CTAs per SM the non-GEOM build is compiled for (64 registers; C3's shared memory at K <= 4) */
+
+__device__ __forceinline__ void cp_async8(uint32_t smem_addr, const void* gptr) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_addr), "l"(gptr) : "memory");
+}
+
+template <bool GEOM, bool GT = false>
+__global__ void __launch_bounds__(EV2_THREADS, GEOM ? 2 : EVP_MINB) k_trial_eval2p(const __grid_constant__ DevBatch db,
+                                                                                  const __grid_constant__ KParams kp,
+                                                                                  const __grid_constant__ SpecBufs sp, int iteration,
+                                                                                  int round, int g, int tag) {
+  extern __shared__ __align__(16) unsigned char ev_raw[];
+  const int SPEC_K = sp.K;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int nthreads = blockDim.x; /* as k_trial_eval2: one warp per 30-pose tile of n_cap, 2 .. 8 */
+  const size_t nc4 = (size_t)4 * db.n_cap;
+  const size_t buf_doubles = ((size_t)SPEC_K + 2) * nc4;
+  TebObstacle* so_s = reinterpret_cast<TebObstacle*>(ev_raw + buf_doubles * sizeof(double));
+  double* sPart = reinterpret_cast<double*>(so_s + (GT ? 1 : (db.M_cap > 0 ? db.M_cap : 1))); /* [K][tiles(n_cap)][5] */
+  double* sRes = sPart + (size_t)SPEC_K * ev2_tiles(db.n_cap) * 5;                                /* [K][RES_STRIDE] */
+  int* sAcc = reinterpret_cast<int*>(sRes + (size_t)SPEC_K * RES_STRIDE);
+
+  const int nslots = round > 0 ? sp.cnt[g] : (sp.sel_list ? *sp.sel_cnt : db.B);
+  const int step = (int)gridDim.x;
+  /* the next slot of this CTA at or after s whose band exists and is active (every thread computes the same) */
+  auto next_band = [&](int s, int& b) {
+    for (; s < nslots; s += step) {
+      b = spec_band(db, sp, round, g, s);
+      if (b >= 0 && db.state[b].active) return s;
+    }
+    return nslots;
+  };
+  /* the cp.async copies of slot s / band b: rows r < N of the current band, the rhs and every trial */
+  auto stage = [&](int s, int b) {
+    const uint32_t dst = smem_u32(ev_raw);
+    const int N = 4 * db.n[b];
+    const double* gP = db.poses + (size_t)b * nc4;
+    const double* grhs = db.rhs + (size_t)b * nc4;
+    const uint32_t p0 = dst + (uint32_t)(SPEC_K * nc4 * sizeof(double)), b0 = p0 + (uint32_t)(nc4 * sizeof(double));
+    for (int p = tid; p < N / 2; p += nthreads) { /* N is a multiple of 4: whole 16-byte pieces */
+      cp_async16(p0 + 16u * p, gP + 2 * p);
+      cp_async16(b0 + 16u * p, grhs + 2 * p);
+    }
+    /* trial kk: system K s + kk, solver warp (K s + kk) >> 5, lane (K s + kk) & 31; adjacent threads take adjacent trials */
+    const int tsys0 = s * SPEC_K;
+    for (int e = tid; e < N * SPEC_K; e += nthreads) {
+      const int r = e / SPEC_K, kk = e - r * SPEC_K;
+      const int tsys = tsys0 + kk;
+      cp_async8(dst + (uint32_t)(((size_t)kk * nc4 + r) * sizeof(double)), sp.dx + (size_t)(tsys >> 5) * 32 * nc4 + (size_t)r * 32 + (tsys & 31));
+    }
+  };
+  auto stage_table = [&](int sc) {
+    const unsigned char* go = reinterpret_cast<const unsigned char*>(db.obstacles + (size_t)sc * db.M_cap);
+    const uint32_t dst = smem_u32(so_s);
+    const int pieces = db.obst_count[sc] * (int)(sizeof(TebObstacle) / 16);
+    for (int p = tid; p < pieces; p += nthreads) cp_async16(dst + 16u * p, go + 16 * (size_t)p);
+  };
+
+  int b = -1;
+  int s = next_band((int)blockIdx.x, b);
+  if (s >= nslots) return;
+  int sc_staged = -1; /* scene whose table is in shared memory */
+  if constexpr (!GT) { sc_staged = db.scene_id[b]; stage_table(sc_staged); }
+  stage(s, b);
+  cp_async_commit();
+  while (s < nslots) {
+    cp_async_wait<0>();
+    __syncthreads(); /* band s is in shared memory (and its scene's table in so_s) */
+    double* sdx = reinterpret_cast<double*>(ev_raw); /* [K][4 n_cap] trial solutions */
+    double* sP0 = sdx + (size_t)SPEC_K * nc4;        /* [n_cap][4] current band */
+    double* sB = sP0 + nc4;                          /* [4 n_cap] right-hand side */
+    BandState* st = &db.state[b];
+    const int q0 = (round == 0) ? 0 : sp.qmax[b];
+    const int n = db.n[b];
+    const int N = 4 * n;
+    const int tiles = (n + EV2_TILE - 1) / EV2_TILE;
+    const int sc = db.scene_id[b];
+    const int M = db.obst_count[sc];
+    const TebObstacle* so = GT ? db.obstacles + (size_t)sc * db.M_cap : so_s;
+    const int kact = min(SPEC_K, 10 - q0); /* trials of this round that exist (g2o stops after 10) */
+    const double* vs = db.vel_start + 4 * (size_t)b;
+    const double* vg = db.vel_goal + 4 * (size_t)b;
+    for (int task = warp; task < kact * tiles; task += nthreads / 32) {
+      const int k = task / tiles, tile = task - k * tiles;
+      const double* res = sp.res + ((size_t)b * SPEC_K_MAX + k) * RES_STRIDE;
+      double chi[4], scl;
+      eval_tile_task<GEOM, GT>(kp, db, b, sc, n, tile, lane, res[5] != 0.0, res[6], sdx + (size_t)k * nc4, sP0, sB, so, M, vs, vg,
+                               chi, scl);
+      if (lane == 0) {
+        double* pp = sPart + ((size_t)k * ev2_tiles(db.n_cap) + tile) * 5;
+        pp[0] = chi[0]; pp[1] = chi[1]; pp[2] = chi[2]; pp[3] = chi[3]; pp[4] = scl;
+      }
+    }
+    __syncthreads();
+    if (tid < kact) { /* fold the tile partials of trial tid in tile order */
+      double* gr = sp.res + ((size_t)b * SPEC_K_MAX + tid) * RES_STRIDE;
+      const double okv = gr[5];
+      double a[5] = {0, 0, 0, 0, 0};
+      for (int t = 0; t < tiles; ++t) {
+        const double* pp = sPart + ((size_t)tid * ev2_tiles(db.n_cap) + t) * 5;
+#pragma unroll
+        for (int c = 0; c < 5; ++c) a[c] += pp[c];
+      }
+      double* r = sRes + tid * RES_STRIDE;
+      r[0] = a[0]; r[1] = a[1]; r[2] = a[2]; r[3] = a[3]; r[4] = a[4];
+      r[5] = okv;
+#pragma unroll
+      for (int c = 0; c < 5; ++c) gr[c] = a[c];
+    }
+    __syncthreads();
+    if (tid == 0) { /* accept / reject replay, sequential over the K trials */
+      DecideArgs da;
+      da.st = st; da.chi_parts = db.chi_parts + (size_t)b * db.chunks * 4;
+      da.lambda_init = (round == 0 && iteration == 0) ? band_lambda_init(db, b, n) : 0.0;
+      da.need = sp.need + b; da.qmax = sp.qmax + b; da.cnt_next = sp.cnt + g + 1;
+      da.list_next = sp.list + (size_t)((g + 1) % SPEC_LISTS) * db.B;
+      da.defer = db.defer + b; da.tag = tag;
+      da.b = b; da.n = n; da.K = SPEC_K; da.iteration = iteration; da.round = round; da.q0 = q0; da.tile = db.tile;
+      sAcc[0] = spec_decide(da, sRes);
+    }
+    __syncthreads();
+    const int accepted = sAcc[0];
+    if (accepted >= 0) { /* discardTop(): the accepted trial state becomes the band (same arithmetic as k_trial_eval2) */
+      double* gP = db.poses + (size_t)b * nc4;
+      const double* adx = sdx + (size_t)accepted * nc4;
+      const bool ok = sRes[accepted * RES_STRIDE + 5] != 0.0;
+      for (int r = tid; r < N; r += nthreads) {
+        if (!row_is_real(r, n)) continue;
+        const double dxv = ok ? adx[r] : sB[r];
+        const double xv = sP0[r] + dxv;
+        gP[r] = ((r & 3) == 2) ? normalize_theta(xv) : xv;
+      }
+    }
+    int b_nx = -1;
+    const int s_nx = next_band(s + step, b_nx);
+    if (s_nx < nslots) { /* every thread is done with the band's shared memory (and the table): stage the next band */
+      __syncthreads();
+      if constexpr (!GT) {
+        if (db.scene_id[b_nx] != sc_staged) { sc_staged = db.scene_id[b_nx]; stage_table(sc_staged); }
+      }
+      stage(s_nx, b_nx);
+      cp_async_commit();
+    }
+    s = s_nx;
+    b = b_nx;
+  }
+  cp_async_wait<0>();
+}
+
+/* ====================================================================================================================
  * k_trial_eval3 — the trial evaluation of the LATENCY regime (one planning request: a few dozen bands). k_trial_eval2
  * gives a band ONE CTA, i.e. 32 candidates keep 32 of the 132 SMs busy. Here a CTA owns one (band, trial)
  * pair - grid (K, bands), one warp per 30-pose tile - so a request spreads over the whole chip; the per-trial chi2 /
  * scale go to sp.res in global memory and the LAST CTA of a band to arrive (one atomic counter per band) replays the
  * accept / reject chain and commits the accepted trial, reading its dx back from the solver's scratch.
- * Same tile tasks, same fold order, same spec_decide as k_trial_eval2: the results are bit-identical.
+ * Same tile tasks, same fold order, same spec_decide as k_trial_eval2 / k_trial_eval2p: the results are bit-identical.
  * ==================================================================================================================== */
 __host__ __device__ inline size_t eval3_smem_bytes(int n_cap, int M_cap, int K) {
   return (size_t)3 * 4 * n_cap * sizeof(double) + (size_t)(M_cap > 0 ? M_cap : 1) * sizeof(TebObstacle) +
