@@ -310,7 +310,14 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
 /* Introspection for measurement scripts. which: 0 speculation width used by the last optimize call, 1 kernel-A variant,
  * 2 solver, 3 communicator size (1 without tebgpu_comm_init), 4 communicator rank, 5 CUDA-graph replay enabled,
  * 6 number of captured graphs held by the context, 7 speculation width of the first LM iteration after a graph rebuild
- * (key 0 reports the width of the later iterations). Returns -1 for an unknown key. */
+ * (key 0 reports the width of the later iterations), 8 grid in CTAs of the last trial-evaluation launch the context
+ * issued (0 before the first; a replayed CUDA graph issues none), 9 which build that launch ran (TEBGPU_EVAL_BUILD_*,
+ * -1 before the first). Returns -1 for an unknown key. */
+#define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
+#define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */
+#define TEBGPU_EVAL_BUILD_EVAL2 2       /* k_trial_eval2 (B <= 2 x SMs): B CTAs */
+#define TEBGPU_EVAL_BUILD_EVAL2P 3      /* k_trial_eval2p, persistent (B > 2 x SMs): resident CTAs per SM x SMs */
+#define TEBGPU_EVAL_BUILD_EVAL3 4       /* k_trial_eval3 (latency regime or TEBGPU_EVAL3=1): K x B CTAs */
 int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which);
 
 /* Linearise only: build the padded banded normal equations of every band at its current state for

@@ -232,6 +232,13 @@ class TebGpu:
         """speculation width (trials solved concurrently per round) chosen by the last optimize call"""
         return self.info(0)
 
+    EVAL_BUILDS = {0: "v1", 1: "eval2_wide", 2: "eval2", 3: "eval2p", 4: "eval3"}   # TEBGPU_EVAL_BUILD_*
+
+    def last_trial_eval(self):
+        """(build, grid in CTAs) of the last trial-evaluation launch this context issued: build is one of EVAL_BUILDS'
+        names, or None before the first launch"""
+        return self.EVAL_BUILDS.get(self.info(9)), self.info(8)
+
     def launch_count(self):
         return int(self.lib.tebgpu_last_launch_count(self.ctx))
 

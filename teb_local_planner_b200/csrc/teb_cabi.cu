@@ -67,6 +67,8 @@ struct tebgpu_ctx {
   int ka_staged = 1;   /* kernel A output: 1 (default) shared-memory slot + TMA bulk store per lane, 0 direct 128-bit global stores */
   int last_spec_k = 0; /* round-0 width of the later LM iterations of the last optimize call */
   int last_spec_first = 0; /* round-0 width of the first LM iteration after a graph rebuild */
+  int last_eval_build = -1;      /* the last trial-evaluation launch this context issued: its build (TEBGPU_EVAL_BUILD_*) */
+  long long last_eval_grid = 0;  /* ... and its grid in CTAs */
   int spec_k = 0;  /* speculation width: 0 = auto (6 when B*6 systems fit one warp per SM sub-partition, else 4) */
   int solver = 2;  /* 2: speculative thread-per-(band,trial) LDL^T (default), 1: block cyclic reduction, 0: sequential */
   int MW = 1;
@@ -197,6 +199,8 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 5: return ctx->graph_mode;
     case 6: return (int64_t)ctx->graphs.size();
     case 7: return ctx->last_spec_first;
+    case 8: return ctx->last_eval_grid;
+    case 9: return ctx->last_eval_build;
     default: return -1;
   }
 }
@@ -544,6 +548,7 @@ static void launch_trial_eval(tebgpu_ctx* ctx, const SpecBufs& spec, const DevBa
     int warps = ev2_tiles(db.n_cap);
     warps = warps < 1 ? 1 : (warps > 16 ? 16 : warps);
     const dim3 grid(K, B);
+    ctx->last_eval_build = TEBGPU_EVAL_BUILD_EVAL3; ctx->last_eval_grid = (long long)K * B;
     if (gt && kp.generic) k_trial_eval3<true, true><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
     else if (gt) k_trial_eval3<false, true><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
     else if (kp.generic) k_trial_eval3<true><<<grid, 32 * warps, smem3, st>>>(db, kp, spec, it, round, g, tag, ctx->arrive);
@@ -560,6 +565,7 @@ static void launch_trial_eval(tebgpu_ctx* ctx, const SpecBufs& spec, const DevBa
       /* a CTA per band, compiled for 1 CTA per SM (all registers): right while every CTA is resident anyway */
       if (wide) warps = 2 * warps;
       const int nt = 32 * warps;
+      ctx->last_eval_build = wide ? TEBGPU_EVAL_BUILD_EVAL2_WIDE : TEBGPU_EVAL_BUILD_EVAL2; ctx->last_eval_grid = B;
       if (gt && kp.generic) k_trial_eval2<true, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
       else if (gt) k_trial_eval2<false, true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
       else if (kp.generic) k_trial_eval2<true><<<B, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
@@ -571,6 +577,7 @@ static void launch_trial_eval(tebgpu_ctx* ctx, const SpecBufs& spec, const DevBa
     auto go = [&](auto kern) {
       int per_sm = 0;
       if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, nt, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+      ctx->last_eval_build = TEBGPU_EVAL_BUILD_EVAL2P; ctx->last_eval_grid = (long long)per_sm * ctx->sms;
       kern<<<per_sm * ctx->sms, nt, smem, st>>>(db, kp, spec, it, round, g, tag);
     };
     if (gt && kp.generic) go(k_trial_eval2p<true, true>);
@@ -579,6 +586,7 @@ static void launch_trial_eval(tebgpu_ctx* ctx, const SpecBufs& spec, const DevBa
     else go(k_trial_eval2p<false, false>);
     return;
   }
+  ctx->last_eval_build = TEBGPU_EVAL_BUILD_V1; ctx->last_eval_grid = B;
   if (kp.generic) k_trial_eval<2, true><<<B, 32 * K, smem, st>>>(db, kp, spec, it, round, g, tag);
   else if (ctx->eval_minb == 3) k_trial_eval<3, false><<<B, 32 * K, smem, st>>>(db, kp, spec, it, round, g, tag);
   else k_trial_eval<2, false><<<B, 32 * K, smem, st>>>(db, kp, spec, it, round, g, tag);
