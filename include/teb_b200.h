@@ -312,12 +312,18 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * 6 number of captured graphs held by the context, 7 speculation width of the first LM iteration after a graph rebuild
  * (key 0 reports the width of the later iterations), 8 grid in CTAs of the last trial-evaluation launch the context
  * issued (0 before the first; a replayed CUDA graph issues none), 9 which build that launch ran (TEBGPU_EVAL_BUILD_*,
- * -1 before the first). Returns -1 for an unknown key. */
+ * -1 before the first), 10 grid in CTAs of the last kernel-A launch the context issued (0 before the first; a replayed
+ * CUDA graph issues none), 11 which build that launch ran (TEBGPU_KA_BUILD_*, -1 before the first). Returns -1 for an
+ * unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2 2       /* k_trial_eval2 (B <= 2 x SMs): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2P 3      /* k_trial_eval2p, persistent (B > 2 x SMs): resident CTAs per SM x SMs */
 #define TEBGPU_EVAL_BUILD_EVAL3 4       /* k_trial_eval3 (latency regime or TEBGPU_EVAL3=1): K x B CTAs */
+#define TEBGPU_KA_BUILD_V1 0       /* k_linearize, first generation (tebgpu_set_linearize_variant(1)): chunks x B CTAs */
+#define TEBGPU_KA_BUILD_ONESHOT 1  /* k_linearize2, staged output (TEBGPU_KA_PERSIST=0): ceil(chunks / 4) x B CTAs */
+#define TEBGPU_KA_BUILD_DIRECT 2   /* k_linearize2, direct stores (TEBGPU_KA_STAGED=0): ceil(chunks / 4) x B CTAs */
+#define TEBGPU_KA_BUILD_PERSIST 3  /* k_linearize2p (default): resident one-warp CTAs per SM x SMs, at most chunks x B */
 int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which);
 
 /* Linearise only: build the padded banded normal equations of every band at its current state for
@@ -369,6 +375,12 @@ int32_t tebgpu_solve_system(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, const dou
 int32_t tebgpu_build_system_graph(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_index, const int32_t* list,
                                   int32_t list_len, double* Hb_out, double* chi_fam_out, uint64_t* assoc_out,
                                   uint64_t* assoc3_out, uint64_t* occ_out, int32_t* via_idx_out, double* dyn_t_out);
+/* Kernel A's other outputs of the last tebgpu_build_system(_graph) call on a batch of B bands and n_cap poses, HOST
+ * buffers (any may be NULL): rhs_out [B][4 n_cap]; chi_parts_out [B][T][4] the tile partials of chi2 by family;
+ * dmax_parts_out [B][T] the tile partials of the largest diagonal entry. T = ceil(n_cap / 29), ceil(n_cap / 32) under
+ * linearize variant 1. */
+int32_t tebgpu_read_linearize_outputs(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, double* rhs_out, double* chi_parts_out,
+                                      double* dmax_parts_out);
 
 /* Trial evaluation only: one round of the speculative LM step's trial evaluation and accept / reject chain, launched by
  * the same code as in tebgpu_optimize_batch (the kernel TEBGPU_EVAL_V1 / TEBGPU_EVAL3 and the batch size select). Test /

@@ -84,6 +84,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_build_system.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, vp, C.c_int32]
     L.tebgpu_build_system_graph.restype = C.c_int32
     L.tebgpu_build_system_graph.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp]
+    L.tebgpu_read_linearize_outputs.restype = C.c_int32
+    L.tebgpu_read_linearize_outputs.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
     L.tebgpu_solve_system.restype = C.c_int32
     L.tebgpu_solve_system.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32,
                                       vp, vp, vp]
@@ -238,6 +240,25 @@ class TebGpu:
         """(build, grid in CTAs) of the last trial-evaluation launch this context issued: build is one of EVAL_BUILDS'
         names, or None before the first launch"""
         return self.EVAL_BUILDS.get(self.info(9)), self.info(8)
+
+    KA_BUILDS = {0: "v1", 1: "oneshot", 2: "direct", 3: "persistent"}   # TEBGPU_KA_BUILD_*
+
+    def last_linearize(self):
+        """(build, grid in CTAs) of the last kernel-A launch this context issued: build is one of KA_BUILDS' names, or
+        None before the first launch"""
+        return self.KA_BUILDS.get(self.info(11)), self.info(10)
+
+    def linearize_outputs(self, B, n_cap):
+        """kernel A's rhs [B][4 n_cap], chi2 tile partials [B][tiles][4] and max-diagonal tile partials [B][tiles]
+        (tiles = ceil(n_cap / 29), ceil(n_cap / 32) under linearize variant 1) of the last build_system call on B bands
+        of n_cap poses"""
+        import numpy as np
+        tile = 32 if self.info(1) == 1 else 29
+        tiles = (n_cap + tile - 1) // tile
+        out = dict(rhs=np.empty((B, 4 * n_cap)), chi_parts=np.empty((B, tiles, 4)), dmax_parts=np.empty((B, tiles)))
+        self._check(self.lib.tebgpu_read_linearize_outputs(self.ctx, int(B), int(n_cap), *(out[k].ctypes.data for k in
+                                                           ("rhs", "chi_parts", "dmax_parts"))), "tebgpu_read_linearize_outputs")
+        return out
 
     def launch_count(self):
         return int(self.lib.tebgpu_last_launch_count(self.ctx))

@@ -65,6 +65,9 @@ struct tebgpu_ctx {
                           1 streamed through HBM, 11 / 22 / 33 recomputed in segments of that many rows */
   int eval_v1 = 0;     /* TEBGPU_EVAL_V1=1: first-generation trial evaluation (warp per trial, chunk per lane) */
   int ka_staged = 1;   /* kernel A output: 1 (default) shared-memory slot + TMA bulk store per lane, 0 direct 128-bit global stores */
+  int ka_persist = 1;  /* kernel A with the staged output: 1 (default) persistent k_linearize2p, 0 one-shot k_linearize2 (TEBGPU_KA_PERSIST) */
+  int last_ka_build = -1;      /* the last kernel-A launch this context issued: its build (TEBGPU_KA_BUILD_*) */
+  long long last_ka_grid = 0;  /* ... and its grid in CTAs */
   int last_spec_k = 0; /* round-0 width of the later LM iterations of the last optimize call */
   int last_spec_first = 0; /* round-0 width of the first LM iteration after a graph rebuild */
   int last_eval_build = -1;      /* the last trial-evaluation launch this context issued: its build (TEBGPU_EVAL_BUILD_*) */
@@ -201,6 +204,8 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 7: return ctx->last_spec_first;
     case 8: return ctx->last_eval_grid;
     case 9: return ctx->last_eval_build;
+    case 10: return ctx->last_ka_grid;
+    case 11: return ctx->last_ka_build;
     default: return -1;
   }
 }
@@ -374,8 +379,14 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize2<H, G, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   KA2G_ATTR(false, false) KA2G_ATTR(false, true) KA2G_ATTR(true, false) KA2G_ATTR(true, true)
 #undef KA2G_ATTR
+#define KA2P_ATTR(H, G, T) \
+  CUDA_TRY(c, cudaFuncSetAttribute(k_linearize2p<H, G, T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  KA2P_ATTR(false, false, false) KA2P_ATTR(false, true, false) KA2P_ATTR(true, false, false) KA2P_ATTR(true, true, false)
+  KA2P_ATTR(false, false, true) KA2P_ATTR(false, true, true) KA2P_ATTR(true, false, true) KA2P_ATTR(true, true, true)
+#undef KA2P_ATTR
   c->ka_staged = 1; /* TMA bulk store per lane: direct 128-bit stores fill only half of each 32-byte sector */
   if (const char* e = std::getenv("TEBGPU_KA_STAGED")) c->ka_staged = std::atoi(e) != 0; /* staged path (M_cap <= 1024) only */
+  if (const char* e = std::getenv("TEBGPU_KA_PERSIST")) c->ka_persist = std::atoi(e) != 0;
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_a));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_a));
   CUDA_TRY(c, cudaFuncSetAttribute(k_linearize<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_a));
@@ -491,10 +502,33 @@ static int32_t check_path(tebgpu_ctx* ctx, const TebBatch* bt, bool solves) {
 static void launch_linearize(tebgpu_ctx* ctx, const DevBatch& db, const KParams& kp, int B, int M_cap, cudaStream_t st) {
   const bool holo = kp.holo_vel || kp.holo_acc;
   const bool geom = kp.generic != 0;
+  if (ctx->ka_persist && ctx->linearize_variant == 0 && (ctx->ka_staged || global_table(M_cap))) {
+    /* persistent one-warp CTAs, as many as are resident, never more than the launch has units */
+    const size_t sm = holo ? ka2p_smem_bytes<true>() : ka2p_smem_bytes<false>();
+    auto go = [&](auto kern) {
+      int per_sm = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32, sm) != cudaSuccess || per_sm < 1) per_sm = 1;
+      long long grid = (long long)per_sm * ctx->sms;
+      if (grid > (long long)B * db.chunks) grid = (long long)B * db.chunks;
+      ctx->last_ka_build = TEBGPU_KA_BUILD_PERSIST; ctx->last_ka_grid = grid;
+      kern<<<(unsigned)grid, 32, sm, st>>>(db, kp, B);
+    };
+    const bool gt = global_table(M_cap);
+    if (gt && holo && geom) go(k_linearize2p<true, true, true>);
+    else if (gt && holo) go(k_linearize2p<true, false, true>);
+    else if (gt && geom) go(k_linearize2p<false, true, true>);
+    else if (gt) go(k_linearize2p<false, false, true>);
+    else if (holo && geom) go(k_linearize2p<true, true, false>);
+    else if (holo) go(k_linearize2p<true, false, false>);
+    else if (geom) go(k_linearize2p<false, true, false>);
+    else go(k_linearize2p<false, false, false>);
+    return;
+  }
   if (global_table(M_cap)) { /* output through the staged slot, the default form: TEBGPU_KA_STAGED=0 (direct stores,
                                 same results) applies to the staged path only */
     const dim3 g2((db.chunks + KA2_W - 1) / KA2_W, B);
     const size_t sm = holo ? ka2_smem_bytes<true>(0) : ka2_smem_bytes<false>(0);
+    ctx->last_ka_build = TEBGPU_KA_BUILD_ONESHOT; ctx->last_ka_grid = (long long)g2.x * B;
     if (holo && geom) k_linearize2<true, true, false, true><<<g2, KA2_THREADS, sm, st>>>(db, kp);
     else if (holo) k_linearize2<true, false, false, true><<<g2, KA2_THREADS, sm, st>>>(db, kp);
     else if (geom) k_linearize2<false, true, false, true><<<g2, KA2_THREADS, sm, st>>>(db, kp);
@@ -502,6 +536,7 @@ static void launch_linearize(tebgpu_ctx* ctx, const DevBatch& db, const KParams&
   } else if (ctx->linearize_variant == 1) {
     const dim3 grid(db.chunks, B);
     const size_t sm = ka_smem_bytes(M_cap);
+    ctx->last_ka_build = TEBGPU_KA_BUILD_V1; ctx->last_ka_grid = (long long)grid.x * B;
     if (holo && geom) k_linearize<true, true><<<grid, KA_THREADS, sm, st>>>(db, kp);
     else if (holo) k_linearize<true, false><<<grid, KA_THREADS, sm, st>>>(db, kp);
     else if (geom) k_linearize<false, true><<<grid, KA_THREADS, sm, st>>>(db, kp);
@@ -509,6 +544,7 @@ static void launch_linearize(tebgpu_ctx* ctx, const DevBatch& db, const KParams&
   } else {
     const dim3 g2((db.chunks + KA2_W - 1) / KA2_W, B);
     const size_t sm = holo ? ka2_smem_bytes<true>(M_cap) : ka2_smem_bytes<false>(M_cap);
+    ctx->last_ka_build = ctx->ka_staged ? TEBGPU_KA_BUILD_ONESHOT : TEBGPU_KA_BUILD_DIRECT; ctx->last_ka_grid = (long long)g2.x * B;
 #define KA2_LAUNCH(H, G)                                                                      \
   do {                                                                                        \
     if (ctx->ka_staged) k_linearize2<H, G, false><<<g2, KA2_THREADS, sm, st>>>(db, kp);       \
@@ -921,7 +957,7 @@ static uint64_t graph_key(const tebgpu_ctx* ctx, const TebBatch* bt, const TebOp
   mix(bt, sizeof(*bt));
   mix(a, sizeof(*a));
   mix(&ctx->params_version, sizeof(ctx->params_version));
-  const int sw[11] = {ctx->solver, ctx->spec_k, ctx->linearize_variant, ctx->ka_staged, ctx->eval_v1, ctx->overlap, ctx->eval_minb, ctx->warp_solver, ctx->eval_mode, ctx->split, ctx->solve_form};
+  const int sw[12] = {ctx->solver, ctx->spec_k, ctx->linearize_variant, ctx->ka_staged, ctx->eval_v1, ctx->overlap, ctx->eval_minb, ctx->warp_solver, ctx->eval_mode, ctx->split, ctx->solve_form, ctx->ka_persist};
   mix(sw, sizeof(sw));
   mix(&st, sizeof(st));
   return h;
@@ -1202,7 +1238,7 @@ int32_t tebgpu_build_system(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_i
   const int B = bt->B, tb = 128, gb = ((B > bt->S ? B : bt->S) + tb - 1) / tb;
   k_begin<<<gb, tb, 0, st>>>(db, kp);
   launch_build_graph(db, kp, B, (size_t)(bt->M_cap > 0 ? bt->M_cap : 1) * sizeof(TebObstacle), st);
-  launch_linearize(ctx, db, kp, B, bt->M_cap, st);
+  prof_begin(ctx, st, 3); launch_linearize(ctx, db, kp, B, bt->M_cap, st); prof_end(ctx, st);
   if (kp.has_vor) launch_vor(db, kp, B, (size_t)(bt->M_cap > 0 ? bt->M_cap : 1) * sizeof(TebObstacle), st);
   ctx->launches = 3;
   CUDA_TRY(ctx, cudaGetLastError());
@@ -1248,6 +1284,20 @@ static void fold_chi_parts(const double* parts, const DevBatch& db, int b, int n
   for (int ch = 0; ch < used; ++ch)
     for (int c = 0; c < 4; ++c) cur[c] += parts[((size_t)b * db.chunks + ch) * 4 + c];
   for (int c = 0; c < 4; ++c) out4[c] = cur[c];
+}
+
+int32_t tebgpu_read_linearize_outputs(tebgpu_ctx* ctx, int32_t B, int32_t n_cap, double* rhs_out, double* chi_parts_out,
+                                      double* dmax_parts_out) {
+  if (!ctx || B < 1 || B > ctx->lim.max_bands || n_cap < 3 || n_cap > ctx->lim.max_poses) return TEBGPU_ERR_INVALID_ARG;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const int tile = ctx->linearize_variant == 1 ? TP : KA2_TP; /* make_devbatch's tile: the layout of the partials */
+  const size_t tiles = (size_t)B * ((n_cap + tile - 1) / tile);
+  if (rhs_out) CUDA_TRY(ctx, cudaMemcpyAsync(rhs_out, ctx->rhs, (size_t)B * 4 * n_cap * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (chi_parts_out) CUDA_TRY(ctx, cudaMemcpyAsync(chi_parts_out, ctx->chi_parts, tiles * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (dmax_parts_out) CUDA_TRY(ctx, cudaMemcpyAsync(dmax_parts_out, ctx->dmax_parts, tiles * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
 }
 
 int32_t tebgpu_build_system_graph(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_index, const int32_t* list,

@@ -1,5 +1,5 @@
 /*
- * teb_linearize.cuh — "kernel A", second generation (the default): residuals + closed-form Jacobians of every edge
+ * teb_linearize.cuh — "kernel A", second generation (k_linearize2p below is its persistent form, the default): residuals + closed-form Jacobians of every edge
  * family + banded J^T Omega J / b assembly, ONE THREAD PER POSE, ONE WARP PER TILE, no block-wide barrier on the path.
  *
  * Mapping. A warp owns KA2_TP = 29 consecutive poses of one band; lane l <-> pose / anchor i = q0 - 2 + l (two halo
@@ -530,64 +530,19 @@ __device__ __forceinline__ void unary_terms2(const KParams& kp, const DevBatch& 
 
 __device__ __forceinline__ double shfl_down1(double v) { return __shfl_down_sync(0xffffffffu, v, 1); }
 
-/* ------------------------------------------------------------------ k_linearize2 */
-/* GT = global-table path (M_cap > STAGED_MAX_OBST): no TMA copy of the scene's obstacle table, rows read from global
- * memory, associations walked via the occupancy words */
-template <bool HOLO, bool GEOM, bool OUT_DIRECT, bool GT = false>
-__global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  using L = JL<HOLO>;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  double* sP = reinterpret_cast<double*>(smem_raw);                      /* poses, slot j <-> pose P0 + j */
-  double* sW = sP + KA2Smem::POSES + (size_t)warp * KA2Smem::warp_doubles<HOLO>(); /* this warp's records / output slots */
-  double* sStart = sW + KA2Smem::rec_doubles<HOLO>();                    /* EdgeAccelerationStart rows (tile of anchor 0) */
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sP + KA2Smem::POSES + (size_t)KA2_W * KA2Smem::warp_doubles<HOLO>());
-  TebObstacle* so_s = reinterpret_cast<TebObstacle*>((reinterpret_cast<uintptr_t>(bar) + 16 + 15) & ~static_cast<uintptr_t>(15));
-
-  /* everything the prologue needs is loaded at once: no chain of dependent global loads */
-  const int y = blockIdx.y;
-  int b = y, skip = 0;
-  if (db.a_list) { if (y < *db.a_cnt) b = db.a_list[y]; else skip = 1; }
-  else if (db.skip_tag != 0 && deferred_since(db.defer[y], db.skip_tag)) skip = 1;
-  if (skip) return; /* uniform for the CTA */
-  const int active = db.state[b].active;
-  const int n = db.n[b];
-  const int s = db.scene_id[b];
-  const int P0 = blockIdx.x * (KA2_W * KA2_TP) - 2;                       /* pose of slot 0 */
-  const int lo = max(P0, 0), hi = min(P0 + KA2_SLOTS, db.n_cap);          /* staged range: independent of n */
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    mbar_fence_init();
-  }
-  if (!active || P0 + 2 >= n) return;                                     /* uniform for the CTA, nothing in flight yet */
-  if (tid == 0) {
-    const uint32_t bytesP = (uint32_t)(hi - lo) * 32u;
-    const uint32_t bytesO = GT ? 0u : (uint32_t)db.M_cap * (uint32_t)sizeof(TebObstacle);
-    mbar_expect_tx(bar, bytesP + bytesO);
-    tma_load_1d(sP + (size_t)(lo - P0) * 4, db.poses + ((size_t)b * db.n_cap + lo) * 4, bytesP, bar);
-    if (bytesO) tma_load_1d(so_s, db.obstacles + (size_t)s * db.M_cap, bytesO, bar);
-  }
-  const int slot = warp * KA2_TP + lane;
-  const int i = P0 + slot;                                                /* pose / anchor of this lane */
-  const int q0 = P0 + 2 + warp * KA2_TP;                                  /* first pose this warp produces */
+/* ------------------------------------------------------------------ P1 - P4 and the tile partials of one warp tile
+ * (shared by k_linearize2 and k_linearize2p). Lane `lane` owns pose / anchor i, whose staged record starts at pa (the
+ * next poses follow at pa + 4, pa + 8); so is the scene's obstacle table (shared or global memory), mask0 the first
+ * association (GT: occupancy) word of pose i, sW / sStart the warp's record region and start block, tile the index of
+ * the tile partials. mid() runs between P1 and P2, after the neighbour shuffles: it must leave the warp's records and
+ * start block zeroed and the warp converged. */
+template <bool HOLO, bool GEOM, bool OUT_DIRECT, bool GT, class Mid>
+__device__ __forceinline__ void ka2_tile(const DevBatch& db, const KParams& kp, int b, int s, int n, int i, int lane,
+                                         const double* pa, const TebObstacle* so, unsigned long long mask0, double* sW,
+                                         double* sStart, int tile, Mid mid) {
   const bool out = (lane >= 2 && lane <= 30 && i < n);
-  /* while the copies are in flight: association word of the own pose, zeroed record and start block */
-  unsigned long long mask0 = 0ull;
-  if (out && kp.has_obst && i >= 1 && i <= n - 2)
-    mask0 = GT ? db.occ[((size_t)b * db.n_cap + i) * db.OW] : db.assoc[((size_t)b * db.n_cap + i) * db.MW];
-  {
-    double* rec = sW + lane;
-#pragma unroll
-    for (int e = 0; e < L::COUNT; ++e) rec[e * 32] = 0.0;
-    if (lane < KA2Smem::START) sStart[lane] = 0.0;
-  }
-  __syncthreads(); /* the mbarrier initialisation is visible to every waiting thread (the only block-wide barrier) */
-  mbar_wait(bar, 0);
-  if (q0 >= n) return; /* whole warp: tile beyond the band */
-
   double chi[4] = {0, 0, 0, 0}; /* obstacles, via, time-optimal, other */
   const bool have_pose = (i >= 0 && i < n);
-  const double* pa = sP + 4 * slot;
   double cs = 1, sn = 0;
   SegDer sd;
   sd.v = 0; sd.w = 0; sd.idt = 0;
@@ -598,9 +553,7 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
   if (have_pose) {
     sincos(pa[2], &sn, &cs);
     if (i <= n - 2) sd = seg_derivs(kp, pa[0], pa[1], pa[2], cs, sn, pa[4], pa[5], pa[6], pa[3]);
-    if (out)
-      unary_terms2<GEOM, GT>(kp, db, b, s, i, n, pa[0], pa[1], cs, sn, GT ? db.obstacles + (size_t)s * db.M_cap : so_s, mask0, U, ub,
-                             chi[0], chi[1]);
+    if (out) unary_terms2<GEOM, GT>(kp, db, b, s, i, n, pa[0], pa[1], cs, sn, so, mask0, U, ub, chi[0], chi[1]);
   }
   /* the right neighbour's sin / cos and segment bundle (lane 31 receives nothing useful and anchors nothing) */
   SegDer sd2;
@@ -608,7 +561,7 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
   sd2.v = shfl_down1(sd.v); sd2.w = shfl_down1(sd.w); sd2.idt = shfl_down1(sd.idt);
 #pragma unroll
   for (int k = 0; k < 6; ++k) sd2.dv[k] = shfl_down1(sd.dv[k]);
-  __syncwarp(); /* start block zeroed by other lanes */
+  mid();
   /* ---- P2: chain edges anchored at i */
   if (have_pose && i <= n - 2 && lane < 31) {
     JRec J;
@@ -671,7 +624,7 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
       r2[1] = make_double2(brow[2], brow[3]);
     }
   } else {
-    __syncwarp(); /* every lane is done reading the records: the region becomes the output slots */
+    __syncwarp(); /* every lane is done reading the records (and the poses): the region becomes the output slots */
     if (out) {
       double2* o2 = reinterpret_cast<double2*>(sW + (size_t)lane * OUT_STRIDE);
 #pragma unroll
@@ -689,18 +642,175 @@ __global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_cons
     }
   }
   /* tile partials: chi2 by family and the max diagonal of the real rows (computeLambdaInit), fixed order */
-  {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) chi[k] = warp_sum(chi[k]);
-    dm = warp_max(dm);
-    if (lane == 0) {
-      const int tile = blockIdx.x * KA2_W + warp;
-      double* cp = db.chi_parts + ((size_t)b * db.chunks + tile) * 4;
-      cp[0] = chi[0]; cp[1] = chi[1]; cp[2] = chi[2]; cp[3] = chi[3];
-      db.dmax_parts[(size_t)b * db.chunks + tile] = dm;
-    }
+  for (int k = 0; k < 4; ++k) chi[k] = warp_sum(chi[k]);
+  dm = warp_max(dm);
+  if (lane == 0) {
+    double* cp = db.chi_parts + ((size_t)b * db.chunks + tile) * 4;
+    cp[0] = chi[0]; cp[1] = chi[1]; cp[2] = chi[2]; cp[3] = chi[3];
+    db.dmax_parts[(size_t)b * db.chunks + tile] = dm;
   }
+}
+
+/* ------------------------------------------------------------------ k_linearize2 */
+/* GT = global-table path (M_cap > STAGED_MAX_OBST): no TMA copy of the scene's obstacle table, rows read from global
+ * memory, associations walked via the occupancy words */
+template <bool HOLO, bool GEOM, bool OUT_DIRECT, bool GT = false>
+__global__ void __launch_bounds__(KA2_THREADS, 3) k_linearize2(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  using L = JL<HOLO>;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  double* sP = reinterpret_cast<double*>(smem_raw);                      /* poses, slot j <-> pose P0 + j */
+  double* sW = sP + KA2Smem::POSES + (size_t)warp * KA2Smem::warp_doubles<HOLO>(); /* this warp's records / output slots */
+  double* sStart = sW + KA2Smem::rec_doubles<HOLO>();                    /* EdgeAccelerationStart rows (tile of anchor 0) */
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sP + KA2Smem::POSES + (size_t)KA2_W * KA2Smem::warp_doubles<HOLO>());
+  TebObstacle* so_s = reinterpret_cast<TebObstacle*>((reinterpret_cast<uintptr_t>(bar) + 16 + 15) & ~static_cast<uintptr_t>(15));
+
+  /* everything the prologue needs is loaded at once: no chain of dependent global loads */
+  const int y = blockIdx.y;
+  int b = y, skip = 0;
+  if (db.a_list) { if (y < *db.a_cnt) b = db.a_list[y]; else skip = 1; }
+  else if (db.skip_tag != 0 && deferred_since(db.defer[y], db.skip_tag)) skip = 1;
+  if (skip) return; /* uniform for the CTA */
+  const int active = db.state[b].active;
+  const int n = db.n[b];
+  const int s = db.scene_id[b];
+  const int P0 = blockIdx.x * (KA2_W * KA2_TP) - 2;                       /* pose of slot 0 */
+  const int lo = max(P0, 0), hi = min(P0 + KA2_SLOTS, db.n_cap);          /* staged range: independent of n */
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    mbar_fence_init();
+  }
+  if (!active || P0 + 2 >= n) return;                                     /* uniform for the CTA, nothing in flight yet */
+  if (tid == 0) {
+    const uint32_t bytesP = (uint32_t)(hi - lo) * 32u;
+    const uint32_t bytesO = GT ? 0u : (uint32_t)db.M_cap * (uint32_t)sizeof(TebObstacle);
+    mbar_expect_tx(bar, bytesP + bytesO);
+    tma_load_1d(sP + (size_t)(lo - P0) * 4, db.poses + ((size_t)b * db.n_cap + lo) * 4, bytesP, bar);
+    if (bytesO) tma_load_1d(so_s, db.obstacles + (size_t)s * db.M_cap, bytesO, bar);
+  }
+  const int slot = warp * KA2_TP + lane;
+  const int i = P0 + slot;                                                /* pose / anchor of this lane */
+  const int q0 = P0 + 2 + warp * KA2_TP;                                  /* first pose this warp produces */
+  const bool out = (lane >= 2 && lane <= 30 && i < n);
+  /* while the copies are in flight: association word of the own pose, zeroed record and start block */
+  unsigned long long mask0 = 0ull;
+  if (out && kp.has_obst && i >= 1 && i <= n - 2)
+    mask0 = GT ? db.occ[((size_t)b * db.n_cap + i) * db.OW] : db.assoc[((size_t)b * db.n_cap + i) * db.MW];
+  {
+    double* rec = sW + lane;
+#pragma unroll
+    for (int e = 0; e < L::COUNT; ++e) rec[e * 32] = 0.0;
+    if (lane < KA2Smem::START) sStart[lane] = 0.0;
+  }
+  __syncthreads(); /* the mbarrier initialisation is visible to every waiting thread (the only block-wide barrier) */
+  mbar_wait(bar, 0);
+  if (q0 >= n) return; /* whole warp: tile beyond the band */
+  ka2_tile<HOLO, GEOM, OUT_DIRECT, GT>(db, kp, b, s, n, i, lane, sP + 4 * slot, GT ? db.obstacles + (size_t)s * db.M_cap : so_s,
+                                       mask0, sW, sStart, blockIdx.x * KA2_W + warp,
+                                       [] { __syncwarp(); /* start block zeroed by other lanes */ });
   if (!OUT_DIRECT && out) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); /* the slot must outlive the copy's read */
+}
+
+/* ------------------------------------------------------------------ k_linearize2p
+ * Kernel A in a PERSISTENT grid of one-warp CTAs, as many as are resident. A unit is one (band slot, tile) pair: slot y
+ * of the launch (band y, or a_list[y] for the first *a_cnt slots of a listed launch) and its tile t = 0 .. chunks - 1,
+ * unit y chunks + t. Warp w of G takes the units w, w + G, w + 2G, ... and skips, before it touches shared memory, a
+ * unit whose band is deferred (skip_tag) or inactive or whose first pose q0 = 29 t is >= n. Per unit it runs
+ * k_linearize2's P1 - P4 (ka2_tile: same lanes, same formulas, same fold order, the padded output slot and one bulk
+ * store per lane, the tile partials at (b, t)), so every output is the same bits. What differs:
+ *   - the tile's 33-pose window (poses q0 - 2 .. q0 + 30) is double-buffered on two per-warp mbarriers: the NEXT unit's
+ *     window is TMA-issued as soon as the current unit's P1 has run, so it arrives while P2 - P4 run;
+ *   - the previous unit's bulk stores drain while the current unit runs P1: the region they read becomes this unit's
+ *     records only after cp.async.bulk.wait_group.read 0;
+ *   - obstacle rows are read from global memory (L2: 64 B per row, one table per 32 bands on C3) with the staged
+ *     association walk; the GT build walks the occupancy words as k_linearize2<., ., ., true> does. A shared copy of
+ *     the table would cost a resident warp per SM (20.3 KB per warp with C3's 4 KB table: 11 warps instead of 12).
+ * No prologue per tile (mbarrier set-up, block barrier, cold window and table loads) and no idle warp in a band's last
+ * CTA. Non-holonomic builds: 15.6 KB of shared memory per warp, 12 warps per SM (the 168-register cap); holonomic
+ * builds: 20.5 KB, 10 warps per SM. */
+constexpr int KA2P_SLOTS = KA2_TP + 4; /* poses staged per unit: slot j <-> pose q0 - 2 + j */
+template <bool HOLO>
+__host__ __device__ constexpr size_t ka2p_smem_bytes() {
+  return (2 * KA2P_SLOTS * 4 + KA2Smem::warp_doubles<HOLO>()) * sizeof(double) + 2 * sizeof(uint64_t);
+}
+
+template <bool HOLO, bool GEOM, bool GT = false>
+__global__ void __launch_bounds__(32, 12) k_linearize2p(const __grid_constant__ DevBatch db, const __grid_constant__ KParams kp,
+                                                        int B) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  using L = JL<HOLO>;
+  const int lane = threadIdx.x;
+  double* sPw = reinterpret_cast<double*>(smem_raw);                        /* two windows of KA2P_SLOTS poses */
+  double* sW = sPw + 2 * KA2P_SLOTS * 4;                                     /* records / output slots */
+  double* sStart = sW + KA2Smem::rec_doubles<HOLO>();                        /* EdgeAccelerationStart rows */
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sW + KA2Smem::warp_doubles<HOLO>());
+
+  const int units = (db.a_list ? *db.a_cnt : B) * db.chunks;
+  const int step = (int)gridDim.x;
+  /* the first unit at or after u of this warp that has work: its band, n and first pose (every lane computes the same) */
+  auto next_unit = [&](int u, int& b, int& n, int& q0) {
+    for (; u < units; u += step) {
+      const int y = u / db.chunks;
+      const int t = u - y * db.chunks;
+      int bb = y;
+      if (db.a_list) bb = db.a_list[y];
+      else if (db.skip_tag != 0 && deferred_since(db.defer[y], db.skip_tag)) continue;
+      const int nn = db.n[bb];
+      if (!db.state[bb].active || t * KA2_TP >= nn) continue;
+      b = bb; n = nn; q0 = t * KA2_TP;
+      return u;
+    }
+    return units;
+  };
+  /* lane 0: the window of the unit (b, q0) into buffer k; the range staged does not depend on n, as in k_linearize2 */
+  auto issue = [&](int k, int b, int q0) {
+    const int P0 = q0 - 2;
+    const int lo = max(P0, 0), hi = min(P0 + KA2P_SLOTS, db.n_cap);
+    const uint32_t bytes = (uint32_t)(hi - lo) * 32u;
+    mbar_expect_tx(&bar[k], bytes);
+    tma_load_1d(sPw + (size_t)k * KA2P_SLOTS * 4 + (size_t)(lo - P0) * 4, db.poses + ((size_t)b * db.n_cap + lo) * 4, bytes, &bar[k]);
+  };
+
+  int b = 0, n = 0, q0 = 0;
+  int u = next_unit((int)blockIdx.x, b, n, q0);
+  if (u >= units) return;
+  if (lane == 0) {
+    mbar_init(&bar[0], 1);
+    mbar_init(&bar[1], 1);
+    mbar_fence_init();
+  }
+  __syncwarp();
+  if (lane == 0) issue(0, b, q0);
+  int k = 0;           /* buffer of the current unit */
+  uint32_t parity = 0; /* bit j: parity of bar[j]'s next phase */
+  while (u < units) {
+    const int s = db.scene_id[b];
+    const int i = q0 - 2 + lane;                                            /* pose / anchor of this lane */
+    unsigned long long mask0 = 0ull;
+    if (lane >= 2 && lane <= 30 && i < n && kp.has_obst && i >= 1 && i <= n - 2)
+      mask0 = GT ? db.occ[((size_t)b * db.n_cap + i) * db.OW] : db.assoc[((size_t)b * db.n_cap + i) * db.MW];
+    mbar_wait(&bar[k], (parity >> k) & 1u);
+    parity ^= 1u << k;
+    int b_nx = 0, n_nx = 0, q0_nx = 0, u_nx = units;
+    ka2_tile<HOLO, GEOM, false, GT>(db, kp, b, s, n, i, lane, sPw + (size_t)k * KA2P_SLOTS * 4 + 4 * lane,
+                                    db.obstacles + (size_t)s * db.M_cap, mask0, sW, sStart, q0 / KA2_TP, [&] {
+      /* the next unit's window goes into the other buffer, which the previous unit finished reading before its P4 */
+      u_nx = next_unit(u + step, b_nx, n_nx, q0_nx);
+      if (lane == 0 && u_nx < units) issue(k ^ 1, b_nx, q0_nx);
+      /* the previous unit's bulk stores have read their output slots: the region becomes this unit's records */
+      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+      __syncwarp();
+      double* rec = sW + lane;
+#pragma unroll
+      for (int e = 0; e < L::COUNT; ++e) rec[e * 32] = 0.0;
+      if (lane < KA2Smem::START) sStart[lane] = 0.0;
+      __syncwarp(); /* records and start block zeroed by every lane */
+    });
+    u = u_nx; b = b_nx; n = n_nx; q0 = q0_nx;
+    k ^= 1;
+  }
+  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); /* the slots must outlive the copies' reads */
 }
 
 }  // namespace tebgpu
