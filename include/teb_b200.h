@@ -37,7 +37,11 @@ extern "C" {
 #define TEBGPU_ERR_NO_DEVICE      -5
 
 /* per-band status bits written to status[] */
-#define TEB_STATUS_OPTIMIZED       1   /* optimizeTEB returned true (optimal_planner.cpp:220)      */
+#define TEB_STATUS_OPTIMIZED       1   /* optimizeTEB returned true (optimal_planner.cpp:230): every outer iteration
+                                          optimised the band, or iterations_outerloop == 0 (cost stays HUGE_VAL). Never
+                                          with iterations_innerloop == 0 and iterations_outerloop > 0: optimizeGraph
+                                          fails when optimize() runs no iteration (:393), so only the first outer
+                                          iteration's autoResize / buildGraph run */
 #define TEB_STATUS_TOO_FEW_POSES   2   /* sizePoses < min_samples guard (optimal_planner.cpp:377)   */
 #define TEB_STATUS_CHOL_FAILED     4   /* at least one trial factorisation hit a non-positive pivot */
 #define TEB_STATUS_NONFINITE       8   /* non-finite chi2 / lambda encountered                      */
@@ -400,6 +404,14 @@ int32_t tebgpu_read_linearize_outputs(tebgpu_ctx* ctx, int32_t B, int32_t n_cap,
  * need_out [B] 1 when the band is queued for another round, 0 when its iteration ended, -1 where no band decided;
  * next_list [B] and *next_len the bands queued, in queue order. */
 #define TEBGPU_EVAL_STATE 14
+/* The state every band was left in by the context's last tebgpu_optimize_batch(_device) call (a CUDA-graph replay
+ * included; tebgpu_build_system(_graph) and tebgpu_eval_trials overwrite it), in the TEBGPU_EVAL_STATE layout: lambda
+ * and nu of the last LM iteration, currentChi, chi2 by family at the current state (4) and at the last evaluated trial
+ * (4), status bits (without TEB_STATUS_OPTIMIZED, which only the outputs carry), active (0 once the band's last LM
+ * iteration returned Terminate, or the band failed), LM iterations. out [B][TEBGPU_EVAL_STATE], HOST buffer. Test entry
+ * point: it tells which exit each band's last LM iteration took (nu = 2^11 after ten rejected trials). Synchronises the
+ * context's stream; after tebgpu_optimize_batch_device on another stream, synchronise that stream first. */
+int32_t tebgpu_read_band_state(tebgpu_ctx* ctx, int32_t B, double* out);
 int32_t tebgpu_eval_trials(tebgpu_ctx* ctx, TebBatch* bt, int32_t outer_index, int32_t iteration, int32_t K, const double* dx,
                            const double* ok, const double* lambda_k, const double* state, const int32_t* qmax,
                            const int32_t* list, int32_t list_len, double* res_out, double* chi_lin, double* state_out,

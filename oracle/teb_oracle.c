@@ -1580,6 +1580,7 @@ static int lm_solve(Graph* g, int iteration, LMState* lm, const OracleOptions* o
   } while (!stop);
   st->chi2_final = currentChi;
   st->lambda_final = lm->lambda;
+  st->nu_final = lm->ni;
   if (opt->verbose) fprintf(stderr, "LMTRIALS %d %d %.6g %.6g\n", iteration, qmax, currentChi, lm->lambda);
   return !lm_terminates(qmax, rho, lm);
 }
@@ -1760,14 +1761,16 @@ int32_t teb_oracle_optimize(const TebParams* cfg, double* rec, int32_t* n_io, in
       /* optimizeGraph guards optimal_planner.cpp:370-382 */
       if (cfg->max_vel_x < 0.01) { st.status |= TEB_STATUS_DISABLED; success = 0; clear_graph(&g); break; }
       if (g.n < cfg->min_samples || g.n < 3) { st.status |= TEB_STATUS_TOO_FEW_POSES; success = 0; clear_graph(&g); break; }
-      st.lm_iters += optimize_graph_lm(&g, args->iterations_innerloop, &o, &st);
+      const int iters = optimize_graph_lm(&g, args->iterations_innerloop, &o, &st);
+      st.lm_iters += iters;
       st.n_edges_last = g.n_edges;
+      if (!iters) { success = 0; clear_graph(&g); break; } /* optimizeGraph: if (!iter) return false (:393) */
       if (args->compute_cost_afterwards && i == args->iterations_outerloop - 1 && cost_out)
         *cost_out = compute_current_cost(&g, args->obst_cost_scale, args->viapoint_cost_scale, args->alternative_time_cost);
       clear_graph(&g);
       weight_multiplier *= cfg->weight_adapt_factor;
     }
-    if (success && args->iterations_outerloop > 0) st.status |= TEB_STATUS_OPTIMIZED;
+    if (success) st.status |= TEB_STATUS_OPTIMIZED; /* optimizeTEB returned true: also with no outer iteration */
     *n_io = g.n;
     graph_free(&g);
   }

@@ -45,6 +45,7 @@ typedef struct OracleStats {
   int32_t n_edges_last;    /* active edges in the last graph                                          */
   int32_t status;          /* TEB_STATUS_* bits                                                       */
   int32_t n_final;
+  double  nu_final;        /* LM nu after the last LM iteration (2^11 after ten rejected trials)       */
 } OracleStats;
 
 /* One band, one optimizeTEB call (optimal_planner.cpp:182-231). rec [n_cap][4] in/out, n in/out. */

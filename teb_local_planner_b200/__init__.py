@@ -92,6 +92,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_eval_trials.restype = C.c_int32
     L.tebgpu_eval_trials.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp,
                                      C.c_int32, vp, vp, vp, vp, vp, vp, vp]
+    L.tebgpu_read_band_state.restype = C.c_int32
+    L.tebgpu_read_band_state.argtypes = [vp, C.c_int32, vp]
     L.tebgpu_select_best.restype = C.c_int32
     L.tebgpu_select_best.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double]
     L.tebgpu_auto_resize_host.restype = C.c_int32
@@ -349,6 +351,15 @@ class TebGpu:
                                                 chi_lin.ctypes.data, st_out.ctypes.data, q_out.ctypes.data, need.ctypes.data,
                                                 nxt.ctypes.data, C.byref(nlen)), "tebgpu_eval_trials")
         return dict(res=res, chi_lin=chi_lin, state=st_out, qmax=q_out, need=need, next_list=nxt[:nlen.value].copy())
+
+    def band_state(self, B):
+        """[B][EVAL_STATE] state of every band after the last optimize / optimize_device call (tebgpu_read_band_state):
+        lambda, nu, currentChi, chi2 by family at the current state (4) and at the last evaluated trial (4), status bits
+        (without OPTIMIZED), active, LM iterations"""
+        import numpy as np
+        out = np.empty((int(B), self.EVAL_STATE))
+        self._check(self.lib.tebgpu_read_band_state(self.ctx, int(B), out.ctypes.data), "tebgpu_read_band_state")
+        return out
 
     def close(self):
         if self.ctx:

@@ -835,7 +835,10 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
   int last_r1 = 0;      /* index g of round 1 of the latest LM iteration: its list = the side stream's bands */
   bool carried = false; /* the side stream already ran autoResize / buildGraph / kernel A of this outer iteration for the
                            bands that were still in a retry round when the previous outer iteration ended */
-  for (int o = 0; o < args->iterations_outerloop; ++o) {
+  /* optimizeGraph returns false when optimize() ran no iteration (optimal_planner.cpp:393), so with no inner iterations
+   * optimizeTEB stops after the first outer iteration's autoResize / buildGraph, unoptimised */
+  const int outer = args->iterations_innerloop == 0 && args->iterations_outerloop > 1 ? 1 : args->iterations_outerloop;
+  for (int o = 0; o < outer; ++o) {
     kp = make_kparams(ctx, bt, weight_multiplier);
     {
       DevBatch dm = db;
@@ -908,7 +911,7 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
             launch_linearize(ctx, dl, kp, B, bt->M_cap, ctx->side); ++launches;
             deferred_done = true;
             CUDA_TRY(ctx, cudaEventRecord(ctx->ev_join, ctx->side));
-          } else if (o + 1 < args->iterations_outerloop) {
+          } else if (o + 1 < outer) {
             /* last inner iteration: the side stream goes on with the next outer iteration's autoResize / buildGraph /
              * first kernel A for its bands (next weight multiplier), the main stream does the same for all others */
             const KParams kn = make_kparams(ctx, bt, weight_multiplier * p.weight_adapt_factor);
@@ -936,7 +939,11 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
     }
     weight_multiplier *= p.weight_adapt_factor; /* optimal_planner.cpp:227 */
   }
-  prof_begin(ctx, st, 5); k_finalize<<<gb, tb, 0, st>>>(db, kp, *args); ++launches; prof_end(ctx, st);
+  /* With no outer iteration optimizeTEB returns true without computing a cost (optimal_planner.cpp:230): k_finalize
+   * sets OPTIMIZED for a band that has not failed and leaves cost = HUGE_VAL when told of one iteration, no cost. */
+  TebOptimizeArgs fa = *args;
+  if (fa.iterations_outerloop == 0) { fa.iterations_outerloop = 1; fa.iterations_innerloop = 1; fa.compute_cost_afterwards = 0; }
+  prof_begin(ctx, st, 5); k_finalize<<<gb, tb, 0, st>>>(db, kp, fa); ++launches; prof_end(ctx, st);
   ctx->launches = launches;
   if (ctx->profiling && ctx->ev_used > 4096) { cudaStreamSynchronize(st); prof_collect(ctx); }
   CUDA_TRY(ctx, cudaGetLastError());
@@ -1300,6 +1307,23 @@ int32_t tebgpu_read_linearize_outputs(tebgpu_ctx* ctx, int32_t B, int32_t n_cap,
   return TEBGPU_OK;
 }
 
+/* one band's state in the TEBGPU_EVAL_STATE layout */
+static void pack_band_state(const BandState& x, double* s) {
+  s[0] = x.lambda; s[1] = x.ni; s[2] = x.current_chi;
+  for (int c = 0; c < 4; ++c) { s[3 + c] = x.parts_cur[c]; s[7 + c] = x.parts_last[c]; }
+  s[11] = x.status; s[12] = x.active; s[13] = x.lm_iters;
+}
+
+int32_t tebgpu_read_band_state(tebgpu_ctx* ctx, int32_t B, double* out) {
+  if (!ctx || !out || B < 1 || B > ctx->lim.max_bands) return TEBGPU_ERR_INVALID_ARG;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  std::vector<BandState> bs((size_t)B);
+  CUDA_TRY(ctx, cudaMemcpyAsync(bs.data(), ctx->state, (size_t)B * sizeof(BandState), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int b = 0; b < B; ++b) pack_band_state(bs[b], out + (size_t)b * TEBGPU_EVAL_STATE);
+  return TEBGPU_OK;
+}
+
 int32_t tebgpu_build_system_graph(tebgpu_ctx* ctx, const TebBatch* bt, int32_t outer_index, const int32_t* list,
                                   int32_t list_len, double* Hb_out, double* chi_fam_out, uint64_t* assoc_out,
                                   uint64_t* assoc3_out, uint64_t* occ_out, int32_t* via_idx_out, double* dyn_t_out) {
@@ -1588,13 +1612,7 @@ int32_t tebgpu_eval_trials(tebgpu_ctx* ctx, TebBatch* bt, int32_t outer_index, i
       for (int k = 0; k < K; ++k)
         for (int c = 0; c < 5; ++c) res_out[((size_t)b * K + k) * 5 + c] = hres[((size_t)b * SPEC_K_MAX + k) * RES_STRIDE + c];
     if (chi_lin) fold_chi_parts(parts.data(), db, b, bt->n[b], chi_lin + (size_t)b * 4);
-    if (state_out) {
-      double* s = state_out + (size_t)b * TEBGPU_EVAL_STATE;
-      const BandState& x = bs[b];
-      s[0] = x.lambda; s[1] = x.ni; s[2] = x.current_chi;
-      for (int c = 0; c < 4; ++c) { s[3 + c] = x.parts_cur[c]; s[7 + c] = x.parts_last[c]; }
-      s[11] = x.status; s[12] = x.active; s[13] = x.lm_iters;
-    }
+    if (state_out) pack_band_state(bs[b], state_out + (size_t)b * TEBGPU_EVAL_STATE);
     if (qmax_out) qmax_out[b] = hq[b];
     if (need_out) need_out[b] = hneed[b];
   }

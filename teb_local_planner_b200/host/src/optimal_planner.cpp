@@ -153,7 +153,7 @@ bool TebOptimalPlanner::optimizeTEB(int iterations_innerloop, int iterations_out
   if (!optimizeTebBatch(*cfg_, one, iterations_innerloop, iterations_outerloop, compute_cost_afterwards, obst_cost_scale,
                         viapoint_cost_scale, alternative_time_cost, gpu_))
     return false;
-  return optimized_;
+  return (status_ & TEB_STATUS_OPTIMIZED) != 0; /* optimizeTEB's return value; optimized_ may still be false (:230) */
 }
 
 static int rotdir_code(RotType r) { return r == RotType::left ? TEB_ROTDIR_LEFT : (r == RotType::right ? TEB_ROTDIR_RIGHT : TEB_ROTDIR_NONE); }
@@ -299,7 +299,9 @@ bool TebOptimalPlanner::runBatch(const TebConfig& cfg, const std::vector<TebOpti
     TebOptimalPlanner* pl = planners[b];
     pl->status_ = status[b];
     pl->chi2_ = chi2[b];
-    pl->optimized_ = (status[b] & TEB_STATUS_OPTIMIZED) != 0;
+    /* OPTIMIZED is optimizeTEB's return value (returned by optimizeTEB above); with no outer iteration optimizeTEB
+     * returns true with optimized_ still false */
+    pl->optimized_ = (status[b] & TEB_STATUS_OPTIMIZED) != 0 && iterations_outerloop > 0;
     if (pl->optimized_ || cfg.trajectory.teb_autosize) pl->teb().fromRecords(&poses[(size_t)b * n_cap * 4], n[b]);
     if (pl->optimized_ && compute_cost_afterwards) pl->cost_ = cost[b];
   }

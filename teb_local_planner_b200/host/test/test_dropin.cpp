@@ -204,6 +204,17 @@ static int gpu_checks() {
   ok = planner.plan(PoseSE2(-3.9, 0.01, 0.02), PoseSE2(4, 0, 0), &v0);
   std::printf("WARM_OK %d\n", ok ? 1 : 0);
   print_band("WARM", planner.teb());
+  {
+    /* optimizeTEB's argument edges (optimal_planner.cpp:182-231): no outer iteration returns true and leaves
+     * isOptimized() false; no inner iteration makes optimizeGraph fail (:393), so it returns false */
+    const int n_before = planner.teb().sizePoses();
+    const bool r0 = planner.optimizeTEB(5, 0, true);
+    const bool opt0 = planner.isOptimized();
+    CHECK(r0 && !opt0 && planner.teb().sizePoses() == n_before);
+    const bool r1 = planner.optimizeTEB(0, 3, true);
+    CHECK(!r1 && !planner.isOptimized());
+    std::printf("EDGES %d %d %d\n", r0 ? 1 : 0, opt0 ? 1 : 0, r1 ? 1 : 0);
+  }
 
   /* ---- HomotopyClassPlanner: three seeded candidates, one batched optimisation, selection */
   TebConfig hcfg;

@@ -22,7 +22,7 @@ class OracleOptions(C.Structure):
 class OracleStats(C.Structure):
     _fields_ = [("chi2_final", C.c_double), ("lambda_final", C.c_double), ("lm_iters", C.c_int32),
                 ("lm_trials", C.c_int32), ("rejected", C.c_int32), ("n_edges_last", C.c_int32),
-                ("status", C.c_int32), ("n_final", C.c_int32)]
+                ("status", C.c_int32), ("n_final", C.c_int32), ("nu_final", C.c_double)]
 
 
 def build_oracle():

@@ -122,6 +122,8 @@ def test_dropin_gpu_scenes_match_oracle(exe, oracle):
                                       jac_mode=oracle.JAC_ANALYTIC, n_cap=512)
     wgot = bands["WARM"]
     assert len(wgot) == len(wref) and np.abs(wgot - wref).max() < 1e-6
+    # optimizeTEB(5, 0) returns true with isOptimized() false; optimizeTEB(0, 3) returns false (optimal_planner.cpp:230, :393)
+    assert vals["EDGES"][0] == ["1", "0", "0"]
     # ---- HomotopyClassPlanner: 3 candidates optimised in one batch, costs with the selection scales, selectBestTeb
     hp = abi.default_params()
     hp.include_dynamic_obstacles = 0
