@@ -191,7 +191,8 @@ class TebGpu:
         bs = hb.struct()
         self._check(self.lib.tebgpu_h_signature(self.ctx, C.byref(bs), int(use_timediffs), out.ctypes.data, 0),
                     "tebgpu_h_signature")
-        return out if three_d else out[:, 0] + 1j * out[:, 1]
+        # the 2-D rows are (Re, Im) pairs: viewed, not composed as Re + 1j * Im, which turns an infinite Im into a NaN Re
+        return out if three_d else out.view(np.complex128)[:, 0].copy()
 
     # ---- the one collective (NCCL all-gather of the per-candidate costs), behind the C-ABI
     def comm_get_unique_id(self, out128):

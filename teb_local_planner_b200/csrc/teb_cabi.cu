@@ -1189,8 +1189,9 @@ int32_t tebgpu_h_signature(tebgpu_ctx* ctx, const TebBatch* bt, int32_t use_time
   int32_t rc = check_batch(ctx, bt);
   if (rc) return rc;
   if (!h_out) return TEBGPU_ERR_INVALID_ARG;
-  /* The 2-D signature is a product over the M - 1 obstacle differences (long double in the reference); at thousands of
-   * obstacles it leaves the fp64 range, so large scenes need a design of their own (DESIGN §9). */
+  /* The 2-D signature's product over the M - 1 obstacle differences (long double in the reference) is carried as an
+   * fp64 mantissa and a binary exponent, so its range is not what limits M. What does is the O(M^2) product per band,
+   * one CTA per band, and the staged table in shared memory: larger scenes need a design of their own (DESIGN §9). */
   if (global_table(bt->M_cap)) { ctx->err = "the H-signature supports at most 1024 obstacles per scene"; return TEBGPU_ERR_UNSUPPORTED; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   TebBatch d = *bt;

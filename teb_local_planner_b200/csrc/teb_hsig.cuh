@@ -7,9 +7,16 @@
  *   k_hsig3d  HSignature3d::calculateHSignature h_signature.h:282-353  one value per (band, obstacle)
  *
  * One CTA per band. The reference accumulates the 2-D signature in long double on one thread; here every (segment,
- * obstacle) term is evaluated by its own thread in fp64 and summed by a fixed-order block reduction.
+ * obstacle) term is evaluated by its own thread in fp64 and summed by a fixed-order block reduction. Two places where
+ * fp64 alone would part from long double are handled explicitly:
+ *   - the skip rule |o_l - o_j| < 0.05 is decided on the exact difference (hsig_closer_than_skip), not on the rounded one;
+ *   - A_l = f0 / prod_j (o_l - o_j) is carried as an fp64 mantissa and a binary exponent, and the sum over (k, l) is
+ *     taken at the largest exponent and scaled once, so that a partial product may leave the fp64 range (far obstacles
+ *     listed before near ones) and the result overflows / underflows only where (double) of the long double one does.
  */
 #pragma once
+
+#include <climits>
 
 #include "teb_kernels.cuh"
 
@@ -18,7 +25,22 @@ namespace tebgpu {
 constexpr int HSIG_THREADS = 256;
 
 __host__ __device__ inline size_t hsig_smem_bytes(int n_cap, int M_cap) {
-  return ((size_t)4 * (M_cap > 0 ? M_cap : 1) + (size_t)3 * n_cap + 2 * (HSIG_THREADS / 32) + 8) * sizeof(double);
+  const size_t Mc = M_cap > 0 ? M_cap : 1;
+  return ((size_t)4 * Mc + (size_t)3 * n_cap + 2 * (HSIG_THREADS / 32) + (Mc + 1) / 2 + 8) * sizeof(double);
+}
+
+/* |(ax, ay) - (bx, by)| < 0.05 on the exact difference: each coordinate difference as a two-sum (hi + lo exactly), the
+ * squared modulus as a double-double, compared with 0.05 * 0.05 as a double-double. Differs from the exact decision only
+ * within about 1e-30 relative of the threshold (long double's own decision: about 1e-19). */
+__device__ __forceinline__ bool hsig_closer_than_skip(double ax, double ay, double bx, double by) {
+  const double dx = ax - bx, vx = dx - ax, ex = (ax - (dx - vx)) + (-bx - vx);
+  const double dy = ay - by, vy = dy - ay, ey = (ay - (dy - vy)) + (-by - vy);
+  const double px = dx * dx, pxe = fma(dx, dx, -px);
+  const double py = dy * dy, pye = fma(dy, dy, -py);
+  const double s = px + py, vs = s - px, se = (px - (s - vs)) + (py - vs);
+  const double lo = se + pxe + pye + 2.0 * (dx * ex + dy * ey) + (ex * ex + ey * ey);
+  const double c = 0.05, c2 = c * c, c2e = fma(c, c, -c2);
+  return (s - c2) + (lo - c2e) < 0.0; /* s - c2 is exact here (Sterbenz): this path runs only when s is within 1e-12 of c2 */
 }
 
 __global__ void __launch_bounds__(HSIG_THREADS) k_hsig2d(DevBatch db, KParams kp, double* out) {
@@ -35,10 +57,13 @@ __global__ void __launch_bounds__(HSIG_THREADS) k_hsig2d(DevBatch db, KParams kp
   double* spx = sAi + Mc;
   double* spy = spx + db.n_cap;
   double* sred = spy + 2 * db.n_cap; /* [2][warps] */
+  int* sE = reinterpret_cast<int*>(sred + 2 * (HSIG_THREADS / 32)); /* [Mc] binary exponent of A_l */
+  __shared__ int sEmax;
   if (M == 0 || n < 1) { /* obstacles->empty(): hsignature_ = 0 (:100-104) */
     if (tid == 0) { out[2 * b] = 0; out[2 * b + 1] = 0; }
     return;
   }
+  if (tid == 0) sEmax = INT_MIN;
   const TebObstacle* go = db.obstacles + (size_t)sc * db.M_cap;
   for (int l = tid; l < M; l += HSIG_THREADS) { sox[l] = go[l].x; soy[l] = go[l].y; } /* getCentroidCplx() */
   const double* P = db.poses + (size_t)b * db.n_cap * 4;
@@ -53,23 +78,42 @@ __global__ void __launch_bounds__(HSIG_THREADS) k_hsig2d(DevBatch db, KParams kp
   double blx, bly, trx, try_;
   if (hypot(dx, dy) < 3.0) { blx = sx; bly = sy - 3; trx = sx + 3; try_ = sy + 3; }
   else { blx = sx + dy; bly = sy - dx; trx = sx + dx - dy; try_ = sy + dy + dx; } /* normal = (-dy, dx) */
-  /* A_l = f0(o_l) / prod_{j != l, |o_l - o_j| >= 0.05} (o_l - o_j)  (:149-163) */
+  /* A_l = f0(o_l) / prod_{j != l, |o_l - o_j| >= 0.05} (o_l - o_j)  (:149-163), as (ar + i ai) * 2^E: the long double
+   * product of the reference may pass far outside the fp64 range on its way to an O(1) value */
   for (int l = tid; l < M; l += HSIG_THREADS) {
     const double ox = sox[l], oy = soy[l];
     const double pa = kp.p.h_signature_prescaler * (double)a;
     double ar = pa * (ox - blx), ai = pa * (oy - bly);
     ar *= (double)bq; ai *= (double)bq;
     { const double cr = ox - trx, ci = oy - try_; const double tr = ar * cr - ai * ci; ai = ar * ci + ai * cr; ar = tr; }
+    int E = 0;
     for (int j = 0; j < M; ++j) {
       if (j == l) continue;
       const double cr = ox - sox[j], ci = oy - soy[j];
-      if (hypot(cr, ci) < 0.05) continue; /* skip really close obstacles */
       const double den = cr * cr + ci * ci;
+      /* skip really close obstacles; near the threshold the decision is taken on the exact difference */
+      if (den < 0.0025 * (1 - 1e-12)) continue;
+      if (den <= 0.0025 * (1 + 1e-12) && hsig_closer_than_skip(ox, oy, sox[j], soy[j])) continue;
       const double tr = (ar * cr + ai * ci) / den;
       ai = (ai * cr - ar * ci) / den;
       ar = tr;
+      const double mx = fmax(fabs(ar), fabs(ai));
+      if ((mx > 0x1p+400 || mx < 0x1p-400) && mx > 0 && mx < INFINITY) { /* renormalise: exact scaling by 2^-e */
+        int e;
+        frexp(mx, &e);
+        ar = ldexp(ar, -e); ai = ldexp(ai, -e);
+        E += e;
+      }
     }
     sAr[l] = ar; sAi[l] = ai;
+    sE[l] = (ar == 0 && ai == 0) ? INT_MIN : E;
+    if (ar != 0 || ai != 0) atomicMax(&sEmax, E);
+  }
+  __syncthreads();
+  /* every A_l at the largest exponent (exact unless a term falls below 2^-1022 of the largest one) */
+  const int Emax = sEmax;
+  for (int l = tid; l < M; l += HSIG_THREADS) {
+    if (sE[l] != INT_MIN) { sAr[l] = ldexp(sAr[l], sE[l] - Emax); sAi[l] = ldexp(sAi[l], sE[l] - Emax); }
   }
   __syncthreads();
   /* sum over segments k and obstacles l of A_l * (ln|z2-o|/|z1-o| + i * smallest-magnitude angle difference) (:165-182) */
@@ -99,6 +143,8 @@ __global__ void __launch_bounds__(HSIG_THREADS) k_hsig2d(DevBatch db, KParams kp
   if (tid == 0) {
     double r = 0, i = 0;
     for (int q = 0; q < HSIG_THREADS / 32; ++q) { r += sred[q]; i += sred[HSIG_THREADS / 32 + q]; }
+    /* one scaling to the true exponent: inf / 0 exactly where the long double value lies outside the fp64 range */
+    if (Emax != INT_MIN) { r = ldexp(r, Emax); i = ldexp(i, Emax); }
     out[2 * b] = r; out[2 * b + 1] = i;
   }
 }
@@ -126,7 +172,7 @@ __global__ void __launch_bounds__(HSIG_THREADS) k_hsig3d(DevBatch db, KParams kp
   __syncthreads();
   const TebObstacle* go = db.obstacles + (size_t)sc * db.M_cap;
   const int lane = tid & 31, w = tid >> 5;
-  for (int l = w; l < db.M_cap; l += HSIG_THREADS / 32) {
+  for (int l = w; l < Mc; l += HSIG_THREADS / 32) { /* rows past M (and the one row of M_cap = 0) are written as 0 */
     double H = 0;
     if (l < M) {
       /* obstacle world line s1 -> s2 over 120 s (predictCentroidConstantVelocity), the "conductor" (:291-298) */

@@ -189,10 +189,11 @@ bool TebOptimalPlanner::runBatch(const TebConfig& cfg, const std::vector<TebOpti
   for (auto* oc : scenes)
     if (oc) M_cap = std::max(M_cap, (int)oc->size());
   if (M_cap > 16384) { std::fprintf(stderr, "optimizeTEB: more than 16384 obstacles per scene is not supported\n"); return false; }
-  /* the 2-D H-signature multiplies M - 1 obstacle differences: beyond 1024 obstacles the product leaves the fp64 range */
+  /* the H-signature kernels stage a scene of at most 1024 obstacles in shared memory and form the 2-D signature's
+   * product over the M - 1 obstacle differences, O(M^2) per band, in one CTA */
   if (hsig_out && M_cap > 1024) {
-    std::fprintf(stderr, "H-signature: more than 1024 obstacles per scene is not supported (the product over the obstacles "
-                         "leaves the double range)\n");
+    std::fprintf(stderr, "H-signature: more than 1024 obstacles per scene is not supported (the obstacle table is staged "
+                         "in shared memory)\n");
     return false;
   }
   std::vector<TebObstacle> obst((size_t)S * M_cap);
