@@ -224,8 +224,28 @@ typedef struct tebgpu_ctx tebgpu_ctx;
  * (divergence_detection_enable=0, divergence_detection_max_chi_squared=10). */
 void tebgpu_default_params(TebParams* p);
 
+/* Per-band inputs and outputs of TebOptimalPlanner::plan followed by getVelocityCommand (tebgpu_plan_batch). HOST
+ * pointers for tebgpu_plan_batch, DEVICE pointers for tebgpu_plan_batch_device, like the TebBatch they go with. */
+typedef struct TebPlanInput {
+  const double*  start;          /* [B][3] x, y, theta: plan(start, goal, ...) (optimal_planner.cpp:290); unused with a plan */
+  const double*  goal;           /* [B][3] */
+  const double*  initial_plan;   /* [B][P_cap][3] x, y, yaw, or NULL: plan(initial_plan, ...) (:247); start and goal are
+                                    then the plan's first and last point (:257-258) */
+  const int32_t* plan_count;     /* [B] points of each band's plan, 1 .. P_cap, or NULL: P_cap points each */
+  int32_t        P_cap;          /* plan rows per band (stride) */
+  int32_t        look_ahead_poses;                   /* getVelocityCommand argument (control_look_ahead_poses) */
+  int32_t        prevent_look_ahead_poses_near_goal; /* trajectory.prevent_look_ahead_poses_near_goal (:1145) */
+  int32_t        _pad;
+  double*        cmd;            /* [B][4] out: vx, vy, omega, ok (getVelocityCommand's return value, 1 / 0) */
+  int32_t*       path;           /* [B] out or NULL: TEB_PLAN_PATH_* */
+} TebPlanInput;
+#define TEB_PLAN_PATH_NONE  -1   /* band left as it was: TEB_STATUS_BAD_INPUT or TEB_STATUS_CAPACITY */
+#define TEB_PLAN_PATH_COLD   0   /* n == 0 (!teb_.isInit()): initTrajectoryToGoal */
+#define TEB_PLAN_PATH_WARM   1   /* goal moved < force_reinit_new_goal_dist and turned < _angular: updateAndPruneTEB */
+#define TEB_PLAN_PATH_REINIT 2   /* otherwise: clearTimedElasticBand + initTrajectoryToGoal */
+
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
- * 3 TebOptimizeArgs, 4 TebGpuLimits. */
+ * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -249,6 +269,29 @@ int32_t tebgpu_optimize_batch(tebgpu_ctx* ctx, const TebBatch* batch, const TebO
 int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebOptimizeArgs* args,
                                      void* cuda_stream);
 int32_t tebgpu_synchronize(tebgpu_ctx* ctx);
+
+/* TebOptimalPlanner::plan (optimal_planner.cpp:247-321) followed by getVelocityCommand (:1135-1168) for every band of
+ * the batch, the per-cycle work of a controller:
+ *   1. n[b] == 0: cold start, initTrajectoryToGoal(start, goal, 0, max_vel_x, min_samples, ...) or, with a plan,
+ *      initTrajectoryToGoal(plan, max_vel_x, max_vel_theta, global_plan_overwrite_orientation, min_samples,
+ *      allow_init_with_backwards_motion). n[b] > 0: warm start, updateAndPruneTEB(start, goal, min_samples), when the goal
+ *      lies closer than force_reinit_new_goal_dist to the band's last pose and its heading differs by less than
+ *      force_reinit_new_goal_angular (both strict); otherwise the band is cleared and initialised again.
+ *   2. optimizeTEB(no_inner_iterations, no_outer_iterations) exactly as tebgpu_optimize_batch runs it with `args`
+ *      (pass the parameter block's iteration counts for plan()); vel_start / vel_goal are read from the batch as there,
+ *      so start_vel == NULL and free_goal_vel are expressed through their active flags. cost, chi2, status and
+ *      lm_iters mean what they mean for tebgpu_optimize_batch.
+ *   3. cmd[b] = getVelocityCommand(look_ahead_poses) on the optimised band.
+ * A band whose initialisation needs more than n_cap poses is left as it was and gets TEB_STATUS_CAPACITY; its command
+ * is read from the band as it was. tebgpu_plan_batch: HOST buffers, synchronous; a non-finite start, goal or plan row,
+ * or a plan_count outside 1 .. P_cap, returns TEBGPU_ERR_INVALID_ARG before anything runs. It keeps a device copy of
+ * the plans sized by the largest P_cap it has been called with (allocated by the first call that needs more; there is
+ * no P_cap limit to set). tebgpu_plan_batch_device: DEVICE buffers, stream ordered as tebgpu_optimize_batch_device,
+ * does not synchronise; such a band is left as it was and gets TEB_STATUS_BAD_INPUT, the other bands are planned. In
+ * the CUDA-graph replay of tebgpu_set_graph the whole cycle (plan, optimize, command) is one captured sequence. */
+int32_t tebgpu_plan_batch(tebgpu_ctx* ctx, TebBatch* batch, const TebPlanInput* plan, const TebOptimizeArgs* args);
+int32_t tebgpu_plan_batch_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebPlanInput* plan,
+                                 const TebOptimizeArgs* args, void* cuda_stream);
 
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded
@@ -298,6 +341,8 @@ int32_t tebgpu_set_graph(tebgpu_ctx* ctx, int32_t mode);
  * the accumulated milliseconds and launch count since profiling was enabled, and resets the accumulators. */
 int32_t tebgpu_set_profiling(tebgpu_ctx* ctx, int32_t enable);
 int32_t tebgpu_get_kernel_times(tebgpu_ctx* ctx, double ms_out[9], int64_t count_out[9]);
+/* Same for the two launches only the plan entry points issue: 0 k_plan_begin, 1 k_velocity_command. */
+int32_t tebgpu_get_plan_kernel_times(tebgpu_ctx* ctx, double ms_out[2], int64_t count_out[2]);
 
 /* HomotopyClassPlanner::calculateEquivalenceClass (homotopy_class_planner.hpp:46-63) for every band of the batch, i.e.
  * the step that decides which candidates are kept before they are optimised (renewAndAnalyzeOldTebs,

@@ -44,6 +44,13 @@ def load_library(build_if_missing=False):
     L.tebgpu_optimize_batch.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebOptimizeArgs)]
     L.tebgpu_optimize_batch_device.restype = C.c_int32
     L.tebgpu_optimize_batch_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebOptimizeArgs), vp]
+    L.tebgpu_plan_batch.restype = C.c_int32
+    L.tebgpu_plan_batch.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebPlanInput), C.POINTER(abi.TebOptimizeArgs)]
+    L.tebgpu_plan_batch_device.restype = C.c_int32
+    L.tebgpu_plan_batch_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebPlanInput),
+                                           C.POINTER(abi.TebOptimizeArgs), vp]
+    L.tebgpu_get_plan_kernel_times.restype = C.c_int32
+    L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
     L.tebgpu_set_linearize_variant.argtypes = [vp, C.c_int32]
     L.tebgpu_set_speculation.restype = C.c_int32
@@ -98,7 +105,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_select_best.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double]
     L.tebgpu_auto_resize_host.restype = C.c_int32
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
-    for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits)):
+    for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
+                                abi.TebPlanInput)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -146,6 +154,56 @@ class TebGpu:
     def optimize_device(self, batch_struct, args, stream=None):
         self._check(self.lib.tebgpu_optimize_batch_device(self.ctx, C.byref(batch_struct), C.byref(args), stream),
                     "tebgpu_optimize_batch_device")
+
+    def plan(self, hb, start, goal, args, look_ahead_poses=1, prevent_near_goal=0, initial_plan=None, plan_count=None,
+             path=True):
+        """TebOptimalPlanner::plan followed by getVelocityCommand for every band (tebgpu_plan_batch), host buffers.
+
+        hb (abi.HostBatch) is updated in place: a band with n == 0 is initialised from start to goal, a band with n > 0
+        is warm started (updateAndPruneTEB) or re-initialised when the goal jumped, then optimised with `args`.
+        start, goal: [B][3] (x, y, theta); or initial_plan [B][P_cap][3] (x, y, yaw) with plan_count [B] (None: P_cap
+        points each), start / goal are then ignored. Returns (cmd [B][4] = vx, vy, omega, ok, path [B] TEB_PLAN_PATH_*)."""
+        import numpy as np
+        B = hb.B
+        f64 = lambda a, shape: None if a is None else np.ascontiguousarray(np.broadcast_to(a, shape), dtype=np.float64)
+        cmd = np.zeros((B, 4))
+        pth = np.full(B, -2, np.int32) if path else None
+        pi = abi.TebPlanInput()
+        if initial_plan is not None:
+            ip = np.ascontiguousarray(initial_plan, dtype=np.float64)
+            pc = None if plan_count is None else np.ascontiguousarray(plan_count, dtype=np.int32)
+            pi.initial_plan, pi.plan_count, pi.P_cap = abi.ptr(ip), abi.ptr(pc), ip.shape[1]
+        else:
+            s, g = f64(start, (B, 3)), f64(goal, (B, 3))
+            pi.start, pi.goal = abi.ptr(s), abi.ptr(g)
+        pi.look_ahead_poses, pi.prevent_look_ahead_poses_near_goal = int(look_ahead_poses), int(prevent_near_goal)
+        pi.cmd, pi.path = abi.ptr(cmd), abi.ptr(pth)
+        bs = hb.struct()
+        self._check(self.lib.tebgpu_plan_batch(self.ctx, C.byref(bs), C.byref(pi), C.byref(args)), "tebgpu_plan_batch")
+        return cmd, pth
+
+    def plan_device(self, batch_struct, args, cmd, start=None, goal=None, path=None, initial_plan=None, plan_count=None,
+                    P_cap=0, look_ahead_poses=1, prevent_near_goal=0, stream=None):
+        """tebgpu_plan_batch_device: the same cycle over DEVICE memory (batch_struct: an abi.TebBatch of device
+        pointers). cmd [B][4] float64, start / goal [B][3] float64, path [B] int32 (or None), initial_plan
+        [B][P_cap][3] float64 with plan_count [B] int32 (or None): device pointers as ints, or torch tensors. Stream
+        ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise."""
+        addr = lambda t: None if t is None else (t.data_ptr() if hasattr(t, "data_ptr") else int(t))
+        pi = abi.TebPlanInput()
+        pi.start, pi.goal, pi.initial_plan, pi.plan_count = addr(start), addr(goal), addr(initial_plan), addr(plan_count)
+        if initial_plan is not None and not P_cap and hasattr(initial_plan, "shape"):
+            P_cap = initial_plan.shape[1]
+        pi.P_cap = int(P_cap)
+        pi.look_ahead_poses, pi.prevent_look_ahead_poses_near_goal = int(look_ahead_poses), int(prevent_near_goal)
+        pi.cmd, pi.path = addr(cmd), addr(path)
+        self._check(self.lib.tebgpu_plan_batch_device(self.ctx, C.byref(batch_struct), C.byref(pi), C.byref(args), stream),
+                    "tebgpu_plan_batch_device")
+
+    def plan_kernel_times(self):
+        """{kernel name: (total ms, launches)} of k_plan_begin and k_velocity_command since profiling was enabled"""
+        ms, cnt = (C.c_double * 2)(), (C.c_int64 * 2)()
+        self._check(self.lib.tebgpu_get_plan_kernel_times(self.ctx, C.byref(ms), C.byref(cnt)), "tebgpu_get_plan_kernel_times")
+        return {"k_plan_begin": (ms[0], cnt[0]), "k_velocity_command": (ms[1], cnt[1])}
 
     def set_linearize_variant(self, v):
         self._check(self.lib.tebgpu_set_linearize_variant(self.ctx, int(v)), "tebgpu_set_linearize_variant")

@@ -104,6 +104,16 @@ class TebOptimizeArgs(C.Structure):
                 ("obst_cost_scale", _d), ("viapoint_cost_scale", _d)]
 
 
+class TebPlanInput(C.Structure):
+    """TebOptimalPlanner::plan + getVelocityCommand per band (tebgpu_plan_batch): host or device pointers"""
+    _fields_ = [("start", C.c_void_p), ("goal", C.c_void_p), ("initial_plan", C.c_void_p), ("plan_count", C.c_void_p),
+                ("P_cap", _i), ("look_ahead_poses", _i), ("prevent_look_ahead_poses_near_goal", _i), ("_pad", _i),
+                ("cmd", C.c_void_p), ("path", C.c_void_p)]
+
+
+TEB_PLAN_PATH_NONE, TEB_PLAN_PATH_COLD, TEB_PLAN_PATH_WARM, TEB_PLAN_PATH_REINIT = -1, 0, 1, 2
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

@@ -17,6 +17,7 @@
 #include "teb_solve_warp.cuh"
 #include "teb_solve_lat.cuh"
 #include "teb_hsig.cuh"
+#include "teb_plan.cuh"
 #include "teb_comm.h"
 #include <cstdlib>
 
@@ -97,14 +98,20 @@ struct tebgpu_ctx {
   int32_t* d_ocount = nullptr; double* d_via = nullptr; int32_t* d_vcount = nullptr; double* d_vs = nullptr;
   double* d_vg = nullptr; int32_t* d_rot = nullptr; double* d_cost = nullptr; double* d_chi2 = nullptr;
   int32_t* d_status = nullptr; int32_t* d_iters = nullptr;
+  /* plan entry points: k_plan_begin's per-band status for k_begin, and the host-buffer entry point's mirrors */
+  int32_t* plan_status = nullptr;     /* [max_bands] */
+  double* d_start = nullptr; double* d_goal = nullptr; int32_t* d_pcount = nullptr; double* d_cmd = nullptr;
+  int32_t* d_path = nullptr;
+  double* d_plan = nullptr;           /* [max_bands][plan_rows][3], grown to the largest P_cap tebgpu_plan_batch has seen */
+  size_t plan_rows = 0;
   size_t smem_a = 0, smem_b = 0, smem_g = 0;
   /* profiling */
   bool profiling = false;
   std::vector<cudaEvent_t> ev;      /* pairs */
   std::vector<int> ev_kind;
   size_t ev_used = 0;
-  double prof_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  int64_t prof_cnt[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  double prof_ms[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; /* 9 k_plan_begin, 10 k_velocity_command */
+  int64_t prof_cnt[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 };
 
 static void prof_begin(tebgpu_ctx* c, cudaStream_t st, int kind) {
@@ -185,6 +192,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 2: return (int32_t)sizeof(TebBatch);
     case 3: return (int32_t)sizeof(TebOptimizeArgs);
     case 4: return (int32_t)sizeof(TebGpuLimits);
+    case 5: return (int32_t)sizeof(TebPlanInput);
     default: return -1;
   }
 }
@@ -213,7 +221,8 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
 static void free_all(tebgpu_ctx* c) {
   void* ptrs[] = {c->Lf2, c->dx2, c->arrive, c->d_gather, c->d_hsig, c->assoc3, c->occ, c->dyn_idx, c->dyn_cnt, c->rhs, c->dmax_parts, c->spec.Lf, c->spec.dx, c->spec.res, c->spec.need, c->spec.qmax, c->spec.cnt, c->spec.list, c->defer, c->d_fp, c->d_pverts, c->Hb, c->assoc, c->dyn_t, c->via_idx, c->chi_parts, c->state, c->d_poses, c->d_n, c->d_scene,
                   c->d_obst, c->d_ocount, c->d_via, c->d_vcount, c->d_vs, c->d_vg, c->d_rot, c->d_cost, c->d_chi2,
-                  c->d_status, c->d_iters};
+                  c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
+                  c->d_plan};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -331,6 +340,12 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaMalloc(&c->d_pverts, (S * (size_t)(lim->max_obst_vertices > 0 ? lim->max_obst_vertices : 1)) * 2 * sizeof(double)));
   CUDA_TRY(c, cudaMalloc(&c->d_hsig, B * (Ms > 2 ? Ms : 2) * sizeof(double))); /* tebgpu_h_signature: M_cap <= 1024 */
   CUDA_TRY(c, cudaMalloc(&c->d_vcount, B * sizeof(int32_t)));
+  CUDA_TRY(c, cudaMalloc(&c->plan_status, B * sizeof(int32_t)));
+  CUDA_TRY(c, cudaMalloc(&c->d_start, B * 3 * sizeof(double)));
+  CUDA_TRY(c, cudaMalloc(&c->d_goal, B * 3 * sizeof(double)));
+  CUDA_TRY(c, cudaMalloc(&c->d_pcount, B * sizeof(int32_t)));
+  CUDA_TRY(c, cudaMalloc(&c->d_cmd, B * 4 * sizeof(double)));
+  CUDA_TRY(c, cudaMalloc(&c->d_path, B * sizeof(int32_t)));
   CUDA_TRY(c, cudaMalloc(&c->d_vs, B * 4 * sizeof(double)));
   CUDA_TRY(c, cudaMalloc(&c->d_vg, B * 4 * sizeof(double)));
   CUDA_TRY(c, cudaMalloc(&c->d_rot, B * sizeof(int32_t)));
@@ -753,9 +768,12 @@ static int launch_spec_solve(const tebgpu_ctx* ctx, const DevBatch& db, const Sp
   return 1;
 }
 
-/* the launch sequence of one optimizeTEB over the batch, issued on `st` (directly, or into a stream capture) */
-static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args, cudaStream_t st) {
+/* the launch sequence of one optimizeTEB over the batch, issued on `st` (directly, or into a stream capture);
+ * pre_status: k_plan_begin's per-band status (plan entry points), or NULL */
+static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args, cudaStream_t st,
+                              const int32_t* pre_status = nullptr) {
   DevBatch db = make_devbatch(ctx, bt);
+  db.pre_status = pre_status;
   const TebParams& p = ctx->params;
   const int B = bt->B;
   const int tb = 128, gb = ((B > bt->S ? B : bt->S) + tb - 1) / tb;
@@ -955,7 +973,8 @@ static int32_t issue_optimize(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
  * distinct key (fork / join of the retry side stream included) and replayed afterwards: one graph launch instead of
  * ~130-170 kernel launches. That only matters in the latency regime (a single planning request: kernels of 10-50 us), so
  * graphs are used there by default (tebgpu_set_graph: 0 never, 1 always, 2 automatic). */
-static uint64_t graph_key(const tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* a, cudaStream_t st) {
+static uint64_t graph_key(const tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* a, cudaStream_t st,
+                          const TebPlanInput* plan) {
   uint64_t h = 1469598103934665603ull;
   auto mix = [&](const void* p, size_t nbytes) {
     const unsigned char* c = static_cast<const unsigned char*>(p);
@@ -967,21 +986,36 @@ static uint64_t graph_key(const tebgpu_ctx* ctx, const TebBatch* bt, const TebOp
   const int sw[12] = {ctx->solver, ctx->spec_k, ctx->linearize_variant, ctx->ka_staged, ctx->eval_v1, ctx->overlap, ctx->eval_minb, ctx->warp_solver, ctx->eval_mode, ctx->split, ctx->solve_form, ctx->ka_persist};
   mix(sw, sizeof(sw));
   mix(&st, sizeof(st));
+  if (plan) mix(plan, sizeof(*plan)); /* the plan entry points' cycle: its buffers and read-out arguments */
   return h;
 }
 
-int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args, void* cuda_stream) {
-  int32_t rc = check_batch(ctx, bt);
+/* the launch sequence of the plan entry points: plan / warm start, the optimize sequence, the velocity command */
+static int32_t issue_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebPlanInput* plan, const TebOptimizeArgs* args,
+                          cudaStream_t st) {
+  const DevBatch db = make_devbatch(ctx, bt);
+  const int B = bt->B;
+  prof_begin(ctx, st, 9);
+  k_plan_begin<<<(B + 3) / 4, 128, 0, st>>>(db, ctx->params, *plan, ctx->plan_status);
+  prof_end(ctx, st);
+  const int32_t rc = issue_optimize(ctx, bt, args, st, ctx->plan_status);
   if (rc) return rc;
-  rc = check_path(ctx, bt, true);
-  if (rc) return rc;
-  if (!args || args->iterations_innerloop < 0 || args->iterations_outerloop < 0) { ctx->err = "bad optimize args"; return TEBGPU_ERR_INVALID_ARG; }
-  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  prof_begin(ctx, st, 10);
+  k_velocity_command<<<(B + 127) / 128, 128, 0, st>>>(db, ctx->params, *plan);
+  prof_end(ctx, st);
+  ctx->launches += 2;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+/* one optimize call (plan == NULL) or plan cycle, launched directly or through a captured CUDA graph */
+static int32_t run_sequence(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args, cudaStream_t st,
+                            const TebPlanInput* plan) {
+  auto issue = [&]() { return plan ? issue_plan(ctx, bt, plan, args, st) : issue_optimize(ctx, bt, args, st); };
   const bool latency_regime = (long long)bt->B * 8 <= (long long)ctx->sms * 4 * 32;
   const bool use_graph = !ctx->profiling && (ctx->graph_mode == 1 || (ctx->graph_mode == 2 && latency_regime));
-  if (!use_graph) return issue_optimize(ctx, bt, args, st);
-  const uint64_t key = graph_key(ctx, bt, args, st);
+  if (!use_graph) return issue();
+  const uint64_t key = graph_key(ctx, bt, args, st, plan);
   for (auto& e : ctx->graphs)
     if (e.key == key) {
       e.stamp = ++ctx->graph_clock;
@@ -991,7 +1025,7 @@ int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const 
       return TEBGPU_OK;
     }
   CUDA_TRY(ctx, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  rc = issue_optimize(ctx, bt, args, st);
+  int32_t rc = issue();
   cudaGraph_t graph = nullptr;
   const cudaError_t ce = cudaStreamEndCapture(st, &graph);
   if (rc != TEBGPU_OK || ce != cudaSuccess || !graph) {
@@ -999,7 +1033,7 @@ int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const 
     cudaGetLastError();
     if (rc == TEBGPU_OK) { /* capture itself failed: run the sequence directly */
       ctx->graph_mode = 0;
-      return issue_optimize(ctx, bt, args, st);
+      return issue();
     }
     return rc;
   }
@@ -1008,7 +1042,7 @@ int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const 
   ent.spec_k = ctx->last_spec_k; ent.spec_first = ctx->last_spec_first;
   const cudaError_t ie = cudaGraphInstantiate(&ent.exec, graph, 0);
   cudaGraphDestroy(graph);
-  if (ie != cudaSuccess) { cudaGetLastError(); ctx->graph_mode = 0; return issue_optimize(ctx, bt, args, st); }
+  if (ie != cudaSuccess) { cudaGetLastError(); ctx->graph_mode = 0; return issue(); }
   if (ctx->graphs.size() >= 8) { /* drop the least recently used graph */
     size_t old = 0;
     for (size_t k = 1; k < ctx->graphs.size(); ++k)
@@ -1019,6 +1053,17 @@ int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const 
   ctx->graphs.push_back(ent);
   CUDA_TRY(ctx, cudaGraphLaunch(ent.exec, st));
   return TEBGPU_OK;
+}
+
+int32_t tebgpu_optimize_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args, void* cuda_stream) {
+  int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  rc = check_path(ctx, bt, true);
+  if (rc) return rc;
+  if (!args || args->iterations_innerloop < 0 || args->iterations_outerloop < 0) { ctx->err = "bad optimize args"; return TEBGPU_ERR_INVALID_ARG; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  return run_sequence(ctx, bt, args, st, nullptr);
 }
 
 int32_t tebgpu_set_warp_solver(tebgpu_ctx* ctx, int32_t mode) {
@@ -1045,7 +1090,7 @@ int32_t tebgpu_set_profiling(tebgpu_ctx* ctx, int32_t enable) {
   cudaStreamSynchronize(ctx->stream);
   prof_collect(ctx);
   ctx->profiling = enable != 0;
-  for (int k = 0; k < 9; ++k) { ctx->prof_ms[k] = 0; ctx->prof_cnt[k] = 0; }
+  for (int k = 0; k < 11; ++k) { ctx->prof_ms[k] = 0; ctx->prof_cnt[k] = 0; }
   return TEBGPU_OK;
 }
 
@@ -1055,6 +1100,15 @@ int32_t tebgpu_get_kernel_times(tebgpu_ctx* ctx, double ms_out[9], int64_t count
   CUDA_TRY(ctx, cudaDeviceSynchronize());
   prof_collect(ctx);
   for (int k = 0; k < 9; ++k) { ms_out[k] = ctx->prof_ms[k]; count_out[k] = ctx->prof_cnt[k]; ctx->prof_ms[k] = 0; ctx->prof_cnt[k] = 0; }
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_get_plan_kernel_times(tebgpu_ctx* ctx, double ms_out[2], int64_t count_out[2]) {
+  if (!ctx || !ms_out || !count_out) return TEBGPU_ERR_INVALID_ARG;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  CUDA_TRY(ctx, cudaDeviceSynchronize());
+  prof_collect(ctx);
+  for (int k = 0; k < 2; ++k) { ms_out[k] = ctx->prof_ms[9 + k]; count_out[k] = ctx->prof_cnt[9 + k]; ctx->prof_ms[9 + k] = 0; ctx->prof_cnt[9 + k] = 0; }
   return TEBGPU_OK;
 }
 
@@ -1153,6 +1207,94 @@ int32_t tebgpu_optimize_batch(tebgpu_ctx* ctx, const TebBatch* bt, const TebOpti
   if (bt->chi2) CUDA_TRY(ctx, cudaMemcpyAsync(bt->chi2, ctx->d_chi2, B * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (bt->status) CUDA_TRY(ctx, cudaMemcpyAsync(bt->status, ctx->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   if (bt->lm_iters) CUDA_TRY(ctx, cudaMemcpyAsync(bt->lm_iters, ctx->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+static int32_t check_plan(tebgpu_ctx* ctx, const TebPlanInput* pi) {
+  if (!pi || !pi->cmd) { ctx->err = "plan input or cmd == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (pi->initial_plan ? pi->P_cap < 1 : (!pi->start || !pi->goal)) {
+    ctx->err = "plan input needs start and goal, or initial_plan with P_cap >= 1";
+    return TEBGPU_ERR_INVALID_ARG;
+  }
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_plan_batch_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebPlanInput* plan, const TebOptimizeArgs* args,
+                                 void* cuda_stream) {
+  int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  rc = check_plan(ctx, plan);
+  if (rc) return rc;
+  rc = check_path(ctx, bt, true);
+  if (rc) return rc;
+  if (!args || args->iterations_innerloop < 0 || args->iterations_outerloop < 0) { ctx->err = "bad optimize args"; return TEBGPU_ERR_INVALID_ARG; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  return run_sequence(ctx, bt, args, st, plan);
+}
+
+int32_t tebgpu_plan_batch(tebgpu_ctx* ctx, TebBatch* bt, const TebPlanInput* plan, const TebOptimizeArgs* args) {
+  int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  rc = check_plan(ctx, plan);
+  if (rc) return rc;
+  const size_t B = bt->B, nc = bt->n_cap;
+  /* the rows the device entry point would report as TEB_STATUS_BAD_INPUT are refused here, before anything runs */
+  for (size_t b = 0; b < B; ++b) {
+    if (plan->initial_plan) {
+      const int P = plan->plan_count ? plan->plan_count[b] : plan->P_cap;
+      if (P < 1 || P > plan->P_cap) { ctx->err = "plan_count[b] outside 1 .. P_cap"; return TEBGPU_ERR_INVALID_ARG; }
+      for (int k = 0; k < 3 * P; ++k)
+        if (!std::isfinite(plan->initial_plan[b * plan->P_cap * 3 + k])) { ctx->err = "non-finite plan row"; return TEBGPU_ERR_INVALID_ARG; }
+    } else {
+      for (int k = 0; k < 3; ++k)
+        if (!std::isfinite(plan->start[3 * b + k]) || !std::isfinite(plan->goal[3 * b + k])) {
+          ctx->err = "non-finite start or goal";
+          return TEBGPU_ERR_INVALID_ARG;
+        }
+    }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  rc = upload_batch(ctx, bt);
+  if (rc) return rc;
+  cudaStream_t st = ctx->stream;
+  TebPlanInput dp = *plan;
+  dp.cmd = ctx->d_cmd;
+  dp.path = plan->path ? ctx->d_path : nullptr;
+  if (plan->initial_plan) {
+    if ((size_t)plan->P_cap > ctx->plan_rows) { /* the first call with a longer plan grows the mirror */
+      CUDA_TRY(ctx, cudaStreamSynchronize(st));
+      if (ctx->d_plan) CUDA_TRY(ctx, cudaFree(ctx->d_plan));
+      ctx->d_plan = nullptr;
+      ctx->plan_rows = 0;
+      CUDA_TRY(ctx, cudaMalloc(&ctx->d_plan, (size_t)ctx->lim.max_bands * plan->P_cap * 3 * sizeof(double)));
+      ctx->plan_rows = plan->P_cap;
+    }
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_plan, plan->initial_plan, B * plan->P_cap * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    dp.initial_plan = ctx->d_plan;
+    dp.start = dp.goal = nullptr;
+    if (plan->plan_count) {
+      CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_pcount, plan->plan_count, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+      dp.plan_count = ctx->d_pcount;
+    }
+  } else {
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_start, plan->start, B * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_goal, plan->goal, B * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    dp.start = ctx->d_start; dp.goal = ctx->d_goal;
+    dp.plan_count = nullptr;
+  }
+  TebBatch d = mirror_batch(ctx, bt);
+  rc = tebgpu_plan_batch_device(ctx, &d, &dp, args, nullptr);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(bt->poses, ctx->d_poses, B * nc * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(bt->n, ctx->d_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (bt->cost) CUDA_TRY(ctx, cudaMemcpyAsync(bt->cost, ctx->d_cost, B * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (bt->chi2) CUDA_TRY(ctx, cudaMemcpyAsync(bt->chi2, ctx->d_chi2, B * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (bt->status) CUDA_TRY(ctx, cudaMemcpyAsync(bt->status, ctx->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (bt->lm_iters) CUDA_TRY(ctx, cudaMemcpyAsync(bt->lm_iters, ctx->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(plan->cmd, ctx->d_cmd, B * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (plan->path) CUDA_TRY(ctx, cudaMemcpyAsync(plan->path, ctx->d_path, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
 }

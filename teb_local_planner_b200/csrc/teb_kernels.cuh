@@ -95,6 +95,9 @@ struct DevBatch {
    * association word w of the pose is non-zero, so that per-iteration kernels read only the words that hold bits */
   unsigned long long* occ;    /* [B][n_cap][OW] */
   int32_t OW;                 /* ceil(MW / 64) */
+  /* [B] or NULL: status bits k_plan_begin left for a band it could not plan (teb_plan.cuh); k_begin marks such a band
+   * failed, so the optimize sequence leaves it as it is */
+  const int32_t* pre_status;
 };
 
 /* Global-table path: the obstacles associated with pose row pr = b * n_cap + i, in increasing index order (the order
@@ -205,6 +208,7 @@ __global__ void k_begin(DevBatch db, KParams kp) {
     }
     if (bad) { st.failed = 1; st.status |= TEB_STATUS_BAD_INPUT; }
   }
+  if (db.pre_status && db.pre_status[b]) { st.failed = 1; st.status |= db.pre_status[b]; }
   db.state[b] = st;
 }
 

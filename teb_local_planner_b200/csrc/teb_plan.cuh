@@ -1,0 +1,116 @@
+/*
+ * teb_plan.cuh — the launches that turn one optimizeTEB over a batch into TebOptimalPlanner::plan followed by
+ * getVelocityCommand for every band (tebgpu_plan_batch / tebgpu_plan_batch_device):
+ *
+ *   k_plan_begin        warp per band, before k_begin: input check, cold start / warm start / re-initialisation
+ *                       decision, initTrajectoryToGoal or updateAndPruneTEB            (optimal_planner.cpp:247-321)
+ *   k_velocity_command  thread per band, after k_finalize: getVelocityCommand       (optimal_planner.cpp:1135-1168)
+ *
+ * The band routines are in teb_plan.h. k_plan_begin leaves a band it could not plan untouched and hands the reason
+ * (TEB_STATUS_BAD_INPUT, TEB_STATUS_CAPACITY) to k_begin through DevBatch::pre_status, so the optimize sequence skips
+ * it and k_finalize reports it, as it does for a band autoResize could not grow.
+ */
+#pragma once
+
+#include "teb_kernels.cuh"
+#include "teb_plan.h"
+
+namespace tebgpu {
+
+constexpr int PLAN_PRUNE_MAX = 10; /* updateAndPruneTEB drops at most 10 poses (timed_elastic_band.cpp:563) */
+
+__global__ void __launch_bounds__(128) k_plan_begin(DevBatch db, const __grid_constant__ TebParams p, TebPlanInput pi,
+                                                    int32_t* pre_status) {
+  const int b = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (b >= db.B) return; /* whole warps leave together: B is the same for every lane of a warp */
+  double* rec = db.poses + (size_t)b * db.n_cap * 4;
+  const int n = db.n[b];
+  const double* plan = pi.initial_plan ? pi.initial_plan + (size_t)b * pi.P_cap * 3 : nullptr;
+  const int P = plan ? (pi.plan_count ? pi.plan_count[b] : pi.P_cap) : 0;
+  /* inputs the host entry point rejects with TEBGPU_ERR_INVALID_ARG: a band length outside 0 .. n_cap, a plan length
+   * outside 1 .. P_cap, a non-finite start, goal or plan row */
+  bool bad = n < 0 || n > db.n_cap || (plan && (P < 1 || P > pi.P_cap));
+  if (!bad) {
+    if (plan) {
+      for (int r = lane; r < P; r += 32)
+        bad |= !(isfinite(plan[3 * r]) && isfinite(plan[3 * r + 1]) && isfinite(plan[3 * r + 2]));
+    } else if (lane < 6) {
+      const double v = lane < 3 ? pi.start[3 * b + lane] : pi.goal[3 * b + lane - 3];
+      bad = !isfinite(v);
+    }
+  }
+  bad = __any_sync(0xffffffffu, bad);
+  if (bad) {
+    if (lane == 0) {
+      pre_status[b] = TEB_STATUS_BAD_INPUT;
+      if (pi.path) pi.path[b] = TEB_PLAN_PATH_NONE;
+    }
+    return;
+  }
+  /* start and goal: the given poses, or the plan's first and last point (optimal_planner.cpp:257-258) */
+  double s[3], g[3];
+  if (plan) {
+    const double* lp = plan + 3 * (P - 1);
+    s[0] = plan[0]; s[1] = plan[1]; s[2] = teb_plan_yaw(plan[2]);
+    g[0] = lp[0]; g[1] = lp[1]; g[2] = teb_plan_yaw(lp[2]);
+  } else {
+    for (int c = 0; c < 3; ++c) { s[c] = pi.start[3 * b + c]; g[c] = pi.goal[3 * b + c]; }
+  }
+  const int path = teb_plan_path(rec, n, g, p.force_reinit_new_goal_dist, p.force_reinit_new_goal_angular);
+  int status = 0, code = path;
+  if (path == TEB_PLAN_PATH_WARM) {
+    /* updateAndPruneTEB(start, goal, min_samples): poses 1 .. k go while each is strictly nearer to the new start than
+     * the one before it, k <= lookahead = min(n - min_samples, 10). Lane j holds the distance of pose j. */
+    const int lookahead = min(min(n - p.min_samples, PLAN_PRUNE_MAX), n - 1); /* n - 1: min_samples < 1 */
+    const double d = lane < n && lane <= PLAN_PRUNE_MAX ? teb_plan_dist(s[0], s[1], rec[4 * lane], rec[4 * lane + 1]) : 0.0;
+    const double d_prev = __shfl_up_sync(0xffffffffu, d, 1);
+    const unsigned stop = __ballot_sync(0xffffffffu, lane >= 1 && lane <= lookahead && !(d < d_prev));
+    const int k = lookahead <= 0 ? 0 : (stop ? __ffs(stop) - 2 : lookahead);
+    const int m = n - k;
+    if (k > 0) { /* deletePoses(1, k), deleteTimeDiffs(1, k): record j >= 1 takes record j + k, record 0 keeps dt_0 */
+      for (int base = 1; base < m; base += 32) {
+        const int j = base + lane;
+        double v[4];
+        if (j < m)
+          for (int c = 0; c < 4; ++c) v[c] = rec[4 * (j + k) + c];
+        __syncwarp(); /* every lane holds its source record before any lane overwrites one */
+        if (j < m)
+          for (int c = 0; c < 4; ++c) rec[4 * j + c] = v[c];
+        __syncwarp();
+      }
+    }
+    if (lane == 0) {
+      rec[0] = s[0]; rec[1] = s[1]; rec[2] = s[2];
+      double* back = rec + 4 * (m - 1);
+      back[0] = g[0]; back[1] = g[1]; back[2] = g[2];
+      db.n[b] = m;
+    }
+  } else if (lane == 0) { /* cold start, or clearTimedElasticBand + initTrajectoryToGoal: sequential, one lane */
+    const int m = plan ? teb_init_from_plan_records(rec, db.n_cap, plan, P, p.max_vel_x, p.max_vel_theta,
+                                                    p.global_plan_overwrite_orientation, p.min_samples,
+                                                    p.allow_init_with_backwards_motion)
+                       : teb_init_to_goal_records(rec, db.n_cap, s, g, p.max_vel_x, p.min_samples);
+    if (m < 0) { status = TEB_STATUS_CAPACITY; code = TEB_PLAN_PATH_NONE; }
+    else db.n[b] = m;
+  }
+  if (lane == 0) {
+    pre_status[b] = status;
+    if (pi.path) pi.path[b] = code;
+  }
+}
+
+__global__ void k_velocity_command(DevBatch db, const __grid_constant__ TebParams p, TebPlanInput pi) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= db.B) return;
+  const int n = db.n[b];
+  double v[3] = {0, 0, 0};
+  const int ok = n >= 0 && n <= db.n_cap
+                     ? teb_velocity_command(db.poses + (size_t)b * db.n_cap * 4, n, pi.look_ahead_poses,
+                                            pi.prevent_look_ahead_poses_near_goal, p.dt_ref, p.max_vel_y, v)
+                     : 0;
+  double* c = pi.cmd + 4 * (size_t)b;
+  c[0] = v[0]; c[1] = v[1]; c[2] = v[2]; c[3] = ok;
+}
+
+}  // namespace tebgpu
