@@ -169,7 +169,7 @@ static inline double obst_dist_t(const TebObstacle* o, double px, double py, dou
  * distance_polygon_to_polygon_2d (:172-262). Besides the distance the functions return the pair of closest points,
  * from which the closed-form gradient follows: d d / d(x, y) = n, d d / d theta = n . J (c_robot - p), n the unit
  * vector from the obstacle's to the robot's closest point (0 when the shapes intersect). */
-#define ORACLE_MAX_SHAPE 64
+#define ORACLE_SMALL_SHAPE 64   /* obstacle vertex lists up to this length are copied to the stack, longer ones to the heap */
 
 /* closest_point_on_line_segment_2d distance_calculations.h:60-75 */
 static void closest_on_segment(const double* pt, const double* a, const double* b, double* out) {
@@ -244,12 +244,12 @@ static int generic_pair(const TebParams* c, const TebObstacle* o) {
 /* calculateDistance / estimateSpatioTemporalDistance for every footprint x obstacle combination; grad may be NULL */
 static double generic_distance(const TebParams* c, const double* pose, const TebObstacle* o, const double* pool, double t,
                                double* grad) {
-  double ov[2 * ORACLE_MAX_SHAPE];
+  double ov_small[2 * ORACLE_SMALL_SHAPE], *ov = ov_small;
   int ok;
   double offx = t * o->vx, offy = t * o->vy;
   if (o->type >= TEB_OBST_LINE && o->vertex_count >= 1 && pool) {
     ok = o->vertex_count;
-    if (ok > ORACLE_MAX_SHAPE) ok = ORACLE_MAX_SHAPE;
+    if (ok > ORACLE_SMALL_SHAPE) ov = (double*)malloc(sizeof(double) * 2 * (size_t)ok);
     for (int k = 0; k < ok; ++k) {
       ov[2 * k] = pool[2 * (o->vertex_begin + k)] + offx;
       ov[2 * k + 1] = pool[2 * (o->vertex_begin + k) + 1] + offy;
@@ -292,8 +292,10 @@ static double generic_distance(const TebParams* c, const double* pose, const Teb
     }
     double cr[2], co[2];
     double d = shape_distance(rv, rk, ov, ok, obst_first, cr, co) - orad - rrad;
-    if (d < best) { best = d; bcr[0] = cr[0]; bcr[1] = cr[1]; bco[0] = co[0]; bco[1] = co[1]; }
+    /* <=: the rear circle (sub 1) wins an exact front / rear tie, as in footprint_grad (same distance, one gradient) */
+    if (d <= best) { best = d; bcr[0] = cr[0]; bcr[1] = cr[1]; bco[0] = co[0]; bco[1] = co[1]; }
   }
+  if (ov != ov_small) free(ov);
   if (grad) {
     double nx = bcr[0] - bco[0], ny = bcr[1] - bco[1];
     double nn = sqrt(nx * nx + ny * ny);

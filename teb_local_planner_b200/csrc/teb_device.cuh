@@ -333,7 +333,8 @@ __device__ __noinline__ Dist4 generic_distance(int fp_type, const double* __rest
       }
     }
     const double dsub = sbest - orad - rrad;
-    if (dsub < best) { best = dsub; bcrx = scrx; bcry = scry; bcox = scox; bcoy = scoy; }
+    /* <=: the rear circle (sub 1) wins an exact front / rear tie, as in footprint_distance (same distance, one gradient) */
+    if (dsub <= best) { best = dsub; bcrx = scrx; bcry = scry; bcox = scox; bcoy = scoy; }
   }
   Dist4 r;
   r.d = best;
