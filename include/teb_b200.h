@@ -244,8 +244,32 @@ typedef struct TebPlanInput {
 #define TEB_PLAN_PATH_WARM   1   /* goal moved < force_reinit_new_goal_dist and turned < _angular: updateAndPruneTEB */
 #define TEB_PLAN_PATH_REINIT 2   /* otherwise: clearTimedElasticBand + initTrajectoryToGoal */
 
+/* Arguments and outputs of TebOptimalPlanner::isTrajectoryFeasible (optimal_planner.cpp:1250-1310) for every band of a
+ * batch (tebgpu_check_feasible). HOST output pointers for tebgpu_check_feasible, DEVICE pointers for
+ * tebgpu_check_feasible_device.
+ *
+ * World model, the one difference from the reference. The reference asks base_local_planner::CostmapModel::footprintCost
+ * of the costmap; here footprintCost(x, y, theta) == -1 means: the context's footprint model (TebParams.footprint_type and
+ * its geometry) placed at (x, y, theta) has a distance <= collision_distance to some obstacle of the band's scene. The
+ * distance is the optimizer's own footprint-to-obstacle distance (the one the obstacle edges use); all obst_count rows of
+ * the scene are tested, not the association; dynamic obstacles at their current position (a snapshot, no time
+ * prediction). With collision_distance = 0, contact, overlap and containment (distance exactly 0) are collisions. It does
+ * not rasterise the footprint outline over costmap cells and has no inscribed-cost band. A query whose distances are all
+ * > collision_distance except for some NaN ones is undecidable. */
+typedef struct TebFeasibilityArgs {
+  int32_t  look_ahead_idx;      /* feasibility_check_no_poses; < 0 or >= n: the whole band */
+  int32_t  max_queries;         /* footprint queries tested (and stored) per band, >= 1 */
+  double   lookahead_distance;  /* feasibility_check_lookahead_distance; <= 0: off */
+  double   inscribed_radius;    /* the interpolation step between poses, > 0 and finite */
+  double   angular_resolution;  /* trajectory.min_resolution_collision_check_angular, > 0 and finite */
+  double   collision_distance;  /* >= 0 and finite */
+  int32_t* feasible;            /* [B] out: 1 feasible, 0 a query collides, -1 undecidable (see tebgpu_check_feasible) */
+  int32_t* query_count;         /* [B] out: footprint queries the reference makes */
+  double*  queries;             /* [B][max_queries][3] out or NULL: the first min(query_count, max_queries) query poses */
+} TebFeasibilityArgs;
+
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
- * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput. */
+ * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -292,6 +316,35 @@ int32_t tebgpu_synchronize(tebgpu_ctx* ctx);
 int32_t tebgpu_plan_batch(tebgpu_ctx* ctx, TebBatch* batch, const TebPlanInput* plan, const TebOptimizeArgs* args);
 int32_t tebgpu_plan_batch_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebPlanInput* plan,
                                  const TebOptimizeArgs* args, void* cuda_stream);
+
+/* isTrajectoryFeasible (optimal_planner.cpp:1250-1310) for every band of the batch, against the world model described at
+ * TebFeasibilityArgs. Per band:
+ *   1. look_ahead_idx is clamped to n - 1, then, with lookahead_distance > 0, set to i - 1 for the first pose i whose
+ *      std::hypot distance from pose 0 is > lookahead_distance.
+ *   2. The queries, in order: pose i, then for i < look_ahead_idx the reference's intermediate poses towards pose i + 1
+ *      (sequential accumulation, strict > tests against angular_resolution and inscribed_radius). Sample counts beyond
+ *      the int range, where the reference is undefined, saturate at INT_MAX - 1 per segment.
+ *   3. feasible is decided by the first query that is not free: 0 if it collides, -1 if it is undecidable. If every
+ *      query is free: 1, unless the band has more than max_queries queries (then only the first max_queries are
+ *      tested) and none of those is non-free: -1. A non-finite x / y / theta among the checked poses gives -1 with no
+ *      query; so does, in the device entry point, a band whose n or scene_id is out of range or whose scene holds an
+ *      obstacle row the batch cannot describe.
+ *   4. query_count: the queries the reference makes, up to and including the first non-free one. When the band has more
+ *      than max_queries queries and the first max_queries are free, it is the band's total number of queries (what the
+ *      reference makes when all are free), so that a retry can be sized; it saturates at INT32_MAX. n == 0 gives
+ *      feasible 1 and no query.
+ *   5. queries (if not NULL): the first min(query_count, max_queries) query poses; the rows behind them are not written.
+ * Reads only poses, n, scene_id, obstacles, obst_count and obst_vertices of the batch and writes only the outputs in
+ * `args`; nothing the optimize or plan entry points read changes. Argument errors (NULL batch arrays or outputs, a bad
+ * inscribed_radius / angular_resolution / collision_distance / max_queries) return TEBGPU_ERR_INVALID_ARG before anything
+ * is launched. tebgpu_check_feasible: HOST buffers, synchronous; n, scene_id, obst_count or obstacle rows out of range
+ * are refused with TEBGPU_ERR_INVALID_ARG too; the device copies of the outputs are allocated by the first call that
+ * needs them. tebgpu_check_feasible_device: DEVICE buffers, stream ordered as tebgpu_optimize_batch_device, does not
+ * synchronise. M_cap <= 1024 stages the scene's table in shared memory, above that the rows are read from global
+ * memory (tebgpu_get_info keys 12 / 13). */
+int32_t tebgpu_check_feasible(tebgpu_ctx* ctx, const TebBatch* batch, const TebFeasibilityArgs* args);
+int32_t tebgpu_check_feasible_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebFeasibilityArgs* args,
+                                     void* cuda_stream);
 
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded
@@ -362,8 +415,9 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * (key 0 reports the width of the later iterations), 8 grid in CTAs of the last trial-evaluation launch the context
  * issued (0 before the first; a replayed CUDA graph issues none), 9 which build that launch ran (TEBGPU_EVAL_BUILD_*,
  * -1 before the first), 10 grid in CTAs of the last kernel-A launch the context issued (0 before the first; a replayed
- * CUDA graph issues none), 11 which build that launch ran (TEBGPU_KA_BUILD_*, -1 before the first). Returns -1 for an
- * unknown key. */
+ * CUDA graph issues none), 11 which build that launch ran (TEBGPU_KA_BUILD_*, -1 before the first), 12 grid in CTAs of
+ * the last feasibility-check launch (0 before the first), 13 which build that launch ran (TEBGPU_FEAS_BUILD_*, -1 before
+ * the first). Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2 2       /* k_trial_eval2 (B <= 2 x SMs): B CTAs */
@@ -373,6 +427,8 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
 #define TEBGPU_KA_BUILD_ONESHOT 1  /* k_linearize2, staged output (TEBGPU_KA_PERSIST=0): ceil(chunks / 4) x B CTAs */
 #define TEBGPU_KA_BUILD_DIRECT 2   /* k_linearize2, direct stores (TEBGPU_KA_STAGED=0): ceil(chunks / 4) x B CTAs */
 #define TEBGPU_KA_BUILD_PERSIST 3  /* k_linearize2p (default): resident one-warp CTAs per SM x SMs, at most chunks x B */
+#define TEBGPU_FEAS_BUILD_STAGED 0  /* k_feasible, the scene's table staged in shared memory (M_cap <= 1024): B CTAs */
+#define TEBGPU_FEAS_BUILD_GLOBAL 1  /* k_feasible, the table read from global memory / L2 (M_cap > 1024): B CTAs */
 int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which);
 
 /* Linearise only: build the padded banded normal equations of every band at its current state for

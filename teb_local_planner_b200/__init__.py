@@ -5,6 +5,7 @@ Python side: ctypes loader for the in-tree CUDA library (C-ABI in include/teb_b2
 library is missing or no GPU is present, loading / creating a context raises.
 """
 import ctypes as C
+import math
 import os
 
 from . import abi
@@ -49,6 +50,10 @@ def load_library(build_if_missing=False):
     L.tebgpu_plan_batch_device.restype = C.c_int32
     L.tebgpu_plan_batch_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebPlanInput),
                                            C.POINTER(abi.TebOptimizeArgs), vp]
+    L.tebgpu_check_feasible.restype = C.c_int32
+    L.tebgpu_check_feasible.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs)]
+    L.tebgpu_check_feasible_device.restype = C.c_int32
+    L.tebgpu_check_feasible_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs), vp]
     L.tebgpu_get_plan_kernel_times.restype = C.c_int32
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
@@ -106,7 +111,7 @@ def load_library(build_if_missing=False):
     L.tebgpu_auto_resize_host.restype = C.c_int32
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
     for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
-                                abi.TebPlanInput)):
+                                abi.TebPlanInput, abi.TebFeasibilityArgs)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -198,6 +203,36 @@ class TebGpu:
         pi.cmd, pi.path = addr(cmd), addr(path)
         self._check(self.lib.tebgpu_plan_batch_device(self.ctx, C.byref(batch_struct), C.byref(pi), C.byref(args), stream),
                     "tebgpu_plan_batch_device")
+
+    def check_feasible(self, hb, inscribed_radius, look_ahead_idx=-1, lookahead_distance=-1.0, angular_resolution=math.pi,
+                       collision_distance=0.0, max_queries=1024, queries=False):
+        """TebOptimalPlanner::isTrajectoryFeasible for every band of hb (an abi.HostBatch) against its scene's obstacles
+        (tebgpu_check_feasible), host buffers. Returns (feasible [B] int32: 1 feasible, 0 colliding, -1 undecidable,
+        query_count [B] int32), and with queries=True also the query poses [B][max_queries][3] (NaN past each band's
+        min(query_count, max_queries) rows)."""
+        import numpy as np
+        feas = np.zeros(hb.B, np.int32)
+        cnt = np.zeros(hb.B, np.int32)
+        q = np.full((hb.B, int(max_queries), 3), np.nan) if queries else None
+        fa = abi.make_feasibility_args(inscribed_radius, look_ahead_idx, lookahead_distance, angular_resolution,
+                                       collision_distance, max_queries, abi.ptr(feas), abi.ptr(cnt), abi.ptr(q))
+        bs = hb.struct()
+        self._check(self.lib.tebgpu_check_feasible(self.ctx, C.byref(bs), C.byref(fa)), "tebgpu_check_feasible")
+        return (feas, cnt, q) if queries else (feas, cnt)
+
+    def check_feasible_device(self, batch_struct, fargs, stream=None):
+        """tebgpu_check_feasible_device: the same check over DEVICE memory (batch_struct: an abi.TebBatch of device
+        pointers; fargs: an abi.TebFeasibilityArgs whose outputs are device addresses, see abi.make_feasibility_args).
+        Stream ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_check_feasible_device(self.ctx, C.byref(batch_struct), C.byref(fargs), stream),
+                    "tebgpu_check_feasible_device")
+
+    FEAS_BUILDS = {0: "staged", 1: "global"}   # TEBGPU_FEAS_BUILD_*
+
+    def last_feasibility_check(self):
+        """(build, grid in CTAs) of the last feasibility-check launch: build is one of FEAS_BUILDS' names, or None
+        before the first launch"""
+        return self.FEAS_BUILDS.get(self.info(13)), self.info(12)
 
     def plan_kernel_times(self):
         """{kernel name: (total ms, launches)} of k_plan_begin and k_velocity_command since profiling was enabled"""

@@ -114,6 +114,30 @@ class TebPlanInput(C.Structure):
 TEB_PLAN_PATH_NONE, TEB_PLAN_PATH_COLD, TEB_PLAN_PATH_WARM, TEB_PLAN_PATH_REINIT = -1, 0, 1, 2
 
 
+class TebFeasibilityArgs(C.Structure):
+    """TebOptimalPlanner::isTrajectoryFeasible per band (tebgpu_check_feasible): arguments, and host or device output
+    pointers"""
+    _fields_ = [("look_ahead_idx", _i), ("max_queries", _i), ("lookahead_distance", _d), ("inscribed_radius", _d),
+                ("angular_resolution", _d), ("collision_distance", _d),
+                ("feasible", C.c_void_p), ("query_count", C.c_void_p), ("queries", C.c_void_p)]
+
+
+TEBGPU_FEAS_BUILD_STAGED, TEBGPU_FEAS_BUILD_GLOBAL = 0, 1
+
+
+def make_feasibility_args(inscribed_radius, look_ahead_idx=-1, lookahead_distance=-1.0, angular_resolution=np.pi,
+                          collision_distance=0.0, max_queries=1024, feasible=None, query_count=None,
+                          queries=None) -> TebFeasibilityArgs:
+    """TebFeasibilityArgs with the outputs given as addresses (ints, or None for NULL). The defaults are the
+    reference's: the whole band, no look-ahead distance, min_resolution_collision_check_angular = pi."""
+    f = TebFeasibilityArgs()
+    f.look_ahead_idx, f.max_queries = int(look_ahead_idx), int(max_queries)
+    f.lookahead_distance, f.inscribed_radius = float(lookahead_distance), float(inscribed_radius)
+    f.angular_resolution, f.collision_distance = float(angular_resolution), float(collision_distance)
+    f.feasible, f.query_count, f.queries = feasible, query_count, queries
+    return f
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

@@ -4,6 +4,7 @@
  */
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -18,6 +19,7 @@
 #include "teb_solve_lat.cuh"
 #include "teb_hsig.cuh"
 #include "teb_plan.cuh"
+#include "teb_feasible.cuh"
 #include "teb_comm.h"
 #include <cstdlib>
 
@@ -104,6 +106,13 @@ struct tebgpu_ctx {
   int32_t* d_path = nullptr;
   double* d_plan = nullptr;           /* [max_bands][plan_rows][3], grown to the largest P_cap tebgpu_plan_batch has seen */
   size_t plan_rows = 0;
+  /* feasibility check: the host-buffer entry point's output mirrors, allocated by the first call that needs them */
+  int32_t* d_feas = nullptr; int32_t* d_qcount = nullptr;
+  double* d_queries = nullptr;        /* [max_bands][feas_rows][3] */
+  size_t feas_rows = 0;
+  bool feas_ready = false;            /* k_feasible's shared-memory attributes set */
+  int last_feas_build = -1;           /* the last k_feasible launch: its build (TEBGPU_FEAS_BUILD_*) */
+  long long last_feas_grid = 0;       /* ... and its grid in CTAs */
   size_t smem_a = 0, smem_b = 0, smem_g = 0;
   /* profiling */
   bool profiling = false;
@@ -193,6 +202,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 3: return (int32_t)sizeof(TebOptimizeArgs);
     case 4: return (int32_t)sizeof(TebGpuLimits);
     case 5: return (int32_t)sizeof(TebPlanInput);
+    case 6: return (int32_t)sizeof(TebFeasibilityArgs);
     default: return -1;
   }
 }
@@ -214,6 +224,8 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 9: return ctx->last_eval_build;
     case 10: return ctx->last_ka_grid;
     case 11: return ctx->last_ka_build;
+    case 12: return ctx->last_feas_grid;
+    case 13: return ctx->last_feas_build;
     default: return -1;
   }
 }
@@ -222,7 +234,7 @@ static void free_all(tebgpu_ctx* c) {
   void* ptrs[] = {c->Lf2, c->dx2, c->arrive, c->d_gather, c->d_hsig, c->assoc3, c->occ, c->dyn_idx, c->dyn_cnt, c->rhs, c->dmax_parts, c->spec.Lf, c->spec.dx, c->spec.res, c->spec.need, c->spec.qmax, c->spec.cnt, c->spec.list, c->defer, c->d_fp, c->d_pverts, c->Hb, c->assoc, c->dyn_t, c->via_idx, c->chi_parts, c->state, c->d_poses, c->d_n, c->d_scene,
                   c->d_obst, c->d_ocount, c->d_via, c->d_vcount, c->d_vs, c->d_vg, c->d_rot, c->d_cost, c->d_chi2,
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
-                  c->d_plan};
+                  c->d_plan, c->d_feas, c->d_qcount, c->d_queries};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1296,6 +1308,127 @@ int32_t tebgpu_plan_batch(tebgpu_ctx* ctx, TebBatch* bt, const TebPlanInput* pla
   CUDA_TRY(ctx, cudaMemcpyAsync(plan->cmd, ctx->d_cmd, B * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (plan->path) CUDA_TRY(ctx, cudaMemcpyAsync(plan->path, ctx->d_path, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* argument checks of both feasibility entry points: nothing is launched when one fails */
+static int32_t check_feasible_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!bt || !fa) { ctx->err = "batch or feasibility args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->B < 1 || bt->n_cap < 1 || bt->S < 1 || bt->M_cap < 0 || bt->PV_cap < 0) { ctx->err = "bad batch dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->B > ctx->lim.max_bands || bt->n_cap > ctx->lim.max_poses || bt->S > ctx->lim.max_scenes ||
+      bt->M_cap > ctx->lim.max_obstacles || bt->PV_cap > ctx->lim.max_obst_vertices) { ctx->err = "batch exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+  if (!bt->poses || !bt->n || !bt->scene_id || !bt->obst_count) { ctx->err = "missing required batch array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->M_cap > 0 && !bt->obstacles) { ctx->err = "obstacles == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->PV_cap > 0 && !bt->obst_vertices) { ctx->err = "obst_vertices == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!fa->feasible || !fa->query_count) { ctx->err = "feasible or query_count == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!(std::isfinite(fa->inscribed_radius) && fa->inscribed_radius > 0)) { ctx->err = "inscribed_radius must be > 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!(std::isfinite(fa->angular_resolution) && fa->angular_resolution > 0)) { ctx->err = "angular_resolution must be > 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!(std::isfinite(fa->collision_distance) && fa->collision_distance >= 0)) { ctx->err = "collision_distance must be >= 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fa->max_queries < 1) { ctx->err = "max_queries must be >= 1"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!ctx->have_params) { ctx->err = "tebgpu_set_params has not been called"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_feasible on arguments already checked; the path (staged / global table) follows M_cap like every default kernel */
+static int32_t issue_feasible(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa, cudaStream_t st) {
+  if (!ctx->feas_ready) { /* the staged builds take up to 64 KB of obstacle rows beyond the static shared memory */
+    const int smax = STAGED_MAX_OBST * (int)sizeof(TebObstacle);
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_feasible<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smax));
+    CUDA_TRY(ctx, cudaFuncSetAttribute(k_feasible<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smax));
+    ctx->feas_ready = true;
+  }
+  KParams kp = make_kparams(ctx, bt, 1.0);
+  FeasDev fd;
+  std::memset(&fd, 0, sizeof(fd));
+  fd.B = bt->B; fd.n_cap = bt->n_cap; fd.S = bt->S; fd.M_cap = bt->M_cap; fd.PV_cap = bt->PV_cap;
+  fd.poses = bt->poses; fd.n = bt->n; fd.scene_id = bt->scene_id; fd.obstacles = bt->obstacles; fd.obst_count = bt->obst_count;
+  fd.obst_vertices = bt->PV_cap > 0 ? bt->obst_vertices : nullptr;
+  fd.a = *fa;
+  const bool gt = global_table(bt->M_cap);
+  const size_t smem = gt ? 0 : (size_t)bt->M_cap * sizeof(TebObstacle);
+  const int B = bt->B;
+  if (gt && kp.generic) k_feasible<true, true><<<B, FEAS_THREADS, 0, st>>>(fd, kp);
+  else if (gt) k_feasible<false, true><<<B, FEAS_THREADS, 0, st>>>(fd, kp);
+  else if (kp.generic) k_feasible<true, false><<<B, FEAS_THREADS, smem, st>>>(fd, kp);
+  else k_feasible<false, false><<<B, FEAS_THREADS, smem, st>>>(fd, kp);
+  ctx->last_feas_build = gt ? TEBGPU_FEAS_BUILD_GLOBAL : TEBGPU_FEAS_BUILD_STAGED;
+  ctx->last_feas_grid = B;
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_check_feasible_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa, void* cuda_stream) {
+  const int32_t rc = check_feasible_args(ctx, bt, fa);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_feasible(ctx, bt, fa, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_check_feasible(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa) {
+  int32_t rc = check_feasible_args(ctx, bt, fa);
+  if (rc) return rc;
+  /* the rows the device entry point would answer with -1 are refused here, before anything runs */
+  for (int sc = 0; sc < bt->S; ++sc)
+    if (bt->obst_count[sc] < 0 || bt->obst_count[sc] > bt->M_cap) { ctx->err = "obst_count[s] outside 0 .. M_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  for (int b = 0; b < bt->B; ++b) {
+    if (bt->scene_id[b] < 0 || bt->scene_id[b] >= bt->S) { ctx->err = "scene_id[b] outside 0 .. S-1"; return TEBGPU_ERR_INVALID_ARG; }
+    if (bt->n[b] < 0 || bt->n[b] > bt->n_cap) { ctx->err = "n[b] outside 0 .. n_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  for (int sc = 0; sc < bt->S; ++sc)
+    for (int m = 0; m < bt->obst_count[sc]; ++m) {
+      const TebObstacle& o = bt->obstacles[(size_t)sc * bt->M_cap + m];
+      if (o.type < TEB_OBST_POINT || o.type > TEB_OBST_POLYGON) { ctx->err = "unknown obstacle type"; return TEBGPU_ERR_INVALID_ARG; }
+      if (o.type >= TEB_OBST_LINE && (o.vertex_count < 1 || (o.type != TEB_OBST_POLYGON && o.vertex_count != 2) ||
+                                      o.vertex_begin < 0 || (long long)o.vertex_begin + o.vertex_count > bt->PV_cap)) {
+        ctx->err = "obstacle vertex range outside obst_vertices";
+        return TEBGPU_ERR_INVALID_ARG;
+      }
+    }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t B = bt->B, nc = bt->n_cap, mq = fa->max_queries;
+  if (!ctx->d_feas) {
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_feas, ctx->lim.max_bands * sizeof(int32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_qcount, ctx->lim.max_bands * sizeof(int32_t)));
+  }
+  if (fa->queries && mq > ctx->feas_rows) { /* the first call with more query rows grows the mirror */
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    if (ctx->d_queries) CUDA_TRY(ctx, cudaFree(ctx->d_queries));
+    ctx->d_queries = nullptr;
+    ctx->feas_rows = 0;
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_queries, (size_t)ctx->lim.max_bands * mq * 3 * sizeof(double)));
+    ctx->feas_rows = mq;
+  }
+  /* the poses / obstacle mirrors of the host-buffer entry points: every host optimize / plan call uploads them anew */
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_poses, bt->poses, B * nc * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_n, bt->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scene, bt->scene_id, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (bt->M_cap > 0)
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_obst, bt->obstacles, (size_t)bt->S * bt->M_cap * sizeof(TebObstacle), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ocount, bt->obst_count, (size_t)bt->S * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (bt->PV_cap > 0)
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_pverts, bt->obst_vertices, (size_t)bt->S * bt->PV_cap * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  TebBatch d = *bt;
+  d.poses = ctx->d_poses; d.n = ctx->d_n; d.scene_id = ctx->d_scene; d.obstacles = ctx->d_obst; d.obst_count = ctx->d_ocount;
+  d.obst_vertices = bt->PV_cap > 0 ? ctx->d_pverts : nullptr;
+  TebFeasibilityArgs da = *fa;
+  da.feasible = ctx->d_feas; da.query_count = ctx->d_qcount;
+  da.queries = fa->queries ? ctx->d_queries : nullptr;
+  rc = issue_feasible(ctx, &d, &da, st);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(fa->feasible, ctx->d_feas, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(fa->query_count, ctx->d_qcount, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  if (fa->queries) { /* only the rows the kernel wrote reach the caller: min(query_count, max_queries) per band */
+    std::vector<double> q(B * mq * 3);
+    CUDA_TRY(ctx, cudaMemcpy(q.data(), ctx->d_queries, q.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (size_t b = 0; b < B; ++b) {
+      const size_t rows = std::min<size_t>((size_t)std::max(fa->query_count[b], 0), mq);
+      std::memcpy(fa->queries + b * mq * 3, q.data() + b * mq * 3, rows * 3 * sizeof(double));
+    }
+  }
   return TEBGPU_OK;
 }
 
