@@ -268,8 +268,37 @@ typedef struct TebFeasibilityArgs {
   double*  queries;             /* [B][max_queries][3] out or NULL: the first min(query_count, max_queries) query poses */
 } TebFeasibilityArgs;
 
+/* Which bands tebgpu_read_trajectory reads out, and its outputs: TebOptimalPlanner::getVelocityProfile
+ * (optimal_planner.cpp:1170-1188) and getFullTrajectory (:1190-1248) of every band read out. HOST pointers for
+ * tebgpu_read_trajectory, DEVICE pointers for tebgpu_read_trajectory_device. R is the number of rows read out: count
+ * when bands != NULL, B otherwise. Output row r holds band bands[r] (or r).
+ *
+ * Segment k (1 <= k <= n - 1) is extractVelocity(Pose(k - 1), Pose(k), TimeDiff(k - 1)) with the context's max_vel_y
+ * (0: non-holonomic, vx signed by the step's projection on pose k - 1's heading, sign(0) = 0, vy = 0); TimeDiff == 0
+ * gives a zero twist. Definitions:
+ *   Boundary rows: (vx, vy, omega) of vel_start[b] / vel_goal[b] as stored, whatever their active flag. The reference
+ *     reports vel_start_.second / vel_goal_.second and ignores .first (setVelocityGoalFree only clears .first,
+ *     optimal_planner.h:260).
+ *   Profile, n + 1 rows: the start velocity, segments 1 .. n - 1, the goal velocity. n = 0: one row, the goal velocity
+ *     (the reference resizes to 1, and back() overwrites front()).
+ *   Trajectory, n rows: pose i; velocity: the start velocity for i = 0, the goal velocity for i = n - 1 >= 1,
+ *     otherwise 0.5 * (segment i + segment i + 1); time_from_start: TimeDiff(0) + ... + TimeDiff(i - 1), summed in
+ *     that order from 0. n = 0: no row. n = 1: pose 0, the start velocity, t = 0 (the reference reads TimeDiff(0),
+ *     which does not exist there; its answer is undefined).
+ *   theta: the band's stored yaw. Formatting it as the message's quaternion is left to the caller. */
+typedef struct TebTrajectoryArgs {
+  const int32_t* bands;      /* [count] band indices, in output order (repeats and any order allowed), or NULL: all B bands */
+  int32_t        count;      /* rows read out when bands != NULL (>= 0); ignored when bands == NULL */
+  int32_t        _pad;
+  double*        profile;    /* [R][n_cap + 1][3] out or NULL: vx, vy, omega */
+  double*        trajectory; /* [R][n_cap][7] out or NULL: x, y, theta, vx, vy, omega, time_from_start */
+  int32_t*       points;     /* [R] out: n of the band read out; -1 for a row the device entry point could not read (a band
+                                index outside 0 .. B - 1 or n outside 0 .. n_cap). Rows past n + 1 (profile) and n
+                                (trajectory) are not written. */
+} TebTrajectoryArgs;
+
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
- * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs. */
+ * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -346,6 +375,20 @@ int32_t tebgpu_check_feasible(tebgpu_ctx* ctx, const TebBatch* batch, const TebF
 int32_t tebgpu_check_feasible_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebFeasibilityArgs* args,
                                      void* cuda_stream);
 
+/* getVelocityProfile and getFullTrajectory (optimal_planner.cpp:1170-1248) of the bands listed in `args`, as defined at
+ * TebTrajectoryArgs: what a controller publishes as its local plan every cycle. Reads only poses, n, vel_start and
+ * vel_goal of the batch and writes only the outputs in `args`. The holonomic / non-holonomic choice is the context's
+ * max_vel_y != 0 (tebgpu_set_params; the TebConfig default 0 until then), as in extractVelocity. Argument errors (NULL
+ * poses / n / vel_start / vel_goal or points, profile and trajectory both NULL, count < 0 with bands) return
+ * TEBGPU_ERR_INVALID_ARG before anything is launched; count == 0 launches nothing. tebgpu_read_trajectory: HOST buffers, synchronous; a band index outside
+ * 0 .. B - 1 or a band read out whose n is outside 0 .. n_cap is refused with TEBGPU_ERR_INVALID_ARG too; the device
+ * copies of the outputs are allocated by the first call that needs them. tebgpu_read_trajectory_device: DEVICE buffers,
+ * stream ordered as tebgpu_optimize_batch_device, does not synchronise; such a row gets points = -1 and nothing else,
+ * the other rows are read. One warp per row (tebgpu_get_info key 14). */
+int32_t tebgpu_read_trajectory(tebgpu_ctx* ctx, const TebBatch* batch, const TebTrajectoryArgs* args);
+int32_t tebgpu_read_trajectory_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebTrajectoryArgs* args,
+                                      void* cuda_stream);
+
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded
  *   LDL^T with the active window in registers, and the accept / reject chain is replayed in order;
@@ -417,7 +460,8 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * -1 before the first), 10 grid in CTAs of the last kernel-A launch the context issued (0 before the first; a replayed
  * CUDA graph issues none), 11 which build that launch ran (TEBGPU_KA_BUILD_*, -1 before the first), 12 grid in CTAs of
  * the last feasibility-check launch (0 before the first), 13 which build that launch ran (TEBGPU_FEAS_BUILD_*, -1 before
- * the first). Returns -1 for an unknown key. */
+ * the first), 14 grid in CTAs of the last trajectory read-out launch (k_read_trajectory, 4 rows per CTA; 0 before the
+ * first). Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2 2       /* k_trial_eval2 (B <= 2 x SMs): B CTAs */

@@ -54,6 +54,10 @@ def load_library(build_if_missing=False):
     L.tebgpu_check_feasible.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs)]
     L.tebgpu_check_feasible_device.restype = C.c_int32
     L.tebgpu_check_feasible_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs), vp]
+    L.tebgpu_read_trajectory.restype = C.c_int32
+    L.tebgpu_read_trajectory.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebTrajectoryArgs)]
+    L.tebgpu_read_trajectory_device.restype = C.c_int32
+    L.tebgpu_read_trajectory_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebTrajectoryArgs), vp]
     L.tebgpu_get_plan_kernel_times.restype = C.c_int32
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
@@ -111,7 +115,7 @@ def load_library(build_if_missing=False):
     L.tebgpu_auto_resize_host.restype = C.c_int32
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
     for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
-                                abi.TebPlanInput, abi.TebFeasibilityArgs)):
+                                abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -226,6 +230,40 @@ class TebGpu:
         Stream ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise."""
         self._check(self.lib.tebgpu_check_feasible_device(self.ctx, C.byref(batch_struct), C.byref(fargs), stream),
                     "tebgpu_check_feasible_device")
+
+    def read_trajectory(self, hb, bands=None, profile=True, trajectory=True):
+        """getVelocityProfile / getFullTrajectory of the bands of hb (an abi.HostBatch) listed in `bands` (None: all B, in
+        order) on the device (tebgpu_read_trajectory), host buffers, with the context's max_vel_y. Returns (profile
+        [R][n_cap + 1][3] vx, vy, omega, trajectory [R][n_cap][7] x, y, theta, vx, vy, omega, time_from_start, points
+        [R] int32: each row's n); rows past n + 1 / n are NaN. profile=False / trajectory=False: None in its place."""
+        import numpy as np
+        bl = None if bands is None else np.ascontiguousarray(bands, dtype=np.int32).reshape(-1)
+        R = hb.B if bl is None else len(bl)
+        prof = np.full((R, hb.n_cap + 1, 3), np.nan) if profile else None
+        traj = np.full((R, hb.n_cap, 7), np.nan) if trajectory else None
+        pts = np.zeros(R, np.int32)
+        ta = abi.TebTrajectoryArgs()
+        ta.bands, ta.count = abi.ptr(bl), R
+        ta.profile, ta.trajectory, ta.points = abi.ptr(prof), abi.ptr(traj), abi.ptr(pts)
+        bs = hb.struct()
+        self._check(self.lib.tebgpu_read_trajectory(self.ctx, C.byref(bs), C.byref(ta)), "tebgpu_read_trajectory")
+        return prof, traj, pts
+
+    def read_trajectory_device(self, batch_struct, trajectory=None, profile=None, points=None, bands=None, count=None,
+                               stream=None):
+        """tebgpu_read_trajectory_device: the same read-out over DEVICE memory (batch_struct: an abi.TebBatch of device
+        pointers). trajectory [R][n_cap][7] / profile [R][n_cap + 1][3] float64 (either may be None, not both), points
+        [R] int32, bands [count] int32 or None (all B bands): device pointers as ints, or torch tensors; count defaults
+        to the length of a `bands` tensor. Stream ordered on `stream` (a cudaStream_t handle; None: the context's
+        stream); does not synchronise."""
+        addr = lambda t: None if t is None else (t.data_ptr() if hasattr(t, "data_ptr") else int(t))
+        if count is None:
+            count = bands.numel() if hasattr(bands, "numel") else 0
+        ta = abi.TebTrajectoryArgs()
+        ta.bands, ta.count = addr(bands), int(count)
+        ta.profile, ta.trajectory, ta.points = addr(profile), addr(trajectory), addr(points)
+        self._check(self.lib.tebgpu_read_trajectory_device(self.ctx, C.byref(batch_struct), C.byref(ta), stream),
+                    "tebgpu_read_trajectory_device")
 
     FEAS_BUILDS = {0: "staged", 1: "global"}   # TEBGPU_FEAS_BUILD_*
 

@@ -138,6 +138,13 @@ def make_feasibility_args(inscribed_radius, look_ahead_idx=-1, lookahead_distanc
     return f
 
 
+class TebTrajectoryArgs(C.Structure):
+    """getVelocityProfile / getFullTrajectory read-out (tebgpu_read_trajectory): the bands to read (NULL: all B) and
+    host or device output pointers"""
+    _fields_ = [("bands", C.c_void_p), ("count", _i), ("_pad", _i), ("profile", C.c_void_p), ("trajectory", C.c_void_p),
+                ("points", C.c_void_p)]
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

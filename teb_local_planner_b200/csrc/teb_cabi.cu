@@ -113,6 +113,10 @@ struct tebgpu_ctx {
   bool feas_ready = false;            /* k_feasible's shared-memory attributes set */
   int last_feas_build = -1;           /* the last k_feasible launch: its build (TEBGPU_FEAS_BUILD_*) */
   long long last_feas_grid = 0;       /* ... and its grid in CTAs */
+  /* trajectory read-out: the host-buffer entry point's band list and output mirrors, grown by the first call that needs more */
+  int32_t* d_tbands = nullptr; int32_t* d_tpoints = nullptr; double* d_tprof = nullptr; double* d_ttraj = nullptr;
+  size_t tbands_bytes = 0, tpoints_bytes = 0, tprof_bytes = 0, ttraj_bytes = 0;
+  long long last_traj_grid = 0;       /* grid in CTAs of the last k_read_trajectory launch */
   size_t smem_a = 0, smem_b = 0, smem_g = 0;
   /* profiling */
   bool profiling = false;
@@ -203,6 +207,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 4: return (int32_t)sizeof(TebGpuLimits);
     case 5: return (int32_t)sizeof(TebPlanInput);
     case 6: return (int32_t)sizeof(TebFeasibilityArgs);
+    case 7: return (int32_t)sizeof(TebTrajectoryArgs);
     default: return -1;
   }
 }
@@ -226,6 +231,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 11: return ctx->last_ka_build;
     case 12: return ctx->last_feas_grid;
     case 13: return ctx->last_feas_build;
+    case 14: return ctx->last_traj_grid;
     default: return -1;
   }
 }
@@ -234,7 +240,7 @@ static void free_all(tebgpu_ctx* c) {
   void* ptrs[] = {c->Lf2, c->dx2, c->arrive, c->d_gather, c->d_hsig, c->assoc3, c->occ, c->dyn_idx, c->dyn_cnt, c->rhs, c->dmax_parts, c->spec.Lf, c->spec.dx, c->spec.res, c->spec.need, c->spec.qmax, c->spec.cnt, c->spec.list, c->defer, c->d_fp, c->d_pverts, c->Hb, c->assoc, c->dyn_t, c->via_idx, c->chi_parts, c->state, c->d_poses, c->d_n, c->d_scene,
                   c->d_obst, c->d_ocount, c->d_via, c->d_vcount, c->d_vs, c->d_vg, c->d_rot, c->d_cost, c->d_chi2,
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
-                  c->d_plan, c->d_feas, c->d_qcount, c->d_queries};
+                  c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1429,6 +1435,100 @@ int32_t tebgpu_check_feasible(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeas
       std::memcpy(fa->queries + b * mq * 3, q.data() + b * mq * 3, rows * 3 * sizeof(double));
     }
   }
+  return TEBGPU_OK;
+}
+
+/* argument checks of both trajectory read-out entry points: nothing is launched when one fails */
+static int32_t check_trajectory_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebTrajectoryArgs* ta) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!bt || !ta) { ctx->err = "batch or trajectory args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->B < 1 || bt->n_cap < 1) { ctx->err = "bad batch dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->B > ctx->lim.max_bands || bt->n_cap > ctx->lim.max_poses) { ctx->err = "batch exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+  if (!bt->poses || !bt->n || !bt->vel_start || !bt->vel_goal) { ctx->err = "missing required batch array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!ta->points) { ctx->err = "points == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!ta->profile && !ta->trajectory) { ctx->err = "profile and trajectory both NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (ta->bands && ta->count < 0) { ctx->err = "count < 0"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!ctx->have_params) { ctx->err = "tebgpu_set_params has not been called"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_read_trajectory on arguments already checked */
+static int32_t issue_read_trajectory(tebgpu_ctx* ctx, const TebBatch* bt, const TebTrajectoryArgs* ta, cudaStream_t st) {
+  const int R = ta->bands ? ta->count : bt->B;
+  ctx->launches = 0;
+  if (R == 0) return TEBGPU_OK;
+  const long long grid = ((long long)R * 32 + TRAJ_THREADS - 1) / TRAJ_THREADS;
+  k_read_trajectory<<<(unsigned)grid, TRAJ_THREADS, 0, st>>>(*bt, *ta, R, ctx->params.max_vel_y);
+  ctx->last_traj_grid = grid;
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_read_trajectory_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebTrajectoryArgs* ta, void* cuda_stream) {
+  const int32_t rc = check_trajectory_args(ctx, bt, ta);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_read_trajectory(ctx, bt, ta, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+/* grows one of the read-out's device mirrors to at least `bytes` */
+static int32_t grow_mirror(tebgpu_ctx* ctx, void** p, size_t* have, size_t bytes, cudaStream_t st) {
+  if (bytes <= *have) return TEBGPU_OK;
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  if (*p) CUDA_TRY(ctx, cudaFree(*p));
+  *p = nullptr;
+  *have = 0;
+  CUDA_TRY(ctx, cudaMalloc(p, bytes));
+  *have = bytes;
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_read_trajectory(tebgpu_ctx* ctx, const TebBatch* bt, const TebTrajectoryArgs* ta) {
+  int32_t rc = check_trajectory_args(ctx, bt, ta);
+  if (rc) return rc;
+  const size_t R = ta->bands ? ta->count : bt->B;
+  /* the rows the device entry point would answer with -1 are refused here, before anything runs */
+  for (size_t r = 0; r < R; ++r) {
+    const int b = ta->bands ? ta->bands[r] : (int)r;
+    if (b < 0 || b >= bt->B) { ctx->err = "bands[r] outside 0 .. B-1"; return TEBGPU_ERR_INVALID_ARG; }
+    if (bt->n[b] < 0 || bt->n[b] > bt->n_cap) { ctx->err = "n[b] outside 0 .. n_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  if (R == 0) { ctx->launches = 0; return TEBGPU_OK; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t B = bt->B, nc = bt->n_cap, prow = (nc + 1) * 3, trow = nc * 7;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_tpoints, &ctx->tpoints_bytes, R * sizeof(int32_t), st))) return rc;
+  if (ta->bands && (rc = grow_mirror(ctx, (void**)&ctx->d_tbands, &ctx->tbands_bytes, R * sizeof(int32_t), st))) return rc;
+  if (ta->profile && (rc = grow_mirror(ctx, (void**)&ctx->d_tprof, &ctx->tprof_bytes, R * prow * sizeof(double), st))) return rc;
+  if (ta->trajectory && (rc = grow_mirror(ctx, (void**)&ctx->d_ttraj, &ctx->ttraj_bytes, R * trow * sizeof(double), st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_poses, bt->poses, B * nc * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_n, bt->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_vs, bt->vel_start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_vg, bt->vel_goal, B * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
+  if (ta->bands) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_tbands, ta->bands, R * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  TebBatch d = *bt;
+  d.poses = ctx->d_poses; d.n = ctx->d_n; d.vel_start = ctx->d_vs; d.vel_goal = ctx->d_vg;
+  TebTrajectoryArgs da = *ta;
+  da.bands = ta->bands ? ctx->d_tbands : nullptr;
+  da.points = ctx->d_tpoints;
+  da.profile = ta->profile ? ctx->d_tprof : nullptr;
+  da.trajectory = ta->trajectory ? ctx->d_ttraj : nullptr;
+  rc = issue_read_trajectory(ctx, &d, &da, st);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(ta->points, ctx->d_tpoints, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  /* only the rows the kernel wrote reach the caller: n + 1 profile rows and n trajectory rows per band read out */
+  auto rows_back = [&](double* dst, const double* src, size_t width, int extra) -> int32_t {
+    const size_t row = (nc + extra) * width;
+    std::vector<double> h(R * row);
+    CUDA_TRY(ctx, cudaMemcpy(h.data(), src, h.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (size_t r = 0; r < R; ++r)
+      std::memcpy(dst + r * row, h.data() + r * row, (size_t)(ta->points[r] + extra) * width * sizeof(double));
+    return TEBGPU_OK;
+  };
+  if (ta->profile && (rc = rows_back(ta->profile, ctx->d_tprof, 3, 1))) return rc;
+  if (ta->trajectory && (rc = rows_back(ta->trajectory, ctx->d_ttraj, 7, 0))) return rc;
   return TEBGPU_OK;
 }
 

@@ -6,6 +6,10 @@
  *                       decision, initTrajectoryToGoal or updateAndPruneTEB            (optimal_planner.cpp:247-321)
  *   k_velocity_command  thread per band, after k_finalize: getVelocityCommand       (optimal_planner.cpp:1135-1168)
  *
+ * and, on its own (tebgpu_read_trajectory / tebgpu_read_trajectory_device):
+ *
+ *   k_read_trajectory   warp per band read out: getVelocityProfile, getFullTrajectory (optimal_planner.cpp:1170-1248)
+ *
  * The band routines are in teb_plan.h. k_plan_begin leaves a band it could not plan untouched and hands the reason
  * (TEB_STATUS_BAD_INPUT, TEB_STATUS_CAPACITY) to k_begin through DevBatch::pre_status, so the optimize sequence skips
  * it and k_finalize reports it, as it does for a band autoResize could not grow.
@@ -111,6 +115,58 @@ __global__ void k_velocity_command(DevBatch db, const __grid_constant__ TebParam
                      : 0;
   double* c = pi.cmd + 4 * (size_t)b;
   c[0] = v[0]; c[1] = v[1]; c[2] = v[2]; c[3] = ok;
+}
+
+constexpr int TRAJ_THREADS = 128; /* k_read_trajectory: 4 output rows per CTA */
+
+/* getVelocityProfile / getFullTrajectory (optimal_planner.cpp:1170-1248) of band bands[r] (or r) into output row r, one
+ * warp per row (tebgpu_read_trajectory). Lane l takes poses l, l + 32, ...; pose i recomputes its two adjacent segments
+ * (i - 1 -> i and i -> i + 1) as the reference does. time_from_start is the reference's sequential sum: the warp walks
+ * the 32 time differences of a step one shuffle at a time, in order, so the sum is never reassociated. */
+__global__ void __launch_bounds__(TRAJ_THREADS) k_read_trajectory(TebBatch bt, TebTrajectoryArgs a, int R, double max_vel_y) {
+  const int r = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= R) return; /* whole warps leave together */
+  const int b = a.bands ? a.bands[r] : r;
+  const int n = b >= 0 && b < bt.B ? bt.n[b] : -1;
+  if (n < 0 || n > bt.n_cap) {
+    if (lane == 0) a.points[r] = -1;
+    return;
+  }
+  if (lane == 0) a.points[r] = n;
+  const double* rec = bt.poses + (size_t)b * bt.n_cap * 4;
+  const double* vs = bt.vel_start + 4 * (size_t)b;
+  const double* vg = bt.vel_goal + 4 * (size_t)b;
+  double* prof = a.profile ? a.profile + (size_t)r * (bt.n_cap + 1) * 3 : nullptr;
+  double* traj = a.trajectory ? a.trajectory + (size_t)r * bt.n_cap * 7 : nullptr;
+  double carry = 0.0; /* time_from_start of the next step's first pose, the same on every lane */
+  for (int base = 0; base <= n; base += 32) {
+    const int i = base + lane;
+    double v1[3] = {0, 0, 0}, v2[3] = {0, 0, 0};
+    if (i >= 1 && i <= n - 1) teb_extract_velocity(rec + 4 * (i - 1), rec + 4 * i, rec[4 * (i - 1) + 3], max_vel_y, v1);
+    if (prof && i <= n) { /* n == 0: the one row is the goal velocity */
+      const double* v = i == n ? vg : (i == 0 ? vs : v1);
+      for (int c = 0; c < 3; ++c) prof[3 * i + c] = v[c];
+    }
+    if (!traj) continue;
+    const double dt = i < n ? rec[4 * i + 3] : 0.0;
+    double t = 0.0;
+    for (int j = 0; j < 32; ++j) {
+      if (lane == j) t = carry;
+      carry = teb_add(carry, __shfl_sync(0xffffffffu, dt, j));
+    }
+    if (i >= n) continue;
+    double* o = traj + 7 * (size_t)i;
+    o[0] = rec[4 * i]; o[1] = rec[4 * i + 1]; o[2] = rec[4 * i + 2];
+    if (i == 0 || i == n - 1) { /* n == 1: the start velocity */
+      const double* v = i == 0 ? vs : vg;
+      o[3] = v[0]; o[4] = v[1]; o[5] = v[2];
+    } else {
+      teb_extract_velocity(rec + 4 * i, rec + 4 * (i + 1), dt, max_vel_y, v2);
+      for (int c = 0; c < 3; ++c) o[3 + c] = teb_mul(0.5, teb_add(v1[c], v2[c]));
+    }
+    o[6] = t;
+  }
 }
 
 }  // namespace tebgpu

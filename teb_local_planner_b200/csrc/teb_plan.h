@@ -10,6 +10,8 @@
  *   updateAndPruneTEB                          src/timed_elastic_band.cpp:555-597 (the search and the shift are
  *                                              spread over a warp in k_plan_begin; the distance is teb_plan_dist)
  *   getVelocityCommand / extractVelocity       src/optimal_planner.cpp:1097-1168
+ *   getVelocityProfile / getFullTrajectory     src/optimal_planner.cpp:1170-1248 (teb_extract_velocity per segment,
+ *                                              spread over a warp in k_read_trajectory)
  *
  * Record layout as in teb_resize.h: rec[4*i+0..3] = x_i, y_i, theta_i, dt_i; record n-1 has dt = 0.
  *
@@ -149,6 +151,25 @@ TEB_HD inline int teb_init_from_plan_records(double* rec, int n_cap, const doubl
   return k;
 }
 
+/* extractVelocity(pose1, pose2, dt) (optimal_planner.cpp:1097-1133) of the records p1, p2: v[0..2] = vx, vy, omega.
+ * dt == 0 gives zeros. max_vel_y == 0 (non-holonomic): vx is the step length signed by the step's projection on p1's
+ * heading (g2o::sign(0) == 0), vy = 0; otherwise the step in p1's frame over dt. */
+TEB_HD inline void teb_extract_velocity(const double* p1, const double* p2, double dt, double max_vel_y, double* v) {
+  v[0] = v[1] = v[2] = 0;
+  if (dt == 0) return;
+  const double sx = p2[0] - p1[0], sy = p2[1] - p1[1];
+  const double c = cos(p1[2]), s = sin(p1[2]);
+  const double along = teb_add(teb_mul(c, sx), teb_mul(s, sy));
+  if (max_vel_y == 0) {
+    const double sign = along > 0 ? 1.0 : (along < 0 ? -1.0 : 0.0);
+    v[0] = teb_mul(sign, sqrt(teb_add(teb_mul(sx, sx), teb_mul(sy, sy)))) / dt;
+  } else {
+    v[0] = along / dt;
+    v[1] = teb_add(teb_mul(-s, sx), teb_mul(c, sy)) / dt;
+  }
+  v[2] = teb_normalize_theta(p2[2] - p1[2]) / dt;
+}
+
 /* getVelocityCommand(vx, vy, omega, look_ahead_poses) on a band of n poses: v[0..2] = vx, vy, omega; returns the
  * command's validity (0 with zeros for fewer than 2 poses or a non-positive accumulated time) */
 TEB_HD inline int teb_velocity_command(const double* rec, int n, int look_ahead_poses, int prevent_near_goal, double dt_ref,
@@ -163,20 +184,7 @@ TEB_HD inline int teb_velocity_command(const double* rec, int n, int look_ahead_
     if (dt >= dt_ref * target) { target = k + 1; break; }
   }
   if (dt <= 0) return 0;
-  /* extractVelocity(Pose(0), Pose(target), dt) */
-  const double* p1 = rec;
-  const double* p2 = rec + 4 * target;
-  const double sx = p2[0] - p1[0], sy = p2[1] - p1[1];
-  const double c = cos(p1[2]), s = sin(p1[2]);
-  const double along = teb_add(teb_mul(c, sx), teb_mul(s, sy));
-  if (max_vel_y == 0) {
-    const double sign = along > 0 ? 1.0 : (along < 0 ? -1.0 : 0.0);
-    v[0] = teb_mul(sign, sqrt(teb_add(teb_mul(sx, sx), teb_mul(sy, sy)))) / dt;
-  } else {
-    v[0] = along / dt;
-    v[1] = teb_add(teb_mul(-s, sx), teb_mul(c, sy)) / dt;
-  }
-  v[2] = teb_normalize_theta(p2[2] - p1[2]) / dt;
+  teb_extract_velocity(rec, rec + 4 * target, dt, max_vel_y, v);
   return 1;
 }
 
