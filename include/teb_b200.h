@@ -297,8 +297,50 @@ typedef struct TebTrajectoryArgs {
                                 (trajectory) are not written. */
 } TebTrajectoryArgs;
 
+/* Each scene's obstacle table built from its local costmap (tebgpu_costmap_obstacles): the branch of
+ * TebLocalPlannerROS::updateObstacleContainerWithCostmap without a costmap_converter plugin, the reference's default
+ * (teb_local_planner_ros.cpp:343-352, :478-504), followed by the custom obstacles (:552-625). HOST pointers for
+ * tebgpu_costmap_obstacles, DEVICE pointers for tebgpu_costmap_obstacles_device.
+ *
+ * Inputs of scene s: the costmap's size (sx, sy) = grid[s] in cells, its origin (ox, oy) and resolution r = origin[s],
+ * the robot pose (rx, ry, rt) = robot[s] in the costmap's global frame (robot_pose_), and the char map
+ * cost[s][my * sx + mx], costmap_2d's getCharMap() as it is (getCost(mx, my) reads my * size_x + mx). The rows, in order:
+ *   1. If include_costmap_obstacles != 0, for i = 0 .. sx - 2 (outer) and j = 0 .. sy - 2 (inner): the last column and
+ *      the last row are never visited (the reference's < getSizeInCellsX() - 1); sx < 2 or sy < 2 gives no row (at 0 the
+ *      reference's unsigned size - 1 wraps around). A cell with cost == 254 (LETHAL_OBSTACLE exactly; 253 and 255 do
+ *      not count) has the centre wx = ox + (i + 0.5) * r, wy = oy + (j + 0.5) * r (costmap_2d mapToWorld). With
+ *      dx = wx - rx, dy = wy - ry, c = cos(rt), s = sin(rt) (pose_se2.h:215) it is skipped when
+ *      dx * c + dy * s < 0 && sqrt(dx * dx + dy * dy) > behind_robot_dist (a NaN anywhere keeps it, as in the reference),
+ *      otherwise it gives the row {wx, wy, 0, 0, 0, dynamic 0, TEB_OBST_POINT, 0, 0, _pad 0}: every byte is defined.
+ *      Every product and sum is rounded on its own (no FMA contraction), as in the reference's x86 build.
+ *   2. Then custom[s][0 .. custom_count[s]) verbatim. Their vertex_begin refers to the batch's obst_vertices, which the
+ *      caller fills; Point rows use no vertex, so nothing is rebased.
+ *   3. needed[s] = the number of rows. If it is <= M_cap, obst_count[s] = needed[s]; otherwise the first M_cap rows are
+ *      written and obst_count[s] = -1, which every consumer refuses (TEB_STATUS_BAD_INPUT from the optimize and plan
+ *      entry points, -1 from the feasibility check, NaN from the device H-signature): no obstacle is dropped silently.
+ *      Rows past obst_count (past M_cap on overflow) are not written. */
+typedef struct TebCostmapArgs {
+  int32_t  S;                  /* scenes, 1 .. max_scenes */
+  int32_t  cell_cap;           /* raster bytes per scene (stride of cost), >= sx * sy; a multiple of 16 with a 16-byte
+                                  aligned cost lets the device read the raster with 16-byte loads */
+  int32_t  M_cap;              /* output rows per scene (stride of obstacles), 1 .. max_obstacles */
+  int32_t  C_cap;              /* custom rows per scene (stride of custom), >= 0 */
+  int32_t  include_costmap_obstacles; /* obstacles.include_costmap_obstacles (teb_config.h:133, default true) */
+  int32_t  _pad;
+  double   behind_robot_dist;  /* obstacles.costmap_obstacles_behind_robot_dist (teb_config.h:134, default 1.5) */
+  const uint8_t*     cost;     /* [S][cell_cap] */
+  const int32_t*     grid;     /* [S][2] sx, sy */
+  const double*      origin;   /* [S][3] ox, oy, r */
+  const double*      robot;    /* [S][3] rx, ry, rt */
+  const TebObstacle* custom;   /* [S][C_cap] or NULL (C_cap == 0) */
+  const int32_t*     custom_count; /* [S] or NULL: no custom rows */
+  TebObstacle*       obstacles;    /* [S][M_cap] out, 16-byte aligned */
+  int32_t*           obst_count;   /* [S] out */
+  int32_t*           needed;       /* [S] out or NULL; saturates at INT32_MAX */
+} TebCostmapArgs;
+
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
- * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs. */
+ * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -389,6 +431,19 @@ int32_t tebgpu_read_trajectory(tebgpu_ctx* ctx, const TebBatch* batch, const Teb
 int32_t tebgpu_read_trajectory_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebTrajectoryArgs* args,
                                       void* cuda_stream);
 
+/* The obstacle table of every scene from its local costmap, as defined at TebCostmapArgs, written where a TebBatch reads
+ * it (obstacles, obst_count): convert, then plan and check on the same stream. One CTA per scene stages the raster in
+ * shared memory and enumerates it in the reference's order (tebgpu_get_info key 15). Argument errors (NULL required
+ * arrays, S outside 1 .. max_scenes, M_cap outside 1 .. max_obstacles, cell_cap or C_cap < 0, C_cap > 0 with custom ==
+ * NULL, a misaligned obstacles or custom pointer) return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit)
+ * before anything is launched. tebgpu_costmap_obstacles: HOST buffers, synchronous; a negative size, sx * sy > cell_cap
+ * or a custom_count outside 0 .. C_cap is refused with TEBGPU_ERR_INVALID_ARG too; its device copies are allocated by
+ * the first call that needs them. tebgpu_costmap_obstacles_device: DEVICE buffers, stream ordered as
+ * tebgpu_optimize_batch_device, does not synchronise; such a scene gets obst_count = needed = -1 and nothing else, the
+ * other scenes are converted. */
+int32_t tebgpu_costmap_obstacles(tebgpu_ctx* ctx, const TebCostmapArgs* args);
+int32_t tebgpu_costmap_obstacles_device(tebgpu_ctx* ctx, const TebCostmapArgs* args, void* cuda_stream);
+
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded
  *   LDL^T with the active window in registers, and the accept / reject chain is replayed in order;
@@ -447,7 +502,10 @@ int32_t tebgpu_get_plan_kernel_times(tebgpu_ctx* ctx, double ms_out[2], int64_t 
  * scene, stride M_cap. The path is the band's pose positions; use_timediffs != 0 takes the transition times from the
  * band's dt, 0 approximates them by |z2 - z1| / max_vel_x (h_signature.h:307-315, graph-search candidates have no time
  * information yet). The reference accumulates the 2-D signature in long double; the device uses fp64 (|dH| <= 1e-9 |H|
- * against the long double oracle, far below h_signature_threshold). device_ptrs as in tebgpu_build_system. */
+ * against the long double oracle, far below h_signature_threshold). device_ptrs as in tebgpu_build_system. The host
+ * buffers are checked before anything runs; with device pointers a band whose scene_id is outside 0 .. S - 1, whose
+ * scene's obst_count is outside 0 .. M_cap (-1 from an overflowing tebgpu_costmap_obstacles_device) or whose n is
+ * outside 0 .. n_cap gets NaN in every output of its row. */
 int32_t tebgpu_h_signature(tebgpu_ctx* ctx, const TebBatch* batch, int32_t use_timediffs, double* h_out, int32_t device_ptrs);
 
 /* Number of kernels launched by the last optimize call (for bench.py's gpu_launches). */
@@ -461,7 +519,8 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * CUDA graph issues none), 11 which build that launch ran (TEBGPU_KA_BUILD_*, -1 before the first), 12 grid in CTAs of
  * the last feasibility-check launch (0 before the first), 13 which build that launch ran (TEBGPU_FEAS_BUILD_*, -1 before
  * the first), 14 grid in CTAs of the last trajectory read-out launch (k_read_trajectory, 4 rows per CTA; 0 before the
- * first). Returns -1 for an unknown key. */
+ * first), 15 grid in CTAs of the last costmap conversion (k_costmap_obstacles, one CTA per scene; 0 before the first).
+ * Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2 2       /* k_trial_eval2 (B <= 2 x SMs): B CTAs */

@@ -58,6 +58,10 @@ def load_library(build_if_missing=False):
     L.tebgpu_read_trajectory.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebTrajectoryArgs)]
     L.tebgpu_read_trajectory_device.restype = C.c_int32
     L.tebgpu_read_trajectory_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebTrajectoryArgs), vp]
+    L.tebgpu_costmap_obstacles.restype = C.c_int32
+    L.tebgpu_costmap_obstacles.argtypes = [vp, C.POINTER(abi.TebCostmapArgs)]
+    L.tebgpu_costmap_obstacles_device.restype = C.c_int32
+    L.tebgpu_costmap_obstacles_device.argtypes = [vp, C.POINTER(abi.TebCostmapArgs), vp]
     L.tebgpu_get_plan_kernel_times.restype = C.c_int32
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
@@ -115,7 +119,7 @@ def load_library(build_if_missing=False):
     L.tebgpu_auto_resize_host.restype = C.c_int32
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
     for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
-                                abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs)):
+                                abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -264,6 +268,47 @@ class TebGpu:
         ta.profile, ta.trajectory, ta.points = addr(profile), addr(trajectory), addr(points)
         self._check(self.lib.tebgpu_read_trajectory_device(self.ctx, C.byref(batch_struct), C.byref(ta), stream),
                     "tebgpu_read_trajectory_device")
+
+    def costmap_obstacles(self, cost, grid, origin, robot, M_cap, behind_robot_dist=1.5, include=True, custom=None,
+                          custom_count=None):
+        """Each scene's obstacle table from its local costmap (tebgpu_costmap_obstacles), host buffers: cost [S][cell_cap]
+        uint8 (scene s's char map in its first sx * sy bytes, row my = mx + my * sx), grid [S][2] (sx, sy), origin [S][3]
+        (ox, oy, resolution), robot [S][3] (x, y, yaw), custom [S][C_cap] abi.OBST_DTYPE rows appended after the points,
+        custom_count [S]. Returns (obstacles [S][M_cap] abi.OBST_DTYPE, zero past each scene's written rows, obst_count
+        [S]: the rows, or -1 when they do not fit M_cap, needed [S]: the rows the scene has)."""
+        import numpy as np
+        cost = np.ascontiguousarray(cost, dtype=np.uint8)
+        S = cost.shape[0]
+        cost = cost.reshape(S, -1)
+        grid = np.ascontiguousarray(grid, dtype=np.int32).reshape(S, 2)
+        origin = np.ascontiguousarray(origin, dtype=np.float64).reshape(S, 3)
+        robot = np.ascontiguousarray(robot, dtype=np.float64).reshape(S, 3)
+        obst = np.zeros((S, int(M_cap)), abi.OBST_DTYPE)
+        cnt = np.zeros(S, np.int32)
+        need = np.zeros(S, np.int32)
+        ca = abi.TebCostmapArgs()
+        ca.S, ca.cell_cap, ca.M_cap = S, cost.shape[1], int(M_cap)
+        ca.include_costmap_obstacles, ca.behind_robot_dist = int(bool(include)), float(behind_robot_dist)
+        ca.cost, ca.grid, ca.origin, ca.robot = abi.ptr(cost), abi.ptr(grid), abi.ptr(origin), abi.ptr(robot)
+        if custom is not None:
+            custom = np.ascontiguousarray(custom, dtype=abi.OBST_DTYPE).reshape(S, -1)
+            cc = (np.full(S, custom.shape[1], np.int32) if custom_count is None
+                  else np.ascontiguousarray(custom_count, dtype=np.int32).reshape(S))
+            ca.C_cap, ca.custom, ca.custom_count = custom.shape[1], abi.ptr(custom), abi.ptr(cc)
+        ca.obstacles, ca.obst_count, ca.needed = abi.ptr(obst), abi.ptr(cnt), abi.ptr(need)
+        self._check(self.lib.tebgpu_costmap_obstacles(self.ctx, C.byref(ca)), "tebgpu_costmap_obstacles")
+        return obst, cnt, need
+
+    def costmap_obstacles_device(self, args, stream=None):
+        """tebgpu_costmap_obstacles_device: the same conversion over DEVICE memory (args: an abi.TebCostmapArgs of device
+        pointers, e.g. the obstacles / obst_count of the batch it feeds). Stream ordered on `stream` (a cudaStream_t
+        handle; None: the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_costmap_obstacles_device(self.ctx, C.byref(args), stream),
+                    "tebgpu_costmap_obstacles_device")
+
+    def last_costmap_grid(self):
+        """grid in CTAs (one per scene) of the last costmap conversion, 0 before the first"""
+        return self.info(15)
 
     FEAS_BUILDS = {0: "staged", 1: "global"}   # TEBGPU_FEAS_BUILD_*
 

@@ -145,6 +145,18 @@ class TebTrajectoryArgs(C.Structure):
                 ("points", C.c_void_p)]
 
 
+class TebCostmapArgs(C.Structure):
+    """Each scene's obstacle table from its local costmap (tebgpu_costmap_obstacles): the rasters, their geometry, the
+    robot poses, optional custom rows, and host or device output pointers"""
+    _fields_ = [("S", _i), ("cell_cap", _i), ("M_cap", _i), ("C_cap", _i), ("include_costmap_obstacles", _i), ("_pad", _i),
+                ("behind_robot_dist", _d), ("cost", C.c_void_p), ("grid", C.c_void_p), ("origin", C.c_void_p),
+                ("robot", C.c_void_p), ("custom", C.c_void_p), ("custom_count", C.c_void_p), ("obstacles", C.c_void_p),
+                ("obst_count", C.c_void_p), ("needed", C.c_void_p)]
+
+
+COSTMAP_LETHAL = 254   # costmap_2d::LETHAL_OBSTACLE, the one cost that gives a row
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

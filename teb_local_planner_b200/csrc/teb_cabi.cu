@@ -20,6 +20,7 @@
 #include "teb_hsig.cuh"
 #include "teb_plan.cuh"
 #include "teb_feasible.cuh"
+#include "teb_costmap.cuh"
 #include "teb_comm.h"
 #include <cstdlib>
 
@@ -117,6 +118,13 @@ struct tebgpu_ctx {
   int32_t* d_tbands = nullptr; int32_t* d_tpoints = nullptr; double* d_tprof = nullptr; double* d_ttraj = nullptr;
   size_t tbands_bytes = 0, tpoints_bytes = 0, tprof_bytes = 0, ttraj_bytes = 0;
   long long last_traj_grid = 0;       /* grid in CTAs of the last k_read_trajectory launch */
+  /* costmap conversion: the host-buffer entry point's input and output mirrors, grown by the first call that needs more */
+  uint8_t* d_ccost = nullptr; int32_t* d_cgrid = nullptr; double* d_corigin = nullptr; double* d_crobot = nullptr;
+  TebObstacle* d_ccustom = nullptr; int32_t* d_ccount = nullptr; TebObstacle* d_cobst = nullptr; int32_t* d_cocount = nullptr;
+  int32_t* d_cneeded = nullptr;
+  size_t ccost_bytes = 0, cgrid_bytes = 0, corigin_bytes = 0, crobot_bytes = 0, ccustom_bytes = 0, ccount_bytes = 0,
+         cobst_bytes = 0, cocount_bytes = 0, cneeded_bytes = 0;
+  long long last_costmap_grid = 0;    /* grid in CTAs of the last k_costmap_obstacles launch */
   size_t smem_a = 0, smem_b = 0, smem_g = 0;
   /* profiling */
   bool profiling = false;
@@ -208,6 +216,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 5: return (int32_t)sizeof(TebPlanInput);
     case 6: return (int32_t)sizeof(TebFeasibilityArgs);
     case 7: return (int32_t)sizeof(TebTrajectoryArgs);
+    case 8: return (int32_t)sizeof(TebCostmapArgs);
     default: return -1;
   }
 }
@@ -232,6 +241,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 12: return ctx->last_feas_grid;
     case 13: return ctx->last_feas_build;
     case 14: return ctx->last_traj_grid;
+    case 15: return ctx->last_costmap_grid;
     default: return -1;
   }
 }
@@ -240,7 +250,9 @@ static void free_all(tebgpu_ctx* c) {
   void* ptrs[] = {c->Lf2, c->dx2, c->arrive, c->d_gather, c->d_hsig, c->assoc3, c->occ, c->dyn_idx, c->dyn_cnt, c->rhs, c->dmax_parts, c->spec.Lf, c->spec.dx, c->spec.res, c->spec.need, c->spec.qmax, c->spec.cnt, c->spec.list, c->defer, c->d_fp, c->d_pverts, c->Hb, c->assoc, c->dyn_t, c->via_idx, c->chi_parts, c->state, c->d_poses, c->d_n, c->d_scene,
                   c->d_obst, c->d_ocount, c->d_via, c->d_vcount, c->d_vs, c->d_vg, c->d_rot, c->d_cost, c->d_chi2,
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
-                  c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj};
+                  c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
+                  c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
+                  c->d_cneeded};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1529,6 +1541,90 @@ int32_t tebgpu_read_trajectory(tebgpu_ctx* ctx, const TebBatch* bt, const TebTra
   };
   if (ta->profile && (rc = rows_back(ta->profile, ctx->d_tprof, 3, 1))) return rc;
   if (ta->trajectory && (rc = rows_back(ta->trajectory, ctx->d_ttraj, 7, 0))) return rc;
+  return TEBGPU_OK;
+}
+
+/* argument checks of both costmap conversion entry points: nothing is launched when one fails */
+static int32_t check_costmap_args(tebgpu_ctx* ctx, const TebCostmapArgs* ca) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!ca) { ctx->err = "costmap args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (ca->S < 1 || ca->M_cap < 1 || ca->cell_cap < 0 || ca->C_cap < 0) { ctx->err = "bad costmap dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (ca->S > ctx->lim.max_scenes || ca->M_cap > ctx->lim.max_obstacles) { ctx->err = "costmap scenes exceed the context limits"; return TEBGPU_ERR_CAPACITY; }
+  if (!ca->grid || !ca->origin || !ca->robot || !ca->obstacles || !ca->obst_count) { ctx->err = "missing required costmap array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (ca->cell_cap > 0 && !ca->cost) { ctx->err = "cost == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (ca->C_cap > 0 && ca->custom_count && !ca->custom) { ctx->err = "custom == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if ((reinterpret_cast<uintptr_t>(ca->obstacles) | reinterpret_cast<uintptr_t>(ca->custom)) & 15) { ctx->err = "obstacles / custom not 16-byte aligned"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_costmap_obstacles on arguments already checked */
+static int32_t issue_costmap(tebgpu_ctx* ctx, const TebCostmapArgs* ca, cudaStream_t st) {
+  TebCostmapArgs a = *ca;
+  if (!a.custom_count) a.custom = nullptr;
+  k_costmap_obstacles<<<ca->S, COSTMAP_THREADS, 0, st>>>(a);
+  ctx->last_costmap_grid = ca->S;
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_costmap_obstacles_device(tebgpu_ctx* ctx, const TebCostmapArgs* ca, void* cuda_stream) {
+  const int32_t rc = check_costmap_args(ctx, ca);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_costmap(ctx, ca, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_costmap_obstacles(tebgpu_ctx* ctx, const TebCostmapArgs* ca) {
+  int32_t rc = check_costmap_args(ctx, ca);
+  if (rc) return rc;
+  /* the scenes the device entry point would answer with -1 are refused here, before anything runs */
+  for (int s = 0; s < ca->S; ++s) {
+    const int32_t sx = ca->grid[2 * s], sy = ca->grid[2 * s + 1];
+    if (sx < 0 || sy < 0) { ctx->err = "negative costmap size"; return TEBGPU_ERR_INVALID_ARG; }
+    if ((long long)sx * sy > ca->cell_cap) { ctx->err = "sx * sy > cell_cap"; return TEBGPU_ERR_INVALID_ARG; }
+    if (ca->custom_count && (ca->custom_count[s] < 0 || ca->custom_count[s] > ca->C_cap)) { ctx->err = "custom_count[s] outside 0 .. C_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t S = ca->S, M = ca->M_cap, cells = S * ca->cell_cap;
+  const bool cu = ca->custom_count && ca->C_cap > 0;
+  /* cudaMalloc'd mirrors are 256-byte aligned, so a cell_cap that is a multiple of 16 keeps the 16-byte raster loads */
+  if (cells && (rc = grow_mirror(ctx, (void**)&ctx->d_ccost, &ctx->ccost_bytes, cells, st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_cgrid, &ctx->cgrid_bytes, S * 2 * sizeof(int32_t), st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_corigin, &ctx->corigin_bytes, S * 3 * sizeof(double), st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_crobot, &ctx->crobot_bytes, S * 3 * sizeof(double), st))) return rc;
+  if (cu && (rc = grow_mirror(ctx, (void**)&ctx->d_ccustom, &ctx->ccustom_bytes, S * ca->C_cap * sizeof(TebObstacle), st))) return rc;
+  if (ca->custom_count && (rc = grow_mirror(ctx, (void**)&ctx->d_ccount, &ctx->ccount_bytes, S * sizeof(int32_t), st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_cobst, &ctx->cobst_bytes, S * M * sizeof(TebObstacle), st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_cocount, &ctx->cocount_bytes, S * sizeof(int32_t), st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_cneeded, &ctx->cneeded_bytes, S * sizeof(int32_t), st))) return rc;
+  if (cells) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ccost, ca->cost, cells, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_cgrid, ca->grid, S * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_corigin, ca->origin, S * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_crobot, ca->robot, S * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  if (cu) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ccustom, ca->custom, S * ca->C_cap * sizeof(TebObstacle), cudaMemcpyHostToDevice, st));
+  if (ca->custom_count) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ccount, ca->custom_count, S * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  TebCostmapArgs da = *ca;
+  da.cost = cells ? ctx->d_ccost : nullptr;
+  da.grid = ctx->d_cgrid; da.origin = ctx->d_corigin; da.robot = ctx->d_crobot;
+  da.custom = cu ? ctx->d_ccustom : nullptr;
+  da.custom_count = ca->custom_count ? ctx->d_ccount : nullptr;
+  da.obstacles = ctx->d_cobst; da.obst_count = ctx->d_cocount; da.needed = ctx->d_cneeded;
+  rc = issue_costmap(ctx, &da, st);
+  if (rc) return rc;
+  std::vector<int32_t> need(S);
+  CUDA_TRY(ctx, cudaMemcpyAsync(ca->obst_count, ctx->d_cocount, S * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(need.data(), ctx->d_cneeded, S * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  if (ca->needed) std::memcpy(ca->needed, need.data(), S * sizeof(int32_t));
+  /* only the rows the kernel wrote reach the caller: min(needed, M_cap) per scene */
+  for (size_t s = 0; s < S; ++s) {
+    const size_t rows = std::min<size_t>((size_t)std::max(need[s], 0), M);
+    if (rows)
+      CUDA_TRY(ctx, cudaMemcpyAsync(ca->obstacles + s * M, ctx->d_cobst + s * M, rows * sizeof(TebObstacle), cudaMemcpyDeviceToHost, st));
+  }
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
 }
 

@@ -43,13 +43,22 @@ __device__ __forceinline__ bool hsig_closer_than_skip(double ax, double ay, doub
   return (s - c2) + (lo - c2e) < 0.0; /* s - c2 is exact here (Sterbenz): this path runs only when s is within 1e-12 of c2 */
 }
 
+/* the band's n and scene_id index the staging and the scene's tables; obst_count is range-checked by the caller */
+__device__ __forceinline__ bool hsig_band_ok(const DevBatch& db, int n, int sc) {
+  return n >= 0 && n <= db.n_cap && sc >= 0 && sc < db.S;
+}
+
 __global__ void __launch_bounds__(HSIG_THREADS) k_hsig2d(DevBatch db, KParams kp, double* out) {
   extern __shared__ __align__(16) unsigned char hs_raw[];
   const int b = blockIdx.x, tid = threadIdx.x;
   const int n = db.n[b];
   const int sc = db.scene_id[b];
-  const int M = db.obst_count[sc];
+  const int M = hsig_band_ok(db, n, sc) ? db.obst_count[sc] : -1;
   const int Mc = db.M_cap > 0 ? db.M_cap : 1;
+  if (M < 0 || M > db.M_cap) { /* a scene the batch cannot describe (device pointers only): no signature */
+    if (tid == 0) { out[2 * b] = NAN; out[2 * b + 1] = NAN; }
+    return;
+  }
   double* sox = reinterpret_cast<double*>(hs_raw);
   double* soy = sox + Mc;
   double* sAr = soy + Mc;
@@ -154,8 +163,12 @@ __global__ void __launch_bounds__(HSIG_THREADS) k_hsig3d(DevBatch db, KParams kp
   const int b = blockIdx.x, tid = threadIdx.x;
   const int n = db.n[b];
   const int sc = db.scene_id[b];
-  const int M = db.obst_count[sc];
+  const int M = hsig_band_ok(db, n, sc) ? db.obst_count[sc] : -1;
   const int Mc = db.M_cap > 0 ? db.M_cap : 1;
+  if (M < 0 || M > db.M_cap) { /* a scene the batch cannot describe (device pointers only): no signature */
+    for (int l = tid; l < Mc; l += HSIG_THREADS) out[(size_t)b * Mc + l] = NAN;
+    return;
+  }
   double* spx = reinterpret_cast<double*>(hs_raw) + 4 * Mc;
   double* spy = spx + db.n_cap;
   double* sT = spy + db.n_cap; /* transition time at pose k */

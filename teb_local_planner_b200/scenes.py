@@ -4,6 +4,8 @@ A *request* is one planning problem (start, goal, obstacle table); a *candidate*
 of that request in its own homotopy-like class (lateral sinusoid of amplitude A_k). The batch axis of
 the optimizer is candidates x requests.
 """
+import math
+
 import numpy as np
 
 from . import abi
@@ -226,3 +228,46 @@ def costmap_scene(M, n=100, candidates=3, seed=0, amp=0.6, shapes=True):
     hb = abi.HostBatch(poses, np.full(candidates, n, np.int32), o, np.array([M], np.int32),
                        obst_vertices=pool[None] if shapes else None)
     return p, hb
+
+
+def costmap_raster(S, sx=120, sy=120, res=0.05, lethal=0.05, seed=0, cell_cap=None):
+    """A fleet of S local costmaps the way costmap_2d fills them, for tebgpu_costmap_obstacles: two walls and blobs of
+    LETHAL_OBSTACLE (254) cells until `lethal` of the cells are lethal, an inflation ring around them (253 next to a
+    lethal cell, lower costs further out) and a 4 x 4 patch of NO_INFORMATION (255), so the raster holds values next to
+    254 that must not count. Each map is centred near its robot (a rolling window), whose yaw is drawn over (-pi, pi].
+    -> dict(cost [S][cell_cap] uint8 (row my holds cells my * sx .. my * sx + sx - 1; cell_cap defaults to sx * sy
+    rounded up to 16 bytes), grid [S][2] int32, origin [S][3] (ox, oy, res), robot [S][3] (x, y, yaw))."""
+    rng = np.random.default_rng(seed)
+    cap = ((sx * sy + 15) // 16) * 16 if cell_cap is None else int(cell_cap)
+    cost = np.zeros((S, cap), np.uint8)
+    grid = np.tile(np.array([sx, sy], np.int32), (S, 1))
+    origin = np.zeros((S, 3))
+    robot = np.zeros((S, 3))
+    yy, xx = np.mgrid[0:sy, 0:sx]
+    ring = [(dx, dy, math.hypot(dx, dy)) for dx in range(-4, 5) for dy in range(-4, 5) if 0 < math.hypot(dx, dy) <= 4]
+    for s in range(S):
+        rx, ry = rng.uniform(-20, 20, 2)
+        origin[s] = (rx - 0.5 * sx * res + rng.uniform(-0.3, 0.3), ry - 0.5 * sy * res + rng.uniform(-0.3, 0.3), res)
+        robot[s] = (rx, ry, rng.uniform(-math.pi, math.pi))
+        m = np.zeros((sy, sx), bool)
+        if sx > 0 and sy > 0:
+            for wy in (int(0.15 * sy), int(0.85 * sy)):                   # two walls
+                m[wy, int(0.1 * sx):int(0.9 * sx)] = True
+            target = lethal * sx * sy
+            while m.sum() < target:                                       # blobs
+                cx, cy, r = rng.uniform(0, sx), rng.uniform(0, sy), rng.uniform(1.0, 6.0)
+                m |= (xx - cx) ** 2 + (yy - cy) ** 2 <= r * r
+        d = np.full((sy, sx), np.inf)                                     # distance to the nearest lethal cell, in cells
+        pad = np.pad(m, 4)
+        for dx, dy, h in ring:
+            d = np.where(pad[4 + dy:4 + dy + sy, 4 + dx:4 + dx + sx], np.minimum(d, h), d)
+        c = np.zeros((sy, sx), np.uint8)
+        c[d <= 1.0] = 253                                                 # INSCRIBED_INFLATED_OBSTACLE
+        far = (d > 1.0) & np.isfinite(d)
+        c[far] = (252 * np.exp(-1.5 * (d[far] - 1.0))).astype(np.uint8)
+        c[m] = 254
+        if sx >= 4 and sy >= 4:                                           # NO_INFORMATION
+            px, py = rng.integers(0, sx - 3), rng.integers(0, sy - 3)
+            c[py:py + 4, px:px + 4] = 255
+        cost[s, :sx * sy] = c.reshape(-1)
+    return dict(cost=cost, grid=grid, origin=origin, robot=robot)
