@@ -339,8 +339,99 @@ typedef struct TebCostmapArgs {
   int32_t*           needed;       /* [S] out or NULL; saturates at INT32_MAX */
 } TebCostmapArgs;
 
+/* Each robot's global plan cut into its local plan, goal and via-points (tebgpu_local_plan): the front of
+ * TebLocalPlannerROS::computeVelocityCommands from pruneGlobalPlan up to the start row (teb_local_planner_ros.cpp:268-340),
+ * under the identity transform: the global plan is given in the frame of the costmap and of the obstacle tables. HOST
+ * pointers for tebgpu_local_plan, DEVICE pointers for tebgpu_local_plan_device. Of the batch only B, S and scene_id are
+ * read. One output row per band b; plan / plan_count and via / via_count have the layout of TebPlanInput.initial_plan /
+ * plan_count and TebBatch.via / via_count, so they feed tebgpu_plan_batch(_device) on the same stream.
+ *
+ * Band b's global plan is global_plan[b][plan_begin[b] .. plan_end[b]) (x, y, yaw); g[k] below is its row plan_begin + k
+ * after step 1, n = plan_end - plan_begin its live rows. (rx, ry, rt) = robot[b]. Every product and sum is rounded on its
+ * own (no FMA contraction), pow(d, 2) is d * d, and a NaN goes through every comparison as in the reference (false).
+ *   1. Prune (:657-698): plan_begin moves to the first live row with dx * dx + dy * dy < prune_distance * prune_distance
+ *      (dx = rx - x, dy = ry - y); none: nothing moves. No row is moved in memory.
+ *   2. n == 0: result TEB_LOCAL_PLAN_EMPTY, plan_count = 0, nothing else is written (the reference reads
+ *      global_plan[0] before its empty check).
+ *   3. Transform (:701-822). The window is w * w with w = max((double)sx * r / 2.0, (double)sy * r / 2.0) * 0.85
+ *      ((sx, sy) = grid[scene_id[b]], r = origin[scene_id[b]][2]; max(a, b) = a < b ? b : a). The closest row: from
+ *      sq = 1e10, i = 0, over j = 0 .. n - 1: stop when some earlier row set sq < 0.05 and d_j > sq; take j (sq = d_j,
+ *      i = j) when d_j < sq (strict), d_j the squared distance from the robot. Then rows are taken from i while i < n,
+ *      the squared distance of the row taken last (at first the search's sq) is <= the window, and max_lookahead_dist
+ *      <= 0 or plan_length <= max_lookahead_dist; taking row i > 0 adds distance_points2d(g[i - 1], g[i]) to
+ *      plan_length (only when max_lookahead_dist > 0), in order, so the segment into the closest row counts. The row
+ *      that first leaves the window is still taken. goal_idx = (one past the last row taken) - 1; when no row is taken
+ *      the plan is the one row g[n - 1] and goal_idx = n - 1.
+ *   4. Via-points (:627-646), when via != NULL, from the rows of step 3: none if viapoint_sep <= 0; otherwise rows 1 ..
+ *      in order, each taken when distance_points2d(last via-point or row 0, row) < viapoint_sep is false.
+ *   5. Goal reached (:290-304) when sqrt(dx * dx + dy * dy) < xy_goal_tolerance (dx = g[n - 1].x - rx, ...),
+ *      |normalize_theta(teb_plan_yaw(g[n - 1].yaw) - rt)| < yaw_goal_tolerance, (!complete_global_plan || via count == 0)
+ *      (via == NULL: via_count[b] as given, 0 for NULL) and (stopped || free_goal_vel), stopped =
+ *      |omega| <= theta_stopped_vel && |vx| <= trans_stopped_vel && |vy| <= trans_stopped_vel of robot_vel[b]
+ *      (base_local_planner::stopped). Result TEB_LOCAL_PLAN_GOAL_REACHED: the via-points and goal_idx are written,
+ *      plan_count = 0, so a following tebgpu_plan_batch_device leaves the band as it was; the reference returns a zero
+ *      command there, which is the caller's to apply.
+ *   6. Horizon shrink (:950-977), when shrink_horizon_backup, infeasible_count or since_infeasible is given (NULL counts
+ *      as 0 / inf), goal_idx < size - 1 (size: rows of step 3) and (count > 0 || since < shrink_horizon_min_duration):
+ *      reduction = goal_idx / 2, halved again when count > 9; if size - reduction - 1 > 0 and goal_idx - reduction >= 0
+ *      the rows from size - reduction - 1 on are dropped and goal_idx -= reduction. As in the reference, goal_idx indexes
+ *      the global plan and size counts the rows taken from its closest row on, so goal_idx >= size - 1 and the shrink
+ *      does not fire on a plan from step 3; it is kept so the inputs mean what they mean there.
+ *   7. Goal heading (:318-333, :827-871) of the last row: its stored yaw when TebParams.global_plan_overwrite_orientation
+ *      is 0 (read from the context). Otherwise, with n and goal_idx: goal_idx >= n - 1: teb_plan_yaw(its yaw);
+ *      goal_idx > n - 5: teb_plan_yaw(g[n - 1].yaw); else atan2(sum sin, sum cos) (0 when both sums are 0; sums from 0,
+ *      in order) of the min(3, n - goal_idx - 1) headings atan2(dy, dx) from the last row to g[goal_idx + 1], then
+ *      g[goal_idx + 1] to g[goal_idx + 2], ...
+ *   8. Start row (:335-340): a one-row plan gets a row in front of it; row 0 becomes (rx, ry, rt).
+ *   9. Capacity: more than P_cap rows, or more than V_cap via-points (via != NULL): result TEB_LOCAL_PLAN_CAPACITY,
+ *      plan_count = 0, goal_idx and needed written, no row and no via-point written. No goal is moved silently.
+ * Otherwise result TEB_LOCAL_PLAN_PLANNED with plan_count rows, goal_idx after step 6 and the via-points. needed[b] =
+ * (plan rows, via-points extracted) for every band that reached step 3 (plan rows 0 when the goal is reached). Rows past
+ * plan_count and via_count are not written. tebgpu_local_plan_device answers a band whose plan_begin / plan_end is not
+ * 0 <= plan_begin <= plan_end <= G_cap, or whose scene_id is outside 0 .. S - 1, with TEB_LOCAL_PLAN_BAD_INPUT and
+ * plan_count = 0, and writes nothing else for it. */
+typedef struct TebLocalPlanArgs {
+  int32_t  G_cap;                /* global plan rows per band (stride of global_plan), >= 1 */
+  int32_t  P_cap;                /* local plan rows per band (stride of plan), >= 2 */
+  int32_t  V_cap;                /* via-points per band (stride of via), >= 0 */
+  int32_t  free_goal_vel;        /* goal_tolerance.free_goal_vel (teb_config.h:295, default false) */
+  int32_t  complete_global_plan; /* goal_tolerance.complete_global_plan (:298, default true) */
+  int32_t  shrink_horizon_backup;/* recovery.shrink_horizon_backup (:381, default true) */
+  double   prune_distance;       /* trajectory.global_plan_prune_distance (:264, default 1) */
+  double   max_lookahead_dist;   /* trajectory.max_global_plan_lookahead_dist (:263, default 1); <= 0: no length limit */
+  double   viapoint_sep;         /* trajectory.global_plan_viapoint_sep (:261, default -1: no via-points) */
+  double   xy_goal_tolerance;    /* goal_tolerance (:293, default 0.2) */
+  double   yaw_goal_tolerance;   /* (:294, default 0.2) */
+  double   trans_stopped_vel;    /* (:296, default 0.1) */
+  double   theta_stopped_vel;    /* (:297, default 0.1) */
+  double   shrink_horizon_min_duration; /* recovery (:382, default 10) */
+  const double*  global_plan;    /* [B][G_cap][3] x, y, yaw */
+  int32_t*       plan_begin;     /* [B] in/out: the first live row, moved forward by pruning */
+  const int32_t* plan_end;       /* [B] one past the last live row */
+  const double*  robot;          /* [B][3] x, y, yaw (robot_pose_) */
+  const double*  robot_vel;      /* [B][3] odometry vx, vy, omega */
+  const int32_t* grid;           /* [S][2] sx, sy: the costmap's size in cells (as TebCostmapArgs) */
+  const double*  origin;         /* [S][3] ox, oy, resolution (as TebCostmapArgs; only the resolution is read) */
+  const int32_t* infeasible_count; /* [B] or NULL: no_infeasible_plans_ */
+  const double*  since_infeasible; /* [B] or NULL: seconds since the last infeasible plan, inf: never */
+  double*        plan;           /* [B][P_cap][3] out: x, y, yaw */
+  int32_t*       plan_count;     /* [B] out */
+  int32_t*       goal_idx;       /* [B] out or NULL: the reference's goal_idx, an index into the pruned plan */
+  double*        via;            /* [B][V_cap][2] out, or NULL: the band's via-points are the caller's own
+                                    (custom_via_points_active_); nothing is written and via_count is read */
+  int32_t*       via_count;      /* [B] out (in when via == NULL, NULL there counts 0) */
+  int32_t*       result;         /* [B] out: TEB_LOCAL_PLAN_* */
+  int32_t*       needed;         /* [B][2] out or NULL: plan rows, via-points the band needed */
+} TebLocalPlanArgs;
+#define TEB_LOCAL_PLAN_PLANNED      0  /* plan, goal_idx and via-points written */
+#define TEB_LOCAL_PLAN_GOAL_REACHED 1  /* the global goal is reached: plan_count = 0 */
+#define TEB_LOCAL_PLAN_EMPTY        2  /* no live row in the global plan: plan_count = 0 */
+#define TEB_LOCAL_PLAN_CAPACITY     3  /* more rows than P_cap or via-points than V_cap: plan_count = 0, see needed */
+#define TEB_LOCAL_PLAN_BAD_INPUT    4  /* device entry point only: plan_begin / plan_end / scene_id out of range */
+
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
- * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs. */
+ * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
+ * 9 TebLocalPlanArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -444,6 +535,16 @@ int32_t tebgpu_read_trajectory_device(tebgpu_ctx* ctx, const TebBatch* batch, co
 int32_t tebgpu_costmap_obstacles(tebgpu_ctx* ctx, const TebCostmapArgs* args);
 int32_t tebgpu_costmap_obstacles_device(tebgpu_ctx* ctx, const TebCostmapArgs* args, void* cuda_stream);
 
+/* Every band's local plan, goal and via-points from its global plan, as defined at TebLocalPlanArgs: cut, then plan on
+ * the same stream. One warp per band walks the global plan in 32-row chunks, 4 bands per CTA (tebgpu_get_info key 16).
+ * Argument errors (NULL batch, scene_id or required array, B outside 1 .. max_bands, S outside 1 .. max_scenes, G_cap
+ * < 1, P_cap < 2, V_cap < 0) return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit) before anything is
+ * launched; so does tebgpu_local_plan for a band the device entry point would answer with TEB_LOCAL_PLAN_BAD_INPUT.
+ * tebgpu_local_plan: HOST buffers, synchronous; its device copies are allocated by the first call that needs them.
+ * tebgpu_local_plan_device: DEVICE buffers, stream ordered as tebgpu_optimize_batch_device, does not synchronise. */
+int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args);
+int32_t tebgpu_local_plan_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args, void* cuda_stream);
+
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded
  *   LDL^T with the active window in registers, and the accept / reject chain is replayed in order;
@@ -519,7 +620,8 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * CUDA graph issues none), 11 which build that launch ran (TEBGPU_KA_BUILD_*, -1 before the first), 12 grid in CTAs of
  * the last feasibility-check launch (0 before the first), 13 which build that launch ran (TEBGPU_FEAS_BUILD_*, -1 before
  * the first), 14 grid in CTAs of the last trajectory read-out launch (k_read_trajectory, 4 rows per CTA; 0 before the
- * first), 15 grid in CTAs of the last costmap conversion (k_costmap_obstacles, one CTA per scene; 0 before the first).
+ * first), 15 grid in CTAs of the last costmap conversion (k_costmap_obstacles, one CTA per scene; 0 before the first),
+ * 16 grid in CTAs of the last local-plan launch (k_local_plan, 4 bands per CTA; 0 before the first).
  * Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */

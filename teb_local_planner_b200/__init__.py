@@ -62,6 +62,10 @@ def load_library(build_if_missing=False):
     L.tebgpu_costmap_obstacles.argtypes = [vp, C.POINTER(abi.TebCostmapArgs)]
     L.tebgpu_costmap_obstacles_device.restype = C.c_int32
     L.tebgpu_costmap_obstacles_device.argtypes = [vp, C.POINTER(abi.TebCostmapArgs), vp]
+    L.tebgpu_local_plan.restype = C.c_int32
+    L.tebgpu_local_plan.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs)]
+    L.tebgpu_local_plan_device.restype = C.c_int32
+    L.tebgpu_local_plan_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs), vp]
     L.tebgpu_get_plan_kernel_times.restype = C.c_int32
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
@@ -119,7 +123,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_auto_resize_host.restype = C.c_int32
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
     for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
-                                abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs)):
+                                abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs,
+                                abi.TebLocalPlanArgs)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -309,6 +314,56 @@ class TebGpu:
     def last_costmap_grid(self):
         """grid in CTAs (one per scene) of the last costmap conversion, 0 before the first"""
         return self.info(15)
+
+    def local_plan(self, global_plan, plan_begin, plan_end, robot, robot_vel, grid, origin, P_cap, V_cap=None,
+                   scene_id=None, via_count=None, infeasible_count=None, since_infeasible=None, **scalars):
+        """Each robot's local plan, goal and via-points from its global plan (tebgpu_local_plan), host buffers:
+        global_plan [B][G_cap][3] (x, y, yaw), plan_begin / plan_end [B] (its live rows), robot [B][3], robot_vel [B][3]
+        (vx, vy, omega), grid [S][2] and origin [S][3] of the costmaps, scene_id [B] (None: all 0). V_cap None: the
+        via-points are the caller's own and via_count [B] (or None: 0) holds their counts; otherwise they are extracted
+        into [B][V_cap][2]. infeasible_count / since_infeasible [B] or None. scalars: abi.make_local_plan_args' keywords.
+        Returns a dict: plan_begin (moved by pruning), plan [B][P_cap][3] and via [B][V_cap][2] (NaN past the rows
+        written), plan_count, goal_idx (-1 where not written), via_count, result (TEB_LOCAL_PLAN_*), needed [B][2]."""
+        import numpy as np
+        gp = np.ascontiguousarray(global_plan, dtype=np.float64)
+        B, G_cap = gp.shape[0], gp.shape[1]
+        i32 = lambda x, shape: np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.int32)
+        f64 = lambda x, shape: np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.float64)
+        out = dict(plan_begin=i32(plan_begin, (B,)).copy(), plan=np.full((B, int(P_cap), 3), np.nan),
+                   plan_count=np.zeros(B, np.int32), goal_idx=np.full(B, -1, np.int32), result=np.full(B, -1, np.int32),
+                   needed=np.zeros((B, 2), np.int32))
+        own = V_cap is None
+        out["via"] = None if own else np.full((B, int(V_cap), 2), np.nan)
+        out["via_count"] = (np.zeros(B, np.int32) if via_count is None else i32(via_count, (B,)).copy()) if own else np.zeros(B, np.int32)
+        grid = np.ascontiguousarray(grid, dtype=np.int32).reshape(-1, 2)
+        S = grid.shape[0]
+        keep = dict(pe=i32(plan_end, (B,)), rb=f64(robot, (B, 3)), rv=f64(robot_vel, (B, 3)),
+                    org=f64(np.asarray(origin, np.float64).reshape(S, 3), (S, 3)),
+                    sid=np.zeros(B, np.int32) if scene_id is None else i32(scene_id, (B,)),
+                    inf=None if infeasible_count is None else i32(infeasible_count, (B,)),
+                    since=None if since_infeasible is None else f64(since_infeasible, (B,)))
+        la = abi.make_local_plan_args(G_cap, P_cap, 0 if own else V_cap, **scalars)
+        la.global_plan, la.plan_begin, la.plan_end = abi.ptr(gp), abi.ptr(out["plan_begin"]), abi.ptr(keep["pe"])
+        la.robot, la.robot_vel, la.grid, la.origin = abi.ptr(keep["rb"]), abi.ptr(keep["rv"]), abi.ptr(grid), abi.ptr(keep["org"])
+        la.infeasible_count, la.since_infeasible = abi.ptr(keep["inf"]), abi.ptr(keep["since"])
+        la.plan, la.plan_count, la.goal_idx = abi.ptr(out["plan"]), abi.ptr(out["plan_count"]), abi.ptr(out["goal_idx"])
+        la.via, la.via_count = abi.ptr(out["via"]), (None if own and via_count is None else abi.ptr(out["via_count"]))
+        la.result, la.needed = abi.ptr(out["result"]), abi.ptr(out["needed"])
+        bs = abi.TebBatch()
+        bs.B, bs.S, bs.scene_id = B, S, abi.ptr(keep["sid"])
+        self._check(self.lib.tebgpu_local_plan(self.ctx, C.byref(bs), C.byref(la)), "tebgpu_local_plan")
+        return out
+
+    def local_plan_device(self, batch_struct, args, stream=None):
+        """tebgpu_local_plan_device: the same step over DEVICE memory (batch_struct: an abi.TebBatch whose B, S and
+        scene_id are read; args: an abi.TebLocalPlanArgs of device pointers, see abi.make_local_plan_args). Stream
+        ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_local_plan_device(self.ctx, C.byref(batch_struct), C.byref(args), stream),
+                    "tebgpu_local_plan_device")
+
+    def last_local_plan_grid(self):
+        """grid in CTAs (4 bands each) of the last local-plan launch, 0 before the first"""
+        return self.info(16)
 
     FEAS_BUILDS = {0: "staged", 1: "global"}   # TEBGPU_FEAS_BUILD_*
 

@@ -157,6 +157,47 @@ class TebCostmapArgs(C.Structure):
 COSTMAP_LETHAL = 254   # costmap_2d::LETHAL_OBSTACLE, the one cost that gives a row
 
 
+class TebLocalPlanArgs(C.Structure):
+    """Each robot's global plan cut into its local plan, goal and via-points (tebgpu_local_plan): the global plans, the
+    robots, the costmap sizes, the step's parameters, and host or device output pointers"""
+    _fields_ = [("G_cap", _i), ("P_cap", _i), ("V_cap", _i), ("free_goal_vel", _i), ("complete_global_plan", _i),
+                ("shrink_horizon_backup", _i), ("prune_distance", _d), ("max_lookahead_dist", _d), ("viapoint_sep", _d),
+                ("xy_goal_tolerance", _d), ("yaw_goal_tolerance", _d), ("trans_stopped_vel", _d),
+                ("theta_stopped_vel", _d), ("shrink_horizon_min_duration", _d),
+                ("global_plan", C.c_void_p), ("plan_begin", C.c_void_p), ("plan_end", C.c_void_p), ("robot", C.c_void_p),
+                ("robot_vel", C.c_void_p), ("grid", C.c_void_p), ("origin", C.c_void_p),
+                ("infeasible_count", C.c_void_p), ("since_infeasible", C.c_void_p), ("plan", C.c_void_p),
+                ("plan_count", C.c_void_p), ("goal_idx", C.c_void_p), ("via", C.c_void_p), ("via_count", C.c_void_p),
+                ("result", C.c_void_p), ("needed", C.c_void_p)]
+
+
+# TEB_LOCAL_PLAN_*: the result of a band's local plan
+TEB_LOCAL_PLAN_PLANNED, TEB_LOCAL_PLAN_GOAL_REACHED, TEB_LOCAL_PLAN_EMPTY, TEB_LOCAL_PLAN_CAPACITY, \
+    TEB_LOCAL_PLAN_BAD_INPUT = range(5)
+
+
+def make_local_plan_args(G_cap, P_cap, V_cap=0, prune_distance=1.0, max_lookahead_dist=1.0, viapoint_sep=-1.0,
+                         xy_goal_tolerance=0.2, yaw_goal_tolerance=0.2, trans_stopped_vel=0.1, theta_stopped_vel=0.1,
+                         shrink_horizon_min_duration=10.0, free_goal_vel=False, complete_global_plan=True,
+                         shrink_horizon_backup=True, **arrays) -> TebLocalPlanArgs:
+    """TebLocalPlanArgs with the scalars set (the defaults are the reference's, teb_config.h:259-298, :381-382) and the
+    arrays given by keyword as addresses (ints, or None for NULL): global_plan=..., plan_begin=..., ..."""
+    a = TebLocalPlanArgs()
+    a.G_cap, a.P_cap, a.V_cap = int(G_cap), int(P_cap), int(V_cap)
+    a.free_goal_vel, a.complete_global_plan = int(bool(free_goal_vel)), int(bool(complete_global_plan))
+    a.shrink_horizon_backup = int(bool(shrink_horizon_backup))
+    a.prune_distance, a.max_lookahead_dist, a.viapoint_sep = float(prune_distance), float(max_lookahead_dist), float(viapoint_sep)
+    a.xy_goal_tolerance, a.yaw_goal_tolerance = float(xy_goal_tolerance), float(yaw_goal_tolerance)
+    a.trans_stopped_vel, a.theta_stopped_vel = float(trans_stopped_vel), float(theta_stopped_vel)
+    a.shrink_horizon_min_duration = float(shrink_horizon_min_duration)
+    names = {f[0] for f in TebLocalPlanArgs._fields_[14:]}
+    for k, v in arrays.items():
+        if k not in names:
+            raise TypeError(f"unknown TebLocalPlanArgs array {k}")
+        setattr(a, k, v)
+    return a
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

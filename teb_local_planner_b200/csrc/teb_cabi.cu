@@ -21,6 +21,7 @@
 #include "teb_plan.cuh"
 #include "teb_feasible.cuh"
 #include "teb_costmap.cuh"
+#include "teb_local_plan.cuh"
 #include "teb_comm.h"
 #include <cstdlib>
 
@@ -125,6 +126,10 @@ struct tebgpu_ctx {
   size_t ccost_bytes = 0, cgrid_bytes = 0, corigin_bytes = 0, crobot_bytes = 0, ccustom_bytes = 0, ccount_bytes = 0,
          cobst_bytes = 0, cocount_bytes = 0, cneeded_bytes = 0;
   long long last_costmap_grid = 0;    /* grid in CTAs of the last k_costmap_obstacles launch */
+  /* local plan: the host-buffer entry point's inputs and outputs, staged in one buffer grown by the first call that
+   * needs more */
+  char* d_lplan = nullptr; size_t lplan_bytes = 0;
+  long long last_lplan_grid = 0;      /* grid in CTAs of the last k_local_plan launch */
   size_t smem_a = 0, smem_b = 0, smem_g = 0;
   /* profiling */
   bool profiling = false;
@@ -217,6 +222,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 6: return (int32_t)sizeof(TebFeasibilityArgs);
     case 7: return (int32_t)sizeof(TebTrajectoryArgs);
     case 8: return (int32_t)sizeof(TebCostmapArgs);
+    case 9: return (int32_t)sizeof(TebLocalPlanArgs);
     default: return -1;
   }
 }
@@ -242,6 +248,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 13: return ctx->last_feas_build;
     case 14: return ctx->last_traj_grid;
     case 15: return ctx->last_costmap_grid;
+    case 16: return ctx->last_lplan_grid;
     default: return -1;
   }
 }
@@ -252,7 +259,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
-                  c->d_cneeded};
+                  c->d_cneeded, c->d_lplan};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1625,6 +1632,117 @@ int32_t tebgpu_costmap_obstacles(tebgpu_ctx* ctx, const TebCostmapArgs* ca) {
       CUDA_TRY(ctx, cudaMemcpyAsync(ca->obstacles + s * M, ctx->d_cobst + s * M, rows * sizeof(TebObstacle), cudaMemcpyDeviceToHost, st));
   }
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* argument checks of both local-plan entry points: nothing is launched when one fails */
+static int32_t check_local_plan_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!bt || !la) { ctx->err = "batch or local plan args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->B < 1 || bt->S < 1) { ctx->err = "bad batch dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->B > ctx->lim.max_bands || bt->S > ctx->lim.max_scenes) { ctx->err = "batch exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+  if (la->G_cap < 1 || la->P_cap < 2 || la->V_cap < 0) { ctx->err = "bad local plan strides"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!bt->scene_id || !la->global_plan || !la->plan_begin || !la->plan_end || !la->robot || !la->robot_vel || !la->grid ||
+      !la->origin || !la->plan || !la->plan_count || !la->result || (la->via && !la->via_count)) {
+    ctx->err = "missing required local plan array"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  if (!ctx->have_params) { ctx->err = "tebgpu_set_params has not been called"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_local_plan on arguments already checked */
+static int32_t issue_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la, cudaStream_t st) {
+  const long long grid = ((long long)bt->B * 32 + LPLAN_THREADS - 1) / LPLAN_THREADS;
+  k_local_plan<<<(unsigned)grid, LPLAN_THREADS, 0, st>>>(*la, bt->scene_id, bt->B, bt->S,
+                                                         ctx->params.global_plan_overwrite_orientation);
+  ctx->last_lplan_grid = grid;
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_local_plan_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la, void* cuda_stream) {
+  const int32_t rc = check_local_plan_args(ctx, bt, la);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_local_plan(ctx, bt, la, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la) {
+  int32_t rc = check_local_plan_args(ctx, bt, la);
+  if (rc) return rc;
+  /* the bands the device entry point would answer with TEB_LOCAL_PLAN_BAD_INPUT are refused here, before anything runs */
+  for (int b = 0; b < bt->B; ++b) {
+    if (la->plan_begin[b] < 0 || la->plan_begin[b] > la->plan_end[b] || la->plan_end[b] > la->G_cap) {
+      ctx->err = "plan_begin / plan_end outside 0 .. G_cap"; return TEBGPU_ERR_INVALID_ARG;
+    }
+    if (bt->scene_id[b] < 0 || bt->scene_id[b] >= bt->S) { ctx->err = "scene_id[b] outside 0 .. S-1"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t B = bt->B, S = bt->S, G = la->G_cap, P = la->P_cap, V = la->V_cap;
+  /* one staging buffer: every array at a 256-byte aligned offset */
+  size_t off = 0;
+  auto slot = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_gp = slot(B * G * 3 * sizeof(double)), o_begin = slot(B * 4), o_end = slot(B * 4),
+               o_robot = slot(B * 3 * sizeof(double)), o_vel = slot(B * 3 * sizeof(double)), o_grid = slot(S * 2 * 4),
+               o_origin = slot(S * 3 * sizeof(double)), o_sid = slot(B * 4), o_inf = slot(la->infeasible_count ? B * 4 : 0),
+               o_since = slot(la->since_infeasible ? B * sizeof(double) : 0), o_plan = slot(B * P * 3 * sizeof(double)),
+               o_pcount = slot(B * 4), o_goal = slot(B * 4), o_via = slot(la->via ? B * V * 2 * sizeof(double) : 0),
+               o_vcount = slot(B * 4), o_result = slot(B * 4), o_needed = slot(B * 2 * 4);
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_lplan, &ctx->lplan_bytes, off, st))) return rc;
+  char* d = ctx->d_lplan;
+  auto up = [&](size_t o, const void* src, size_t bytes) -> int32_t {
+    if (src && bytes) CUDA_TRY(ctx, cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, st));
+    return TEBGPU_OK;
+  };
+  /* the outputs a band may leave unwritten go up too, so that they come back as the caller left them */
+  if ((rc = up(o_gp, la->global_plan, B * G * 3 * sizeof(double))) || (rc = up(o_begin, la->plan_begin, B * 4)) ||
+      (rc = up(o_end, la->plan_end, B * 4)) || (rc = up(o_robot, la->robot, B * 3 * sizeof(double))) ||
+      (rc = up(o_vel, la->robot_vel, B * 3 * sizeof(double))) || (rc = up(o_grid, la->grid, S * 2 * 4)) ||
+      (rc = up(o_origin, la->origin, S * 3 * sizeof(double))) || (rc = up(o_sid, bt->scene_id, B * 4)) ||
+      (rc = up(o_inf, la->infeasible_count, B * 4)) || (rc = up(o_since, la->since_infeasible, B * sizeof(double))) ||
+      (rc = up(o_goal, la->goal_idx, B * 4)) || (rc = up(o_vcount, la->via_count, B * 4)) ||
+      (rc = up(o_needed, la->needed, B * 2 * 4)))
+    return rc;
+  TebBatch db = *bt;
+  db.scene_id = (const int32_t*)(d + o_sid);
+  TebLocalPlanArgs da = *la;
+  da.global_plan = (const double*)(d + o_gp);
+  da.plan_begin = (int32_t*)(d + o_begin); da.plan_end = (const int32_t*)(d + o_end);
+  da.robot = (const double*)(d + o_robot); da.robot_vel = (const double*)(d + o_vel);
+  da.grid = (const int32_t*)(d + o_grid); da.origin = (const double*)(d + o_origin);
+  da.infeasible_count = la->infeasible_count ? (const int32_t*)(d + o_inf) : nullptr;
+  da.since_infeasible = la->since_infeasible ? (const double*)(d + o_since) : nullptr;
+  da.plan = (double*)(d + o_plan); da.plan_count = (int32_t*)(d + o_pcount);
+  da.goal_idx = la->goal_idx ? (int32_t*)(d + o_goal) : nullptr;
+  da.via = la->via ? (double*)(d + o_via) : nullptr;
+  da.via_count = la->via_count ? (int32_t*)(d + o_vcount) : nullptr;
+  da.result = (int32_t*)(d + o_result);
+  da.needed = la->needed ? (int32_t*)(d + o_needed) : nullptr;
+  if ((rc = issue_local_plan(ctx, &db, &da, st))) return rc;
+  auto down = [&](void* dst, size_t o, size_t bytes) -> int32_t {
+    if (dst && bytes) CUDA_TRY(ctx, cudaMemcpyAsync(dst, d + o, bytes, cudaMemcpyDeviceToHost, st));
+    return TEBGPU_OK;
+  };
+  if ((rc = down(la->plan_begin, o_begin, B * 4)) || (rc = down(la->plan_count, o_pcount, B * 4)) ||
+      (rc = down(la->goal_idx, o_goal, B * 4)) || (rc = down(la->via ? la->via_count : nullptr, o_vcount, B * 4)) ||
+      (rc = down(la->result, o_result, B * 4)) || (rc = down(la->needed, o_needed, B * 2 * 4)))
+    return rc;
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  /* only the rows the kernel wrote reach the caller: plan_count plan rows, and via_count via-points of a band whose
+   * via-points were written */
+  std::vector<double> h(B * P * 3);
+  CUDA_TRY(ctx, cudaMemcpy(h.data(), d + o_plan, h.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  for (size_t b = 0; b < B; ++b)
+    std::memcpy(la->plan + b * P * 3, h.data() + b * P * 3, (size_t)std::max(la->plan_count[b], 0) * 3 * sizeof(double));
+  if (la->via && V) {
+    h.resize(B * V * 2);
+    CUDA_TRY(ctx, cudaMemcpy(h.data(), d + o_via, h.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (size_t b = 0; b < B; ++b)
+      if (la->result[b] == TEB_LOCAL_PLAN_PLANNED || la->result[b] == TEB_LOCAL_PLAN_GOAL_REACHED)
+        std::memcpy(la->via + b * V * 2, h.data() + b * V * 2, (size_t)std::max(la->via_count[b], 0) * 2 * sizeof(double));
+  }
   return TEBGPU_OK;
 }
 

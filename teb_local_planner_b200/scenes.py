@@ -271,3 +271,47 @@ def costmap_raster(S, sx=120, sy=120, res=0.05, lethal=0.05, seed=0, cell_cap=No
             c[py:py + 4, px:px + 4] = 255
         cost[s, :sx * sy] = c.reshape(-1)
     return dict(cost=cost, grid=grid, origin=origin, robot=robot)
+
+
+def global_plans(B, G_cap=2048, S=4, spacing=0.05, seed=0):
+    """A fleet of B robots following global plans, for tebgpu_local_plan: plans at costmap-like spacing (`spacing` m
+    between rows, yaw along the path) of four kinds by b % 4: smooth curves, loops that pass back by the robot (the
+    closest-row search meets two minima), zig-zags, and short plans that end inside the costmap window. Some rows are
+    repeated (coincident rows), the live rows start at a random plan_begin at or before the robot's row, and the robot
+    stands near that row, slightly off the path, some robots stopped. Scene s has a square costmap of 80 .. 160 cells at
+    0.05 m. -> dict(global_plan [B][G_cap][3] (NaN past plan_end), plan_begin [B], plan_end [B] int32, robot [B][3],
+    robot_vel [B][3], scene_id [B] int32, grid [S][2] int32, origin [S][3])."""
+    rng = np.random.default_rng(seed)
+    gp = np.full((B, G_cap, 3), np.nan)
+    begin, end = np.zeros(B, np.int32), np.zeros(B, np.int32)
+    robot, vel = np.zeros((B, 3)), np.zeros((B, 3))
+    sid = (np.arange(B) % S).astype(np.int32)
+    side = rng.integers(80, 161, S)
+    grid = np.stack([side, side], 1).astype(np.int32)
+    origin = np.zeros((S, 3))
+    origin[:, 2] = 0.05
+    for b in range(B):
+        kind = b % 4
+        n = int(rng.integers(5, 60)) if kind == 3 else int(rng.integers(G_cap // 2, G_cap + 1))
+        head = rng.uniform(-math.pi, math.pi)
+        turn = rng.uniform(-0.02, 0.02, n)
+        if kind == 1:                               # a loop of radius ~1 m two fifths of the way along
+            k0 = int(0.4 * n)
+            turn[k0:k0 + int(2 * math.pi / (spacing / 1.0))] = spacing / 1.0
+        elif kind == 2:                             # zig-zag: turn by +-1 rad every 10 rows
+            turn[::10] = np.where(np.arange(len(turn[::10])) % 2 == 0, 1.0, -1.0)
+        th = head + np.cumsum(turn)
+        step = np.full(n, spacing) * rng.uniform(0.8, 1.2, n)
+        step[rng.random(n) < 0.03] = 0.0            # coincident rows
+        xy = np.cumsum(np.stack([step * np.cos(th), step * np.sin(th)], 1), 0) + rng.uniform(-20, 20, 2)
+        yaw = np.arctan2(np.diff(xy[:, 1], append=xy[-1, 1]), np.diff(xy[:, 0], append=xy[-1, 0]))
+        gp[b, :n, :2], gp[b, :n, 2] = xy, yaw
+        r0 = int(rng.integers(0, max(1, n // 3))) if kind != 3 else int(rng.integers(0, n))
+        if kind == 1:
+            r0 = int(0.4 * n) - 1                   # the loop comes back by the robot
+        begin[b], end[b] = int(rng.integers(0, r0 + 1)), n
+        off = rng.choice([0.0, 0.01, 0.1, 0.5]) * rng.uniform(-1, 1, 2)
+        robot[b] = (xy[r0, 0] + off[0], xy[r0, 1] + off[1], yaw[r0] + rng.uniform(-0.3, 0.3))
+        vel[b] = (0.0, 0.0, 0.0) if rng.random() < 0.3 else (rng.uniform(-0.2, 0.5), rng.uniform(-0.1, 0.1), rng.uniform(-0.5, 0.5))
+    return dict(global_plan=gp, plan_begin=begin, plan_end=end, robot=robot, robot_vel=vel, scene_id=sid, grid=grid,
+                origin=origin)
