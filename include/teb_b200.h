@@ -429,9 +429,112 @@ typedef struct TebLocalPlanArgs {
 #define TEB_LOCAL_PLAN_CAPACITY     3  /* more rows than P_cap or via-points than V_cap: plan_count = 0, see needed */
 #define TEB_LOCAL_PLAN_BAD_INPUT    4  /* device entry point only: plan_begin / plan_end / scene_id out of range */
 
+/* The controller state of every robot between cycles, and the two steps of TebLocalPlannerROS::computeVelocityCommands
+ * around plan() that read and write it: tebgpu_backup_modes, the oscillation half of configureBackupModes
+ * (teb_local_planner_ros.cpp:980-1016, with FailureDetector of recovery_behaviors.cpp), after tebgpu_local_plan and
+ * before tebgpu_plan_batch; and tebgpu_finish_cycle, the back half of the cycle (:360-454 with saturateVelocity :874-919
+ * and convertTransRotVelToSteeringAngle :922-933), after the plan and the feasibility check. HOST pointers for the
+ * synchronous entry points, DEVICE pointers for the _device ones. The velocity limits (max_vel_x, max_vel_x_backwards,
+ * max_vel_y, max_vel_trans, max_vel_theta), min_turning_radius and the divergence settings are the context's
+ * parameters (tebgpu_set_params). Of the batch, B is read by both steps and n, status and chi2 by tebgpu_finish_cycle.
+ * `now` stands for every ros::Time::now() of the step; the stamps last_infeasible / last_oscillation are in its clock,
+ * -inf meaning never, and the caller forms the next local plan's since_infeasible = now - last_infeasible. Every
+ * product and sum is rounded on its own (no FMA contraction); min(a, b) = b < a ? b : a, max(a, b) = a < b ? b : a;
+ * sign(x) = x > 0 ? 1 : x < 0 ? -1 : 0 (g2o::sign, 0 for 0 and NaN); a NaN fails every comparison.
+ *
+ * tebgpu_backup_modes, per band b whose local_plan_result is PLANNED or CAPACITY (the results with which the reference
+ * reaches configureBackupModes; GOAL_REACHED and EMPTY return before it, :296-304, :713-717; the other bands are not
+ * touched), when oscillation_recovery != 0 (else oscillating[b] = 0 and nothing else is written):
+ *   1. The recovery's max_vel_theta: mvc = last_cmd[b].vx >= 0 ? max_vel_x : max_vel_x_backwards; if
+ *      min_turning_radius != 0 && mvc > 0 it is max(mvc / |min_turning_radius|, max_vel_theta), else max_vel_theta.
+ *   2. FailureDetector::update(last_cmd[b]), skipped when buffer_length == 0 (the detector is off, oscillating 0):
+ *      v = last_cmd vx divided by max_vel_x when v > 0 && max_vel_x > 0, else by max_vel_x_backwards when v < 0 && that
+ *      limit is > 0; omega = last_cmd omega divided by step 1's value when it is > 0. (v, omega) is pushed into the
+ *      band's ring of capacity buffer_length; a push into a full ring drops the oldest entry. The ring's k-th oldest
+ *      entry is osc_ring[(head + k) % buffer_length][b], (size, head) = osc_fill[b].
+ *   3. detect: oscillating when size >= buffer_length / 2 (integer division), |v_mean| < oscillation_v_eps,
+ *      |omega_mean| < oscillation_omega_eps and crossings > 1 (all strict), the means summed from 0 over the entries
+ *      from the oldest, in order, then divided by size; crossings counts the entries k >= 1 with sign(omega_k) !=
+ *      sign(omega_{k-1}).
+ *   4. recently = now - last_oscillation[b] < oscillation_recovery_min_duration. Oscillating: if not recently,
+ *      prefer_rotdir[b] = robot_vel[b].omega > 0 ? TEB_ROTDIR_LEFT : TEB_ROTDIR_RIGHT (0 and NaN give RIGHT); then
+ *      last_oscillation[b] = now. Not oscillating, not recently and prefer_rotdir[b] != NONE: prefer_rotdir[b] = NONE.
+ *   oscillating[b] = isOscillating() after the update. Pass prefer_rotdir as TebBatch.prefer_rotdir of the plan.
+ *
+ * tebgpu_finish_cycle, per band b, with r = local_plan_result[b]; outcome[b] is the first that applies. "Failure"
+ * means: cmd_vel[b] = 0, n[b] = 0 (clearPlanner), infeasible_count[b] += 1 (it stops at INT32_MAX), last_infeasible[b]
+ * = now, last_cmd[b] = 0.
+ *   TEB_CYCLE_GOAL_REACHED     r == GOAL_REACHED (:290-304): cmd_vel 0, n = 0 (isGoalReached's clearPlanner); the
+ *                              counters and last_cmd are not touched.
+ *   TEB_CYCLE_NO_PLAN          r == EMPTY, CAPACITY or BAD_INPUT: cmd_vel 0, nothing else is written.
+ *   TEB_CYCLE_PLAN_FAILED      !(status & OPTIMIZED) || status & (CAPACITY | BAD_INPUT) (:361-371): failure.
+ *   TEB_CYCLE_DIVERGED         divergence_detection_enable && chi2 > divergence_detection_max_chi_squared (:374-386,
+ *                              hasDiverged): failure.
+ *   TEB_CYCLE_INFEASIBLE       feasible[b] == 0 (:396-410): failure.
+ *   TEB_CYCLE_UNDECIDABLE      feasible[b] == -1: failure (the safe, infeasible case).
+ *   TEB_CYCLE_INVALID_COMMAND  cmd[b][3] == 0, getVelocityCommand returned false (:413-423): failure.
+ *   TEB_CYCLE_STEERING_NOT_FINITE  cmd_angle_instead_rotvel and a non-finite steering angle (:433-448): failure.
+ *   TEB_CYCLE_COMMAND          otherwise (:425-454): cmd_vel = the saturated (vx, vy, omega) of cmd[b], omega replaced by
+ *                              the steering angle when cmd_angle_instead_rotvel; infeasible_count = 0; last_cmd = cmd_vel
+ *                              (with the steering angle, as in the reference).
+ * saturateVelocity(vx, vy, omega): ratios rx = ry = ro = 1; vx > max_vel_x: rx = max_vel_x / vx; vy > max_vel_y ||
+ *   vy < -max_vel_y: ry = |max_vel_y / vy| (so max_vel_y = 0 zeroes vy, and with proportional saturation the whole
+ *   twist); omega > max_vel_theta || omega < -max_vel_theta: ro = |max_vel_theta / omega|; when max_vel_x_backwards > 0
+ *   and vx < -max_vel_x_backwards, rx = -max_vel_x_backwards / vx. use_proportional_saturation: each component times
+ *   min(min(rx, ry), ro); otherwise vx * rx, vy * ry, omega * ro. Then with l = hypot(vx, vy), l > max_vel_trans: vx
+ *   and vy times max_vel_trans / l. max_vel_trans = 0 is used as it is and zeroes vx and vy: the node never sees 0,
+ *   because its reconfigure replaces it with max_vel_x (teb_config.cpp:219-224); abi.make_cycle_args does the same.
+ * Steering angle of (v, omega) = (vx, omega) after saturation: 0 when omega == 0 || v == 0; else radius = v / omega,
+ *   replaced by sign(radius) * m when |radius| < m, m = 0.95 * min_turning_radius (one rounded product); atan(wheelbase
+ *   / radius).
+ *
+ * Argument errors return TEBGPU_ERR_INVALID_ARG before anything is launched: NULL batch or required array, B outside
+ * 1 .. max_bands, L_cap < 0, buffer_length outside 0 .. L_cap, a non-finite now. The host entry points also refuse a
+ * band with local_plan_result outside 0 .. 4, prefer_rotdir outside 0 .. 2, feasible outside -1 .. 1 or osc_fill
+ * outside 0 .. buffer_length (head 0 when buffer_length is 0), whichever the step reads. The device entry points answer
+ * such a band with outcome TEB_CYCLE_NO_PLAN (cmd_vel 0, nothing else written) or oscillating = -1 (its state not
+ * touched). */
+typedef struct TebCycleArgs {
+  int32_t  use_proportional_saturation; /* robot.use_proportional_saturation (teb_config.h:289, default false) */
+  int32_t  cmd_angle_instead_rotvel;    /* robot.cmd_angle_instead_rotvel (:287, default false) */
+  int32_t  oscillation_recovery;        /* recovery.oscillation_recovery (:383, default true) */
+  int32_t  buffer_length;  /* the detector's capacity: round(oscillation_filter_duration * controller_frequency), the
+                              node's setBufferLength (teb_local_planner_ros.cpp:188); 0: the detector is off */
+  int32_t  L_cap;          /* ring entries per band (stride of osc_ring), >= buffer_length */
+  int32_t  _pad;
+  double   wheelbase;                   /* robot.wheelbase (:286, default 1; may be negative) */
+  double   oscillation_v_eps;           /* recovery (:384, default 0.1) */
+  double   oscillation_omega_eps;       /* (:385, default 0.1) */
+  double   oscillation_recovery_min_duration; /* (:386, default 10) */
+  double   now;                         /* the cycle's ros::Time::now() in seconds, finite */
+  const int32_t* local_plan_result; /* [B] TEB_LOCAL_PLAN_* of tebgpu_local_plan, or NULL: every band PLANNED */
+  const double*  robot_vel;         /* [B][3] odometry vx, vy, omega (robot_vel_); backup modes */
+  const double*  cmd;               /* [B][4] TebPlanInput.cmd: vx, vy, omega, ok; finish */
+  const int32_t* feasible;          /* [B] tebgpu_check_feasible's answer, or NULL: not checked, every band feasible */
+  int32_t*       infeasible_count;  /* [B] in/out: no_infeasible_plans_ (tebgpu_local_plan reads it) */
+  double*        last_infeasible;   /* [B] in/out: time_last_infeasible_plan_, -inf: never */
+  double*        last_oscillation;  /* [B] in/out: time_last_oscillation_, -inf: never */
+  double*        last_cmd;          /* [B][3] in/out: last_cmd_ vx, vy, omega */
+  int32_t*       prefer_rotdir;     /* [B] in/out: last_preferred_rotdir_, TEB_ROTDIR_* (TebBatch.prefer_rotdir) */
+  double*        osc_ring;          /* [L_cap][B][2] in/out: normalised (v, omega), band-minor; may be NULL when buffer_length == 0 */
+  int32_t*       osc_fill;          /* [B][2] in/out: the ring's size and head (slot of its oldest entry) */
+  double*        cmd_vel;           /* [B][3] out: the twist published (finish) */
+  int32_t*       outcome;           /* [B] out: TEB_CYCLE_* (finish) */
+  int32_t*       oscillating;       /* [B] out or NULL: 1 / 0, -1 for out-of-range ring state (backup modes) */
+} TebCycleArgs;
+#define TEB_CYCLE_COMMAND              0
+#define TEB_CYCLE_GOAL_REACHED         1
+#define TEB_CYCLE_NO_PLAN              2
+#define TEB_CYCLE_PLAN_FAILED          3
+#define TEB_CYCLE_DIVERGED             4
+#define TEB_CYCLE_INFEASIBLE           5
+#define TEB_CYCLE_UNDECIDABLE          6
+#define TEB_CYCLE_INVALID_COMMAND      7
+#define TEB_CYCLE_STEERING_NOT_FINITE  8
+
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
- * 9 TebLocalPlanArgs. */
+ * 9 TebLocalPlanArgs, 10 TebCycleArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -545,6 +648,17 @@ int32_t tebgpu_costmap_obstacles_device(tebgpu_ctx* ctx, const TebCostmapArgs* a
 int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args);
 int32_t tebgpu_local_plan_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args, void* cuda_stream);
 
+/* The two controller steps around plan(), as defined at TebCycleArgs. One thread per band, so that the detector's sums
+ * run in the reference's order (tebgpu_get_info key 17). A fleet cycle on one stream: tebgpu_costmap_obstacles_device,
+ * tebgpu_local_plan_device, tebgpu_backup_modes_device, tebgpu_plan_batch_device, tebgpu_check_feasible_device,
+ * tebgpu_finish_cycle_device. tebgpu_backup_modes / tebgpu_finish_cycle: HOST buffers, synchronous; their device copies
+ * are allocated by the first call that needs them. The _device forms: DEVICE buffers, stream ordered as
+ * tebgpu_optimize_batch_device, do not synchronise. */
+int32_t tebgpu_backup_modes(tebgpu_ctx* ctx, const TebBatch* batch, const TebCycleArgs* args);
+int32_t tebgpu_backup_modes_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebCycleArgs* args, void* cuda_stream);
+int32_t tebgpu_finish_cycle(tebgpu_ctx* ctx, TebBatch* batch, const TebCycleArgs* args);
+int32_t tebgpu_finish_cycle_device(tebgpu_ctx* ctx, TebBatch* batch, const TebCycleArgs* args, void* cuda_stream);
+
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded
  *   LDL^T with the active window in registers, and the accept / reject chain is replayed in order;
@@ -621,7 +735,9 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * the last feasibility-check launch (0 before the first), 13 which build that launch ran (TEBGPU_FEAS_BUILD_*, -1 before
  * the first), 14 grid in CTAs of the last trajectory read-out launch (k_read_trajectory, 4 rows per CTA; 0 before the
  * first), 15 grid in CTAs of the last costmap conversion (k_costmap_obstacles, one CTA per scene; 0 before the first),
- * 16 grid in CTAs of the last local-plan launch (k_local_plan, 4 bands per CTA; 0 before the first).
+ * 16 grid in CTAs of the last local-plan launch (k_local_plan, 4 bands per CTA; 0 before the first), 17 grid in CTAs
+ * of the last backup-modes or finish-cycle launch (k_backup_modes / k_finish_cycle, 128 bands per CTA; 0 before the
+ * first).
  * Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */

@@ -66,6 +66,11 @@ def load_library(build_if_missing=False):
     L.tebgpu_local_plan.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs)]
     L.tebgpu_local_plan_device.restype = C.c_int32
     L.tebgpu_local_plan_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs), vp]
+    for name in ("tebgpu_backup_modes", "tebgpu_finish_cycle"):
+        getattr(L, name).restype = C.c_int32
+        getattr(L, name).argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebCycleArgs)]
+        getattr(L, name + "_device").restype = C.c_int32
+        getattr(L, name + "_device").argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebCycleArgs), vp]
     L.tebgpu_get_plan_kernel_times.restype = C.c_int32
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
@@ -124,7 +129,7 @@ def load_library(build_if_missing=False):
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
     for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
                                 abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs,
-                                abi.TebLocalPlanArgs)):
+                                abi.TebLocalPlanArgs, abi.TebCycleArgs)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -364,6 +369,77 @@ class TebGpu:
     def last_local_plan_grid(self):
         """grid in CTAs (4 bands each) of the last local-plan launch, 0 before the first"""
         return self.info(16)
+
+    def _cycle_host(self, fn, state, B, now, local_plan_result, scalars, bs, **arrays):
+        """shared body of backup_modes / finish_cycle: copies the state, fills TebCycleArgs, calls `fn`"""
+        import numpy as np
+        i32 = lambda x, shape: None if x is None else np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.int32)
+        out = {k: np.array(v, dtype=np.int32 if k in abi.CYCLE_STATE_INT else np.float64, order="C")
+               for k, v in state.items()}
+        L_cap = out["osc_ring"].shape[0]
+        scalars.setdefault("buffer_length", L_cap)
+        ca = abi.make_cycle_args(now, L_cap=L_cap, **scalars)
+        keep = dict(lpr=i32(local_plan_result, (B,)))
+        ca.local_plan_result = abi.ptr(keep["lpr"])
+        for k in abi.CYCLE_STATE:
+            setattr(ca, k, abi.ptr(out[k]) if out[k].size else None)
+        for k, v in arrays.items():
+            keep[k] = v
+            setattr(ca, k, abi.ptr(v))
+        self._check(fn(self.ctx, C.byref(bs), C.byref(ca)), fn.__name__)
+        return out
+
+    def backup_modes(self, state, robot_vel, now, local_plan_result=None, **scalars):
+        """The oscillation half of configureBackupModes for every robot (tebgpu_backup_modes), host buffers. state: a
+        dict as abi.make_cycle_state makes it (its osc_ring's first axis is L_cap); robot_vel [B][3] (vx, vy, omega);
+        local_plan_result [B] TEB_LOCAL_PLAN_* or None (all PLANNED); scalars: abi.make_cycle_args' keywords
+        (buffer_length defaults to L_cap). Returns a new state dict plus oscillating [B] (1 / 0, -2 where not written)."""
+        import numpy as np
+        B = len(state["prefer_rotdir"])
+        osc = np.full(B, -2, np.int32)
+        rv = np.ascontiguousarray(np.broadcast_to(robot_vel, (B, 3)), dtype=np.float64)
+        bs = abi.TebBatch()
+        bs.B = B
+        out = self._cycle_host(self.lib.tebgpu_backup_modes, state, B, now, local_plan_result, scalars, bs,
+                               robot_vel=rv, oscillating=osc)
+        out["oscillating"] = osc
+        return out
+
+    def finish_cycle(self, state, n, status, chi2, cmd, now, feasible=None, local_plan_result=None, **scalars):
+        """computeVelocityCommands from plan() on for every robot (tebgpu_finish_cycle), host buffers: n, status, chi2
+        [B] of the planned batch, cmd [B][4] (TebPlanInput.cmd), feasible [B] or None (not checked), local_plan_result
+        [B] or None (all PLANNED); state and scalars as for backup_modes. Returns a new state dict plus n [B] (0 where
+        the planner was cleared), cmd_vel [B][3] and outcome [B] (TEB_CYCLE_*)."""
+        import numpy as np
+        B = len(state["prefer_rotdir"])
+        i32 = lambda x: np.ascontiguousarray(np.broadcast_to(x, (B,)), dtype=np.int32).copy()
+        res = dict(n=i32(n), cmd_vel=np.zeros((B, 3)), outcome=np.full(B, -1, np.int32))
+        st, c2 = i32(status), np.ascontiguousarray(np.broadcast_to(chi2, (B,)), dtype=np.float64)
+        cm = np.ascontiguousarray(np.broadcast_to(cmd, (B, 4)), dtype=np.float64)
+        fz = None if feasible is None else i32(feasible)
+        bs = abi.TebBatch()
+        bs.B, bs.n, bs.status, bs.chi2 = B, abi.ptr(res["n"]), abi.ptr(st), abi.ptr(c2)
+        out = self._cycle_host(self.lib.tebgpu_finish_cycle, state, B, now, local_plan_result, scalars, bs, cmd=cm,
+                               feasible=fz, cmd_vel=res["cmd_vel"], outcome=res["outcome"])
+        out.update(res)
+        return out
+
+    def backup_modes_device(self, batch_struct, args, stream=None):
+        """tebgpu_backup_modes_device: the same step over DEVICE memory (batch_struct: an abi.TebBatch whose B is read;
+        args: an abi.TebCycleArgs of device pointers, see abi.make_cycle_args). Stream ordered on `stream` (a
+        cudaStream_t handle; None: the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_backup_modes_device(self.ctx, C.byref(batch_struct), C.byref(args), stream),
+                    "tebgpu_backup_modes_device")
+
+    def finish_cycle_device(self, batch_struct, args, stream=None):
+        """tebgpu_finish_cycle_device: the same step over DEVICE memory (batch_struct: an abi.TebBatch whose B, n, status
+        and chi2 are read; n is written). Stream ordered as backup_modes_device; does not synchronise."""
+        self._check(self.lib.tebgpu_finish_cycle_device(self.ctx, C.byref(batch_struct), C.byref(args), stream),
+                    "tebgpu_finish_cycle_device")
+
+    def last_cycle_grid(self):
+        """grid in CTAs (128 bands each) of the last backup-modes or finish-cycle launch, 0 before the first"""
+        return self.info(17)
 
     FEAS_BUILDS = {0: "staged", 1: "global"}   # TEBGPU_FEAS_BUILD_*
 

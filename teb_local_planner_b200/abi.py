@@ -198,6 +198,67 @@ def make_local_plan_args(G_cap, P_cap, V_cap=0, prune_distance=1.0, max_lookahea
     return a
 
 
+class TebCycleArgs(C.Structure):
+    """The controller steps around plan() (tebgpu_backup_modes / tebgpu_finish_cycle): their scalars, the per-band
+    inputs, the controller state carried between cycles and the outputs, as host or device pointers"""
+    _fields_ = [("use_proportional_saturation", _i), ("cmd_angle_instead_rotvel", _i), ("oscillation_recovery", _i),
+                ("buffer_length", _i), ("L_cap", _i), ("_pad", _i), ("wheelbase", _d), ("oscillation_v_eps", _d),
+                ("oscillation_omega_eps", _d), ("oscillation_recovery_min_duration", _d), ("now", _d),
+                ("local_plan_result", C.c_void_p), ("robot_vel", C.c_void_p), ("cmd", C.c_void_p),
+                ("feasible", C.c_void_p), ("infeasible_count", C.c_void_p), ("last_infeasible", C.c_void_p),
+                ("last_oscillation", C.c_void_p), ("last_cmd", C.c_void_p), ("prefer_rotdir", C.c_void_p),
+                ("osc_ring", C.c_void_p), ("osc_fill", C.c_void_p), ("cmd_vel", C.c_void_p), ("outcome", C.c_void_p),
+                ("oscillating", C.c_void_p)]
+
+
+# TEB_CYCLE_*: what tebgpu_finish_cycle did with a band
+TEB_CYCLE_COMMAND, TEB_CYCLE_GOAL_REACHED, TEB_CYCLE_NO_PLAN, TEB_CYCLE_PLAN_FAILED, TEB_CYCLE_DIVERGED, \
+    TEB_CYCLE_INFEASIBLE, TEB_CYCLE_UNDECIDABLE, TEB_CYCLE_INVALID_COMMAND, TEB_CYCLE_STEERING_NOT_FINITE = range(9)
+
+
+def make_cycle_args(now, buffer_length=50, L_cap=None, use_proportional_saturation=False,
+                    cmd_angle_instead_rotvel=False, wheelbase=1.0, oscillation_recovery=True, oscillation_v_eps=0.1,
+                    oscillation_omega_eps=0.1, oscillation_recovery_min_duration=10.0, params=None,
+                    **arrays) -> TebCycleArgs:
+    """TebCycleArgs with the scalars set and the arrays given by keyword as addresses (ints, or None for NULL). The
+    defaults are the reference's (teb_config.h:286-289, :383-386); buffer_length 50 is the node's
+    round(oscillation_filter_duration * controller_frequency) = round(10 * 5) (teb_local_planner_ros.cpp:188); L_cap
+    None: buffer_length. params: a TebParams whose max_vel_trans 0 is replaced by max_vel_x here, as the node's
+    reconfigure does (teb_config.cpp:219-224); pass it to set_params afterwards."""
+    if params is not None and params.max_vel_trans == 0.0:
+        params.max_vel_trans = params.max_vel_x
+    a = TebCycleArgs()
+    a.buffer_length = int(buffer_length)
+    a.L_cap = int(buffer_length if L_cap is None else L_cap)
+    a.use_proportional_saturation = int(bool(use_proportional_saturation))
+    a.cmd_angle_instead_rotvel = int(bool(cmd_angle_instead_rotvel))
+    a.oscillation_recovery = int(bool(oscillation_recovery))
+    a.wheelbase, a.now = float(wheelbase), float(now)
+    a.oscillation_v_eps, a.oscillation_omega_eps = float(oscillation_v_eps), float(oscillation_omega_eps)
+    a.oscillation_recovery_min_duration = float(oscillation_recovery_min_duration)
+    names = {f[0] for f in TebCycleArgs._fields_[11:]}
+    for k, v in arrays.items():
+        if k not in names:
+            raise TypeError(f"unknown TebCycleArgs array {k}")
+        setattr(a, k, v)
+    return a
+
+
+# the controller state a robot carries between cycles (TebCycleArgs' in/out arrays), and which of it is int32
+CYCLE_STATE = ("infeasible_count", "last_infeasible", "last_oscillation", "last_cmd", "prefer_rotdir", "osc_ring",
+               "osc_fill")
+CYCLE_STATE_INT = ("infeasible_count", "prefer_rotdir", "osc_fill")
+
+
+def make_cycle_state(B, L_cap=50):
+    """The state of B robots that have not run a cycle yet (the node's constructor): no infeasible plan, never
+    infeasible or oscillating (-inf), last_cmd 0, no preferred turning direction, empty detector rings [L_cap][B][2]"""
+    return dict(infeasible_count=np.zeros(B, np.int32), last_infeasible=np.full(B, -np.inf),
+                last_oscillation=np.full(B, -np.inf), last_cmd=np.zeros((B, 3)),
+                prefer_rotdir=np.full(B, TEB_ROTDIR_NONE, np.int32), osc_ring=np.zeros((int(L_cap), B, 2)),
+                osc_fill=np.zeros((B, 2), np.int32))
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

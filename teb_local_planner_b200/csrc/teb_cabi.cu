@@ -22,6 +22,7 @@
 #include "teb_feasible.cuh"
 #include "teb_costmap.cuh"
 #include "teb_local_plan.cuh"
+#include "teb_cycle.cuh"
 #include "teb_comm.h"
 #include <cstdlib>
 
@@ -130,6 +131,9 @@ struct tebgpu_ctx {
    * needs more */
   char* d_lplan = nullptr; size_t lplan_bytes = 0;
   long long last_lplan_grid = 0;      /* grid in CTAs of the last k_local_plan launch */
+  /* backup modes / finish cycle: the host-buffer entry points' arrays, staged in one buffer grown as above */
+  char* d_cycle = nullptr; size_t cycle_bytes = 0;
+  long long last_cycle_grid = 0;      /* grid in CTAs of the last k_backup_modes / k_finish_cycle launch */
   size_t smem_a = 0, smem_b = 0, smem_g = 0;
   /* profiling */
   bool profiling = false;
@@ -223,6 +227,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 7: return (int32_t)sizeof(TebTrajectoryArgs);
     case 8: return (int32_t)sizeof(TebCostmapArgs);
     case 9: return (int32_t)sizeof(TebLocalPlanArgs);
+    case 10: return (int32_t)sizeof(TebCycleArgs);
     default: return -1;
   }
 }
@@ -249,6 +254,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 14: return ctx->last_traj_grid;
     case 15: return ctx->last_costmap_grid;
     case 16: return ctx->last_lplan_grid;
+    case 17: return ctx->last_cycle_grid;
     default: return -1;
   }
 }
@@ -259,7 +265,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
-                  c->d_cneeded, c->d_lplan};
+                  c->d_cneeded, c->d_lplan, c->d_cycle};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1744,6 +1750,140 @@ int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPla
         std::memcpy(la->via + b * V * 2, h.data() + b * V * 2, (size_t)std::max(la->via_count[b], 0) * 2 * sizeof(double));
   }
   return TEBGPU_OK;
+}
+
+/* the context parameters the controller steps read */
+static TebCycleLimits cycle_limits(const TebParams& p) {
+  TebCycleLimits L;
+  L.max_vel_x = p.max_vel_x; L.max_vel_x_backwards = p.max_vel_x_backwards; L.max_vel_y = p.max_vel_y;
+  L.max_vel_trans = p.max_vel_trans; L.max_vel_theta = p.max_vel_theta; L.min_turning_radius = p.min_turning_radius;
+  L.divergence_max_chi2 = p.divergence_detection_max_chi_squared;
+  L.divergence_enable = p.divergence_detection_enable;
+  return L;
+}
+
+/* argument checks of the four controller-step entry points: nothing is launched when one fails */
+static int32_t check_cycle_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebCycleArgs* ca, bool finish) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!bt || !ca) { ctx->err = "batch or cycle args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->B < 1 || bt->B > ctx->lim.max_bands) { ctx->err = "B outside 1 .. max_bands"; return TEBGPU_ERR_INVALID_ARG; }
+  if (ca->L_cap < 0 || ca->buffer_length < 0 || ca->buffer_length > ca->L_cap) {
+    ctx->err = "buffer_length outside 0 .. L_cap"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  if (!std::isfinite(ca->now)) { ctx->err = "now is not finite"; return TEBGPU_ERR_INVALID_ARG; }
+  const bool missing = finish ? (!bt->n || !bt->status || !bt->chi2 || !ca->cmd || !ca->infeasible_count ||
+                                 !ca->last_infeasible || !ca->last_cmd || !ca->cmd_vel || !ca->outcome)
+                              : (!ca->robot_vel || !ca->last_cmd || !ca->prefer_rotdir || !ca->last_oscillation ||
+                                 !ca->osc_fill || (ca->buffer_length > 0 && !ca->osc_ring));
+  if (missing) { ctx->err = "missing required cycle array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!ctx->have_params) { ctx->err = "tebgpu_set_params has not been called"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+static int32_t issue_cycle(tebgpu_ctx* ctx, TebBatch* bt, const TebCycleArgs* ca, bool finish, cudaStream_t st) {
+  const long long grid = ((long long)bt->B + CYCLE_THREADS - 1) / CYCLE_THREADS;
+  const TebCycleLimits L = cycle_limits(ctx->params);
+  if (finish)
+    k_finish_cycle<<<(unsigned)grid, CYCLE_THREADS, 0, st>>>(*ca, L, bt->n, bt->status, bt->chi2, bt->B);
+  else
+    k_backup_modes<<<(unsigned)grid, CYCLE_THREADS, 0, st>>>(*ca, L, bt->B);
+  ctx->last_cycle_grid = grid;
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_backup_modes_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebCycleArgs* ca, void* cuda_stream) {
+  const int32_t rc = check_cycle_args(ctx, bt, ca, false);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  TebBatch b = *bt;
+  return issue_cycle(ctx, &b, ca, false, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_finish_cycle_device(tebgpu_ctx* ctx, TebBatch* bt, const TebCycleArgs* ca, void* cuda_stream) {
+  const int32_t rc = check_cycle_args(ctx, bt, ca, true);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_cycle(ctx, bt, ca, true, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+/* one array of a host-buffer controller step: staged in ctx->d_cycle at a 256-byte aligned offset, copied up before the
+ * launch (so what a band leaves unwritten comes back as the caller left it) and back after it when the step writes it */
+struct CycleSlot {
+  void* host;
+  size_t bytes;
+  bool out;
+  size_t off;
+  char* dev(char* d) const { return host ? d + off : nullptr; }
+};
+
+/* both host-buffer controller steps: refuse the bands the device would answer with NO_PLAN / -1, stage, launch, copy back */
+static int32_t run_cycle_host(tebgpu_ctx* ctx, TebBatch* bt, const TebCycleArgs* ca, bool finish) {
+  int32_t rc = check_cycle_args(ctx, bt, ca, finish);
+  if (rc) return rc;
+  const size_t B = bt->B;
+  for (size_t b = 0; b < B; ++b)
+    if (finish ? !teb_cycle_finish_valid(*ca, (int)b) : !teb_cycle_backup_valid(*ca, (int)b)) {
+      ctx->err = finish ? "local_plan_result or feasible out of range"
+                        : "local_plan_result, prefer_rotdir or osc_fill out of range";
+      return TEBGPU_ERR_INVALID_ARG;
+    }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t I = sizeof(int32_t), D = sizeof(double);
+  enum { LPR, VEL, CMD, FEAS, NCOUNT, STATUS, CHI2, INF, LINF, LOSC, LCMD, ROT, RING, FILL, CVEL, OUTC, OSC, SLOTS };
+  CycleSlot s[SLOTS] = {
+      {(void*)ca->local_plan_result, B * I, false, 0}, {(void*)ca->robot_vel, B * 3 * D, false, 0},
+      {(void*)ca->cmd, B * 4 * D, false, 0},           {(void*)ca->feasible, B * I, false, 0},
+      {bt->n, B * I, true, 0},                         {bt->status, B * I, false, 0},
+      {bt->chi2, B * D, false, 0},                     {ca->infeasible_count, B * I, true, 0},
+      {ca->last_infeasible, B * D, true, 0},           {ca->last_oscillation, B * D, true, 0},
+      {ca->last_cmd, B * 3 * D, true, 0},              {ca->prefer_rotdir, B * I, true, 0},
+      {ca->osc_ring, (size_t)ca->L_cap * B * 2 * D, true, 0}, {ca->osc_fill, B * 2 * I, true, 0},
+      {ca->cmd_vel, B * 3 * D, true, 0},               {ca->outcome, B * I, true, 0},
+      {ca->oscillating, B * I, true, 0}};
+  /* what the step does not read stays on the host */
+  const int used_finish[] = {LPR, CMD, FEAS, NCOUNT, STATUS, CHI2, INF, LINF, LCMD, CVEL, OUTC};
+  const int used_backup[] = {LPR, VEL, LCMD, ROT, RING, FILL, LOSC, OSC};
+  bool used[SLOTS] = {};
+  if (finish) for (int k : used_finish) used[k] = true;
+  else for (int k : used_backup) used[k] = true;
+  if (!finish) s[LCMD].out = false;
+  size_t off = 0;
+  for (int k = 0; k < SLOTS; ++k) {
+    if (!used[k]) s[k].host = nullptr;
+    s[k].off = off;
+    if (s[k].host) off += (s[k].bytes + 255) & ~(size_t)255;
+  }
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_cycle, &ctx->cycle_bytes, off, st))) return rc;
+  char* d = ctx->d_cycle;
+  for (const CycleSlot& c : s)
+    if (c.host && c.bytes) CUDA_TRY(ctx, cudaMemcpyAsync(d + c.off, c.host, c.bytes, cudaMemcpyHostToDevice, st));
+  TebBatch db = *bt;
+  db.n = (int32_t*)s[NCOUNT].dev(d); db.status = (int32_t*)s[STATUS].dev(d); db.chi2 = (double*)s[CHI2].dev(d);
+  TebCycleArgs da = *ca;
+  da.local_plan_result = (const int32_t*)s[LPR].dev(d); da.robot_vel = (const double*)s[VEL].dev(d);
+  da.cmd = (const double*)s[CMD].dev(d); da.feasible = (const int32_t*)s[FEAS].dev(d);
+  da.infeasible_count = (int32_t*)s[INF].dev(d); da.last_infeasible = (double*)s[LINF].dev(d);
+  da.last_oscillation = (double*)s[LOSC].dev(d); da.last_cmd = (double*)s[LCMD].dev(d);
+  da.prefer_rotdir = (int32_t*)s[ROT].dev(d); da.osc_ring = (double*)s[RING].dev(d); da.osc_fill = (int32_t*)s[FILL].dev(d);
+  da.cmd_vel = (double*)s[CVEL].dev(d); da.outcome = (int32_t*)s[OUTC].dev(d); da.oscillating = (int32_t*)s[OSC].dev(d);
+  if ((rc = issue_cycle(ctx, &db, &da, finish, st))) return rc;
+  for (const CycleSlot& c : s)
+    if (c.host && c.out && c.bytes) CUDA_TRY(ctx, cudaMemcpyAsync(c.host, d + c.off, c.bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_backup_modes(tebgpu_ctx* ctx, const TebBatch* bt, const TebCycleArgs* ca) {
+  if (!bt) return check_cycle_args(ctx, bt, ca, false);
+  TebBatch b = *bt;
+  return run_cycle_host(ctx, &b, ca, false);
+}
+
+int32_t tebgpu_finish_cycle(tebgpu_ctx* ctx, TebBatch* bt, const TebCycleArgs* ca) {
+  return run_cycle_host(ctx, bt, ca, true);
 }
 
 int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args) {
