@@ -248,8 +248,9 @@ typedef struct TebPlanInput {
  * batch (tebgpu_check_feasible). HOST output pointers for tebgpu_check_feasible, DEVICE pointers for
  * tebgpu_check_feasible_device.
  *
- * World model, the one difference from the reference. The reference asks base_local_planner::CostmapModel::footprintCost
- * of the costmap; here footprintCost(x, y, theta) == -1 means: the context's footprint model (TebParams.footprint_type and
+ * World model of tebgpu_check_feasible, which differs from the reference. The reference asks
+ * base_local_planner::CostmapModel::footprintCost of the costmap, which tebgpu_check_feasible_costmap does (see
+ * TebCostmapWorld, with the same arguments and outputs); here footprintCost(x, y, theta) == -1 means: the context's footprint model (TebParams.footprint_type and
  * its geometry) placed at (x, y, theta) has a distance <= collision_distance to some obstacle of the band's scene. The
  * distance is the optimizer's own footprint-to-obstacle distance (the one the obstacle edges use); all obst_count rows of
  * the scene are tested, not the association; dynamic obstacles at their current position (a snapshot, no time
@@ -267,6 +268,55 @@ typedef struct TebFeasibilityArgs {
   int32_t* query_count;         /* [B] out: footprint queries the reference makes */
   double*  queries;             /* [B][max_queries][3] out or NULL: the first min(query_count, max_queries) query poses */
 } TebFeasibilityArgs;
+
+/* The costmap world model of tebgpu_check_feasible_costmap(_device): the reference's own check,
+ * base_local_planner::CostmapModel::footprintCost on each scene's local costmap. base_local_planner and costmap_2d are
+ * not part of the reference checkout; this definition restates navigation's ROS Noetic code (costmap_model.cpp,
+ * line_iterator.h, world_model.h, Costmap2D::worldToMap). HOST pointers for tebgpu_check_feasible_costmap, DEVICE pointers
+ * for tebgpu_check_feasible_costmap_device, except footprint, which is always a host array copied into the launch.
+ *
+ * Scene s's raster is TebCostmapArgs' layout: cost[s][my * sx + mx], (sx, sy) = grid[s], (ox, oy, r) = origin[s]; band b
+ * reads scene scene_id[b], so the rasters uploaded for tebgpu_costmap_obstacles_device feed this check unchanged. The
+ * queries, their order, the look-ahead rule and max_queries are tebgpu_check_feasible's (TebFeasibilityArgs; its
+ * collision_distance is not read). footprintCost(x, y, theta) with F = footprint_count points (robot frame):
+ *   vertices  c = cos theta, s = sin theta once per query; vertex k = (x + (fx c - fy s), y + (fx s + fy c)), every
+ *             product and sum rounded on its own (no FMA contraction).
+ *   worldToMap(wx, wy)  off the map when wx < ox or wy < oy; otherwise mx = (int)((wx - ox) / r), my likewise
+ *             (truncation), on the map when mx < sx and my < sy. A quotient past the int range is off the map.
+ *   1. the centre (x, y) off the map: -3.
+ *   2. F < 3: the centre cell alone: 255 (NO_INFORMATION) -2, 254 (LETHAL) or 253 (INSCRIBED_INFLATED) -1, otherwise
+ *      its cost.
+ *   3. F >= 3: the outline only, never the interior. Edges 0 -> 1, ..., F - 2 -> F - 1, then F - 1 -> 0: an endpoint
+ *      off the map gives -3; otherwise the cells of the integer Bresenham walk (LineIterator) from the start vertex's
+ *      cell to the end vertex's, both included, in walk order: 255 -2, 254 -1, otherwise the cost (253 is not
+ *      negative here). The first negative value met is returned at once.
+ *   4. otherwise the largest cost seen (0 for none).
+ * LineIterator: dx = |x1 - x0|, dy = |y1 - y0|, the increments by sign (x1 >= x0 gives +1). x is the major axis when
+ * dx >= dy: den = dx, num = dx / 2 (integer), numadd = dy, numpixels = dx (y the same with x and y swapped). advance:
+ * num += numadd; if num >= den { num -= den; step the minor axis }; step the major axis. Cells 0 .. numpixels.
+ * Verdict: the first query whose footprintCost is exactly -1 makes the band infeasible (feasible 0, query_count its
+ * index + 1). -2 and -3 are free, as in the reference, so a -2 met earlier on an outline hides a later 254.
+ *
+ * Defined here where the reference is not: a non-finite pose among the checked ones gives feasible -1 and no query (as
+ * tebgpu_check_feasible); more than max_queries queries, the first max_queries free: -1 and the full count (as there).
+ * The device entry point answers a band with feasible -1 and query_count 0 when its n or scene_id is out of range, or
+ * its scene has sx or sy < 1, sx * sy > cell_cap, a non-finite or non-positive resolution or a non-finite origin; the
+ * host entry point refuses the same inputs with TEBGPU_ERR_INVALID_ARG. A caller who wants -2 / -3 to count as
+ * collisions reads query_cost. */
+#define TEB_COSTMAP_FOOTPRINT_MAX  64
+#define TEB_COSTMAP_INSCRIBED      253   /* costmap_2d::INSCRIBED_INFLATED_OBSTACLE */
+#define TEB_COSTMAP_LETHAL         254   /* costmap_2d::LETHAL_OBSTACLE */
+#define TEB_COSTMAP_NO_INFORMATION 255   /* costmap_2d::NO_INFORMATION */
+typedef struct TebCostmapWorld {
+  int32_t        cell_cap;        /* raster bytes per scene (stride of cost), >= 1 */
+  int32_t        footprint_count; /* F, 0 .. TEB_COSTMAP_FOOTPRINT_MAX */
+  const uint8_t* cost;            /* [S][cell_cap] */
+  const int32_t* grid;            /* [S][2] sx, sy */
+  const double*  origin;          /* [S][3] ox, oy, r */
+  const double*  footprint;       /* [F][2] HOST (both entry points), finite: footprint_spec_ in the robot frame */
+  double*        query_cost;      /* [B][max_queries] out or NULL: footprintCost of each query tested, the rows
+                                     TebFeasibilityArgs.queries gets; the rows behind them are not written */
+} TebCostmapWorld;
 
 /* Which bands tebgpu_read_trajectory reads out, and its outputs: TebOptimalPlanner::getVelocityProfile
  * (optimal_planner.cpp:1170-1188) and getFullTrajectory (:1190-1248) of every band read out. HOST pointers for
@@ -534,7 +584,7 @@ typedef struct TebCycleArgs {
 
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
- * 9 TebLocalPlanArgs, 10 TebCycleArgs. */
+ * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -610,6 +660,22 @@ int32_t tebgpu_plan_batch_device(tebgpu_ctx* ctx, const TebBatch* batch, const T
 int32_t tebgpu_check_feasible(tebgpu_ctx* ctx, const TebBatch* batch, const TebFeasibilityArgs* args);
 int32_t tebgpu_check_feasible_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebFeasibilityArgs* args,
                                      void* cuda_stream);
+
+/* isTrajectoryFeasible for every band of the batch against its scene's costmap, the reference's own check, as defined
+ * at TebCostmapWorld. Same queries and outputs as tebgpu_check_feasible; reads only poses, n and scene_id of the batch
+ * (obstacles, obst_count and obst_vertices are not read) and writes only the outputs in `args` and world->query_cost.
+ * One CTA per band, a warp per query, its lanes over the cells of one outline edge; the raster is read through the
+ * read-only cache (tebgpu_get_info keys 12 / 13: B CTAs, TEBGPU_FEAS_BUILD_COSTMAP). Argument errors (NULL batch arrays,
+ * outputs, world or its arrays, a bad inscribed_radius / angular_resolution / max_queries, cell_cap < 1,
+ * footprint_count outside 0 .. TEB_COSTMAP_FOOTPRINT_MAX, a non-finite footprint coordinate) return
+ * TEBGPU_ERR_INVALID_ARG before anything is launched. tebgpu_check_feasible_costmap: HOST buffers, synchronous; the
+ * bands the device entry point answers with -1 are refused with TEBGPU_ERR_INVALID_ARG too; the device copies are
+ * allocated by the first call that needs them. tebgpu_check_feasible_costmap_device: DEVICE buffers, stream ordered as
+ * tebgpu_optimize_batch_device, does not synchronise. */
+int32_t tebgpu_check_feasible_costmap(tebgpu_ctx* ctx, const TebBatch* batch, const TebFeasibilityArgs* args,
+                                      const TebCostmapWorld* world);
+int32_t tebgpu_check_feasible_costmap_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebFeasibilityArgs* args,
+                                             const TebCostmapWorld* world, void* cuda_stream);
 
 /* getVelocityProfile and getFullTrajectory (optimal_planner.cpp:1170-1248) of the bands listed in `args`, as defined at
  * TebTrajectoryArgs: what a controller publishes as its local plan every cycle. Reads only poses, n, vel_start and
@@ -750,6 +816,7 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
 #define TEBGPU_KA_BUILD_PERSIST 3  /* k_linearize2p (default): resident one-warp CTAs per SM x SMs, at most chunks x B */
 #define TEBGPU_FEAS_BUILD_STAGED 0  /* k_feasible, the scene's table staged in shared memory (M_cap <= 1024): B CTAs */
 #define TEBGPU_FEAS_BUILD_GLOBAL 1  /* k_feasible, the table read from global memory / L2 (M_cap > 1024): B CTAs */
+#define TEBGPU_FEAS_BUILD_COSTMAP 2 /* k_feasible, the costmap world (tebgpu_check_feasible_costmap): B CTAs */
 int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which);
 
 /* Linearise only: build the padded banded normal equations of every band at its current state for

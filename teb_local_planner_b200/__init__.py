@@ -54,6 +54,12 @@ def load_library(build_if_missing=False):
     L.tebgpu_check_feasible.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs)]
     L.tebgpu_check_feasible_device.restype = C.c_int32
     L.tebgpu_check_feasible_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs), vp]
+    L.tebgpu_check_feasible_costmap.restype = C.c_int32
+    L.tebgpu_check_feasible_costmap.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs),
+                                                C.POINTER(abi.TebCostmapWorld)]
+    L.tebgpu_check_feasible_costmap_device.restype = C.c_int32
+    L.tebgpu_check_feasible_costmap_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebFeasibilityArgs),
+                                                       C.POINTER(abi.TebCostmapWorld), vp]
     L.tebgpu_read_trajectory.restype = C.c_int32
     L.tebgpu_read_trajectory.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebTrajectoryArgs)]
     L.tebgpu_read_trajectory_device.restype = C.c_int32
@@ -129,7 +135,7 @@ def load_library(build_if_missing=False):
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
     for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
                                 abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs,
-                                abi.TebLocalPlanArgs, abi.TebCycleArgs)):
+                                abi.TebLocalPlanArgs, abi.TebCycleArgs, abi.TebCostmapWorld)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -244,6 +250,44 @@ class TebGpu:
         Stream ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise."""
         self._check(self.lib.tebgpu_check_feasible_device(self.ctx, C.byref(batch_struct), C.byref(fargs), stream),
                     "tebgpu_check_feasible_device")
+
+    def check_feasible_costmap(self, hb, cost, grid, origin, footprint, inscribed_radius, look_ahead_idx=-1,
+                               lookahead_distance=-1.0, angular_resolution=math.pi, max_queries=1024, queries=False,
+                               query_cost=False):
+        """isTrajectoryFeasible for every band of hb (an abi.HostBatch; its poses, n and scene_id are read) against its
+        scene's costmap, CostmapModel::footprintCost as include/teb_b200.h defines it at TebCostmapWorld
+        (tebgpu_check_feasible_costmap), host buffers: cost [S][cell_cap] uint8, grid [S][2] (sx, sy), origin [S][3]
+        (ox, oy, resolution), footprint [F][2] in the robot frame (F < 3: the centre cell only). Returns (feasible [B]
+        int32: 1 feasible, 0 colliding, -1 undecidable, query_count [B] int32), then with queries=True the query poses
+        [B][max_queries][3] and with query_cost=True each tested query's footprintCost [B][max_queries] (NaN past each
+        band's min(query_count, max_queries) rows)."""
+        import numpy as np
+        cost = np.ascontiguousarray(cost, dtype=np.uint8)
+        S = cost.shape[0]
+        cost = cost.reshape(S, -1)
+        grid = np.ascontiguousarray(grid, dtype=np.int32).reshape(S, 2)
+        origin = np.ascontiguousarray(origin, dtype=np.float64).reshape(S, 3)
+        feas = np.zeros(hb.B, np.int32)
+        cnt = np.zeros(hb.B, np.int32)
+        q = np.full((hb.B, int(max_queries), 3), np.nan) if queries else None
+        qc = np.full((hb.B, int(max_queries)), np.nan) if query_cost else None
+        fa = abi.make_feasibility_args(inscribed_radius, look_ahead_idx, lookahead_distance, angular_resolution, 0.0,
+                                       max_queries, abi.ptr(feas), abi.ptr(cnt), abi.ptr(q))
+        w = abi.make_costmap_world(cost.shape[1], abi.ptr(cost), abi.ptr(grid), abi.ptr(origin), footprint, abi.ptr(qc))
+        bs = hb.struct()
+        self._check(self.lib.tebgpu_check_feasible_costmap(self.ctx, C.byref(bs), C.byref(fa), C.byref(w)),
+                    "tebgpu_check_feasible_costmap")
+        return (feas, cnt) + ((q,) if queries else ()) + ((qc,) if query_cost else ())
+
+    def check_feasible_costmap_device(self, batch_struct, fargs, world, stream=None):
+        """tebgpu_check_feasible_costmap_device: the same check over DEVICE memory (batch_struct: an abi.TebBatch of
+        device pointers, of which poses, n and scene_id are read; fargs: an abi.TebFeasibilityArgs whose outputs are
+        device addresses; world: an abi.TebCostmapWorld of device arrays and a host footprint, see
+        abi.make_costmap_world). Stream ordered on `stream` (a cudaStream_t handle; None: the context's stream); does
+        not synchronise."""
+        self._check(self.lib.tebgpu_check_feasible_costmap_device(self.ctx, C.byref(batch_struct), C.byref(fargs),
+                                                                  C.byref(world), stream),
+                    "tebgpu_check_feasible_costmap_device")
 
     def read_trajectory(self, hb, bands=None, profile=True, trajectory=True):
         """getVelocityProfile / getFullTrajectory of the bands of hb (an abi.HostBatch) listed in `bands` (None: all B, in
@@ -441,7 +485,7 @@ class TebGpu:
         """grid in CTAs (128 bands each) of the last backup-modes or finish-cycle launch, 0 before the first"""
         return self.info(17)
 
-    FEAS_BUILDS = {0: "staged", 1: "global"}   # TEBGPU_FEAS_BUILD_*
+    FEAS_BUILDS = {0: "staged", 1: "global", 2: "costmap"}   # TEBGPU_FEAS_BUILD_*
 
     def last_feasibility_check(self):
         """(build, grid in CTAs) of the last feasibility-check launch: build is one of FEAS_BUILDS' names, or None

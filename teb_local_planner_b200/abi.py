@@ -138,6 +138,30 @@ def make_feasibility_args(inscribed_radius, look_ahead_idx=-1, lookahead_distanc
     return f
 
 
+class TebCostmapWorld(C.Structure):
+    """The costmap world of tebgpu_check_feasible_costmap: each scene's raster (TebCostmapArgs' layout), the footprint
+    (a host array, copied into the launch) and an optional query_cost output (host or device pointer)"""
+    _fields_ = [("cell_cap", _i), ("footprint_count", _i), ("cost", C.c_void_p), ("grid", C.c_void_p),
+                ("origin", C.c_void_p), ("footprint", C.c_void_p), ("query_cost", C.c_void_p)]
+
+
+TEBGPU_FEAS_BUILD_COSTMAP = 2
+TEB_COSTMAP_FOOTPRINT_MAX = 64
+COSTMAP_INSCRIBED, COSTMAP_NO_INFORMATION = 253, 255   # costmap_2d::INSCRIBED_INFLATED_OBSTACLE, NO_INFORMATION
+
+
+def make_costmap_world(cell_cap, cost, grid, origin, footprint=None, query_cost=None):
+    """TebCostmapWorld: cost / grid / origin / query_cost as addresses (ints, or None for NULL), footprint a [F][2]
+    array of the robot-frame points (None or empty: F = 0). The returned struct keeps the footprint array alive."""
+    w = TebCostmapWorld()
+    fp = np.ascontiguousarray(np.zeros((0, 2)) if footprint is None else footprint, dtype=np.float64).reshape(-1, 2)
+    w.cell_cap, w.footprint_count = int(cell_cap), len(fp)
+    w.cost, w.grid, w.origin, w.query_cost = cost, grid, origin, query_cost
+    w.footprint = fp.ctypes.data if len(fp) else None
+    w._keep = fp
+    return w
+
+
 class TebTrajectoryArgs(C.Structure):
     """getVelocityProfile / getFullTrajectory read-out (tebgpu_read_trajectory): the bands to read (NULL: all B) and
     host or device output pointers"""

@@ -116,6 +116,8 @@ struct tebgpu_ctx {
   bool feas_ready = false;            /* k_feasible's shared-memory attributes set */
   int last_feas_build = -1;           /* the last k_feasible launch: its build (TEBGPU_FEAS_BUILD_*) */
   long long last_feas_grid = 0;       /* ... and its grid in CTAs */
+  double* d_qcost = nullptr;          /* the costmap check's query_cost mirror, grown by the first call that needs more */
+  size_t qcost_bytes = 0;
   /* trajectory read-out: the host-buffer entry point's band list and output mirrors, grown by the first call that needs more */
   int32_t* d_tbands = nullptr; int32_t* d_tpoints = nullptr; double* d_tprof = nullptr; double* d_ttraj = nullptr;
   size_t tbands_bytes = 0, tpoints_bytes = 0, tprof_bytes = 0, ttraj_bytes = 0;
@@ -228,6 +230,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 8: return (int32_t)sizeof(TebCostmapArgs);
     case 9: return (int32_t)sizeof(TebLocalPlanArgs);
     case 10: return (int32_t)sizeof(TebCycleArgs);
+    case 11: return (int32_t)sizeof(TebCostmapWorld);
     default: return -1;
   }
 }
@@ -265,7 +268,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
-                  c->d_cneeded, c->d_lplan, c->d_cycle};
+                  c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1342,20 +1345,27 @@ int32_t tebgpu_plan_batch(tebgpu_ctx* ctx, TebBatch* bt, const TebPlanInput* pla
   return TEBGPU_OK;
 }
 
-/* argument checks of both feasibility entry points: nothing is launched when one fails */
-static int32_t check_feasible_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa) {
+/* argument checks of every feasibility entry point: nothing is launched when one fails. table: the obstacle-table
+ * check, which also reads the batch's obstacle arrays and collision_distance */
+static int32_t check_feasible_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa, bool table = true) {
   if (!ctx) return TEBGPU_ERR_INVALID_ARG;
   if (!bt || !fa) { ctx->err = "batch or feasibility args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
-  if (bt->B < 1 || bt->n_cap < 1 || bt->S < 1 || bt->M_cap < 0 || bt->PV_cap < 0) { ctx->err = "bad batch dimensions"; return TEBGPU_ERR_INVALID_ARG; }
-  if (bt->B > ctx->lim.max_bands || bt->n_cap > ctx->lim.max_poses || bt->S > ctx->lim.max_scenes ||
-      bt->M_cap > ctx->lim.max_obstacles || bt->PV_cap > ctx->lim.max_obst_vertices) { ctx->err = "batch exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
-  if (!bt->poses || !bt->n || !bt->scene_id || !bt->obst_count) { ctx->err = "missing required batch array"; return TEBGPU_ERR_INVALID_ARG; }
-  if (bt->M_cap > 0 && !bt->obstacles) { ctx->err = "obstacles == NULL"; return TEBGPU_ERR_INVALID_ARG; }
-  if (bt->PV_cap > 0 && !bt->obst_vertices) { ctx->err = "obst_vertices == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (table) {
+    if (bt->B < 1 || bt->n_cap < 1 || bt->S < 1 || bt->M_cap < 0 || bt->PV_cap < 0) { ctx->err = "bad batch dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+    if (bt->B > ctx->lim.max_bands || bt->n_cap > ctx->lim.max_poses || bt->S > ctx->lim.max_scenes ||
+        bt->M_cap > ctx->lim.max_obstacles || bt->PV_cap > ctx->lim.max_obst_vertices) { ctx->err = "batch exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+    if (!bt->poses || !bt->n || !bt->scene_id || !bt->obst_count) { ctx->err = "missing required batch array"; return TEBGPU_ERR_INVALID_ARG; }
+    if (bt->M_cap > 0 && !bt->obstacles) { ctx->err = "obstacles == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+    if (bt->PV_cap > 0 && !bt->obst_vertices) { ctx->err = "obst_vertices == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  } else {
+    if (bt->B < 1 || bt->n_cap < 1 || bt->S < 1) { ctx->err = "bad batch dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+    if (bt->B > ctx->lim.max_bands || bt->n_cap > ctx->lim.max_poses || bt->S > ctx->lim.max_scenes) { ctx->err = "batch exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+    if (!bt->poses || !bt->n || !bt->scene_id) { ctx->err = "missing required batch array"; return TEBGPU_ERR_INVALID_ARG; }
+  }
   if (!fa->feasible || !fa->query_count) { ctx->err = "feasible or query_count == NULL"; return TEBGPU_ERR_INVALID_ARG; }
   if (!(std::isfinite(fa->inscribed_radius) && fa->inscribed_radius > 0)) { ctx->err = "inscribed_radius must be > 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
   if (!(std::isfinite(fa->angular_resolution) && fa->angular_resolution > 0)) { ctx->err = "angular_resolution must be > 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
-  if (!(std::isfinite(fa->collision_distance) && fa->collision_distance >= 0)) { ctx->err = "collision_distance must be >= 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
+  if (table && !(std::isfinite(fa->collision_distance) && fa->collision_distance >= 0)) { ctx->err = "collision_distance must be >= 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
   if (fa->max_queries < 1) { ctx->err = "max_queries must be >= 1"; return TEBGPU_ERR_INVALID_ARG; }
   if (!ctx->have_params) { ctx->err = "tebgpu_set_params has not been called"; return TEBGPU_ERR_INVALID_ARG; }
   return TEBGPU_OK;
@@ -1458,6 +1468,128 @@ int32_t tebgpu_check_feasible(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeas
     for (size_t b = 0; b < B; ++b) {
       const size_t rows = std::min<size_t>((size_t)std::max(fa->query_count[b], 0), mq);
       std::memcpy(fa->queries + b * mq * 3, q.data() + b * mq * 3, rows * 3 * sizeof(double));
+    }
+  }
+  return TEBGPU_OK;
+}
+
+static int32_t grow_mirror(tebgpu_ctx* ctx, void** p, size_t* have, size_t bytes, cudaStream_t st);
+
+/* argument checks of both costmap feasibility entry points: nothing is launched when one fails */
+static int32_t check_feasible_costmap_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa,
+                                           const TebCostmapWorld* w) {
+  const int32_t rc = check_feasible_args(ctx, bt, fa, false);
+  if (rc) return rc;
+  if (!w) { ctx->err = "costmap world == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (w->cell_cap < 1) { ctx->err = "cell_cap must be >= 1"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!w->cost || !w->grid || !w->origin) { ctx->err = "missing required costmap array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (w->footprint_count < 0 || w->footprint_count > TEB_COSTMAP_FOOTPRINT_MAX) { ctx->err = "footprint_count outside 0 .. TEB_COSTMAP_FOOTPRINT_MAX"; return TEBGPU_ERR_INVALID_ARG; }
+  if (w->footprint_count > 0 && !w->footprint) { ctx->err = "footprint == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  for (int k = 0; k < 2 * w->footprint_count; ++k)
+    if (!std::isfinite(w->footprint[k])) { ctx->err = "non-finite footprint point"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_feasible_costmap on arguments already checked: the footprint travels in the launch's parameter block */
+static int32_t issue_feasible_costmap(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa,
+                                      const TebCostmapWorld* w, cudaStream_t st) {
+  FeasDev fd;
+  std::memset(&fd, 0, sizeof(fd));
+  fd.B = bt->B; fd.n_cap = bt->n_cap; fd.S = bt->S;
+  fd.poses = bt->poses; fd.n = bt->n; fd.scene_id = bt->scene_id;
+  fd.a = *fa;
+  FeasRasterDev rd;
+  std::memset(&rd, 0, sizeof(rd));
+  rd.cell_cap = w->cell_cap; rd.F = w->footprint_count;
+  rd.cost = w->cost; rd.grid = w->grid; rd.origin = w->origin; rd.query_cost = w->query_cost;
+  if (rd.F) std::memcpy(rd.fp, w->footprint, (size_t)rd.F * 2 * sizeof(double));
+  const int B = bt->B;
+  k_feasible_costmap<<<B, FEAS_THREADS, 0, st>>>(fd, rd);
+  ctx->last_feas_build = TEBGPU_FEAS_BUILD_COSTMAP;
+  ctx->last_feas_grid = B;
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_check_feasible_costmap_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa,
+                                             const TebCostmapWorld* w, void* cuda_stream) {
+  const int32_t rc = check_feasible_costmap_args(ctx, bt, fa, w);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_feasible_costmap(ctx, bt, fa, w, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_check_feasible_costmap(tebgpu_ctx* ctx, const TebBatch* bt, const TebFeasibilityArgs* fa,
+                                      const TebCostmapWorld* w) {
+  int32_t rc = check_feasible_costmap_args(ctx, bt, fa, w);
+  if (rc) return rc;
+  /* the bands the device entry point would answer with -1 are refused here, before anything runs */
+  for (int b = 0; b < bt->B; ++b) {
+    const int sc = bt->scene_id[b];
+    if (sc < 0 || sc >= bt->S) { ctx->err = "scene_id[b] outside 0 .. S-1"; return TEBGPU_ERR_INVALID_ARG; }
+    if (bt->n[b] < 0 || bt->n[b] > bt->n_cap) { ctx->err = "n[b] outside 0 .. n_cap"; return TEBGPU_ERR_INVALID_ARG; }
+    const int32_t sx = w->grid[2 * sc], sy = w->grid[2 * sc + 1];
+    const double* o = w->origin + 3 * sc;
+    if (sx < 1 || sy < 1) { ctx->err = "costmap size < 1"; return TEBGPU_ERR_INVALID_ARG; }
+    if ((long long)sx * sy > w->cell_cap) { ctx->err = "sx * sy > cell_cap"; return TEBGPU_ERR_INVALID_ARG; }
+    if (!(std::isfinite(o[2]) && o[2] > 0)) { ctx->err = "costmap resolution must be > 0 and finite"; return TEBGPU_ERR_INVALID_ARG; }
+    if (!std::isfinite(o[0]) || !std::isfinite(o[1])) { ctx->err = "non-finite costmap origin"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t B = bt->B, nc = bt->n_cap, mq = fa->max_queries, S = bt->S, cells = S * (size_t)w->cell_cap;
+  if (!ctx->d_feas) {
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_feas, ctx->lim.max_bands * sizeof(int32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_qcount, ctx->lim.max_bands * sizeof(int32_t)));
+  }
+  if (fa->queries && mq > ctx->feas_rows) { /* the first call with more query rows grows the mirror */
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    if (ctx->d_queries) CUDA_TRY(ctx, cudaFree(ctx->d_queries));
+    ctx->d_queries = nullptr;
+    ctx->feas_rows = 0;
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_queries, (size_t)ctx->lim.max_bands * mq * 3 * sizeof(double)));
+    ctx->feas_rows = mq;
+  }
+  /* the rasters share the costmap conversion's input mirrors */
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_ccost, &ctx->ccost_bytes, cells, st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_cgrid, &ctx->cgrid_bytes, S * 2 * sizeof(int32_t), st))) return rc;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_corigin, &ctx->corigin_bytes, S * 3 * sizeof(double), st))) return rc;
+  if (w->query_cost && (rc = grow_mirror(ctx, (void**)&ctx->d_qcost, &ctx->qcost_bytes, B * mq * sizeof(double), st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_poses, bt->poses, B * nc * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_n, bt->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_scene, bt->scene_id, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ccost, w->cost, cells, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_cgrid, w->grid, S * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_corigin, w->origin, S * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  TebBatch d = *bt;
+  d.poses = ctx->d_poses; d.n = ctx->d_n; d.scene_id = ctx->d_scene;
+  TebFeasibilityArgs da = *fa;
+  da.feasible = ctx->d_feas; da.query_count = ctx->d_qcount;
+  da.queries = fa->queries ? ctx->d_queries : nullptr;
+  TebCostmapWorld dw = *w;
+  dw.cost = ctx->d_ccost; dw.grid = ctx->d_cgrid; dw.origin = ctx->d_corigin;
+  dw.query_cost = w->query_cost ? ctx->d_qcost : nullptr;
+  rc = issue_feasible_costmap(ctx, &d, &da, &dw, st);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(fa->feasible, ctx->d_feas, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(fa->query_count, ctx->d_qcount, B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  /* only the rows the kernel wrote reach the caller: min(query_count, max_queries) per band */
+  if (fa->queries) {
+    std::vector<double> q(B * mq * 3);
+    CUDA_TRY(ctx, cudaMemcpy(q.data(), ctx->d_queries, q.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (size_t b = 0; b < B; ++b) {
+      const size_t rows = std::min<size_t>((size_t)std::max(fa->query_count[b], 0), mq);
+      std::memcpy(fa->queries + b * mq * 3, q.data() + b * mq * 3, rows * 3 * sizeof(double));
+    }
+  }
+  if (w->query_cost) {
+    std::vector<double> c(B * mq);
+    CUDA_TRY(ctx, cudaMemcpy(c.data(), ctx->d_qcost, c.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (size_t b = 0; b < B; ++b) {
+      const size_t rows = std::min<size_t>((size_t)std::max(fa->query_count[b], 0), mq);
+      std::memcpy(w->query_cost + b * mq, c.data() + b * mq, rows * sizeof(double));
     }
   }
   return TEBGPU_OK;
