@@ -363,8 +363,8 @@ typedef struct TebTrajectoryArgs {
  *      dx * c + dy * s < 0 && sqrt(dx * dx + dy * dy) > behind_robot_dist (a NaN anywhere keeps it, as in the reference),
  *      otherwise it gives the row {wx, wy, 0, 0, 0, dynamic 0, TEB_OBST_POINT, 0, 0, _pad 0}: every byte is defined.
  *      Every product and sum is rounded on its own (no FMA contraction), as in the reference's x86 build.
- *   2. Then custom[s][0 .. custom_count[s]) verbatim. Their vertex_begin refers to the batch's obst_vertices, which the
- *      caller fills; Point rows use no vertex, so nothing is rebased.
+ *   2. Then custom[s][0 .. custom_count[s]) verbatim (tebgpu_costmap_obstacles_tf moves them, see TebFrameArgs).
+ *      Their vertex_begin refers to the batch's obst_vertices, which the caller fills; Point rows use no vertex, so nothing is rebased.
  *   3. needed[s] = the number of rows. If it is <= M_cap, obst_count[s] = needed[s]; otherwise the first M_cap rows are
  *      written and obst_count[s] = -1, which every consumer refuses (TEB_STATUS_BAD_INPUT from the optimize and plan
  *      entry points, -1 from the feasibility check, NaN from the device H-signature): no obstacle is dropped silently.
@@ -391,7 +391,8 @@ typedef struct TebCostmapArgs {
 
 /* Each robot's global plan cut into its local plan, goal and via-points (tebgpu_local_plan): the front of
  * TebLocalPlannerROS::computeVelocityCommands from pruneGlobalPlan up to the start row (teb_local_planner_ros.cpp:268-340),
- * under the identity transform: the global plan is given in the frame of the costmap and of the obstacle tables. HOST
+ * under the identity transform: the global plan is given in the frame of the costmap and of the obstacle tables
+ * (tebgpu_local_plan_tf takes it in its own frame, see TebFrameArgs). HOST
  * pointers for tebgpu_local_plan, DEVICE pointers for tebgpu_local_plan_device. Of the batch only B, S and scene_id are
  * read. One output row per band b; plan / plan_count and via / via_count have the layout of TebPlanInput.initial_plan /
  * plan_count and TebBatch.via / via_count, so they feed tebgpu_plan_batch(_device) on the same stream.
@@ -478,6 +479,64 @@ typedef struct TebLocalPlanArgs {
 #define TEB_LOCAL_PLAN_EMPTY        2  /* no live row in the global plan: plan_count = 0 */
 #define TEB_LOCAL_PLAN_CAPACITY     3  /* more rows than P_cap or via-points than V_cap: plan_count = 0, see needed */
 #define TEB_LOCAL_PLAN_BAD_INPUT    4  /* device entry point only: plan_begin / plan_end / scene_id out of range */
+
+/* The frames of tebgpu_local_plan_tf and tebgpu_costmap_obstacles_tf (and their _device forms): the transforms the node
+ * has looked up, so that the global plans and the custom obstacles stay in their own frames (usually map) while the
+ * costmap, the robot pose and the obstacle tables are in the costmap's global frame (usually odom). The tf tree and its
+ * lookups (time, transform_tolerance) stay the caller's. A transform is 7 doubles in geometry_msgs/Transform order
+ * tx, ty, tz, qx, qy, qz, qw; the quaternion is taken as given, not normalised. HOST pointers for the synchronous entry
+ * points, DEVICE pointers for the _device ones. Every NULL: the identity transform of TebLocalPlanArgs / TebCostmapArgs.
+ *
+ * The arithmetic is ROS Noetic's (tf2 LinearMath, tf2_geometry_msgs' doTransform, tf2/impl/utils.h getYaw, tf2_eigen's
+ * transformToEigen) and Eigen 3.3's (toRotationMatrix, the fixed-size matrix-vector product of an x86-64 SSE2 build),
+ * none of which is in the reference checkout; csrc/teb_frame.h holds it once for the host and the device. Every product
+ * and sum is rounded on its own (no FMA contraction).
+ *
+ * tf2::doTransform of a plan row (x, y, yaw) under a transform T = (t, q): the row's orientation is r = (0, 0,
+ * sin(yaw / 2), cos(yaw / 2)) (teb_plan_yaw's model) and z = 0. basis(q) is Matrix3x3::setRotation (s = 2 / |q|^2);
+ * the position is basis(T) * (x, y, 0) + t, each row of the basis summed ((b0 x + b1 y) + b2 0) + t_i; the orientation
+ * is getRotation() of basis(T) * basis(r) (the trace branch, else the largest diagonal element's); the yaw stored is
+ * tf2::getYaw of it (sarg = -2 (xz - wy) / |q|^2; sarg <= -0.99999: -2 atan2(y, x); >= 0.99999: 2 atan2(y, x); else
+ * atan2(2 (xy + wz), w^2 + x^2 - y^2 - z^2)). In TebLocalPlanArgs' steps:
+ *   1, 3  compare the rows, still in the plan frame, with doTransform(robot, costmap_to_plan)'s position; the window,
+ *         plan_length and every decision are the plan frame's, as in the reference.
+ *   3     every row taken, and the injected global goal, is doTransform(row, plan_to_costmap); only rows taken are
+ *         transformed: the plan write moves each once, and the via-point count and write (when via-points are
+ *         extracted) move each row they scan once more per pass.
+ *   4     via-points from the transformed rows.
+ *   5     the goal-reached test reads doTransform(g[n - 1], plan_to_costmap): its position, and getYaw of its orientation
+ *         in place of teb_plan_yaw(g[n - 1].yaw).
+ *   7     the stored yaw is the transformed row's; goal_idx >= n - 1: getYaw of the transformed local goal's
+ *         orientation; goal_idx > n - 5: getYaw(q * r(g[n - 1].yaw)), the raw tf2 quaternion product with
+ *         plan_to_costmap's q; else the moving average over the transformed positions of the local goal and g[goal_idx
+ *         + 1 ..].
+ *   8     row 0 is the robot pose as given (the costmap frame).
+ * Custom rows (TebCostmapArgs step 2) under custom_to_costmap: Eigen::Isometry3d(Translation3d(t) * Quaterniond(q)),
+ * whose linear part is toRotationMatrix (no division by |q|^2, so a non-unit quaternion scales here where setRotation
+ * does not, as in the node) and whose translation is 0 + t; a point p moves to linear * (p.x, p.y, 0) + translation,
+ * rows summed as above.
+ *   Point, Circular  (x, y) moves; radius, velocities (not rotated: the reference passes setCentroidVelocity the
+ *                    message's twist as it is), dynamic and the rest verbatim.
+ *   Line, Pill       custom_vertices[s][vertex_begin .. + 2) move into obst_vertices at the same index (vertex_count
+ *                    must be 2); (x, y) = 0.5 * (start + end) of the moved ends.
+ *   Polygon          custom_vertices[s][vertex_begin .. + vertex_count) move into obst_vertices; then finalizePolygon:
+ *                    the last vertex is dropped (fixPolygonClosure, obstacles.cpp:48-55) when Eigen's isApprox (1e-12)
+ *                    finds it equal to the first (vertex_count - 1 in the row), and (x, y) = calcCentroid
+ *                    (obstacles.cpp:57-126) of the moved vertices.
+ *   other types      verbatim.
+ * Where the device and the reference part ways: sin, cos, atan2 and sqrt are the device's (the yaws and the goal
+ * heading, not the positions: those are bit for bit); a stored yaw that came from a tilted transform is read back
+ * downstream through teb_plan_yaw, where the reference keeps the tilted quaternion; an angle the two sides round to
+ * opposite ends of +-pi differs by 2 pi. */
+typedef struct TebFrameArgs {
+  int32_t PV_cap;                  /* vertices per scene (stride of custom_vertices and obst_vertices), >= 0 */
+  int32_t _pad;
+  const double* costmap_to_plan;   /* [B][7] or NULL: lookupTransform(plan_frame, global_frame), moves the robot pose */
+  const double* plan_to_costmap;   /* [B][7] or NULL: plan_to_global_transform, moves the rows taken */
+  const double* custom_to_costmap; /* [S][7] or NULL: obstacle_to_map of each scene's custom obstacles */
+  const double* custom_vertices;   /* [S][PV_cap][2] or NULL: the custom Line / Pill / Polygon vertices in their frame */
+  double*       obst_vertices;     /* [S][PV_cap][2] out (the batch's vertex pool): the moved vertices of the rows written */
+} TebFrameArgs;
 
 /* The controller state of every robot between cycles, and the two steps of TebLocalPlannerROS::computeVelocityCommands
  * around plan() that read and write it: tebgpu_backup_modes, the oscillation half of configureBackupModes
@@ -584,7 +643,7 @@ typedef struct TebCycleArgs {
 
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
- * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld. */
+ * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -713,6 +772,22 @@ int32_t tebgpu_costmap_obstacles_device(tebgpu_ctx* ctx, const TebCostmapArgs* a
  * tebgpu_local_plan_device: DEVICE buffers, stream ordered as tebgpu_optimize_batch_device, does not synchronise. */
 int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args);
 int32_t tebgpu_local_plan_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args, void* cuda_stream);
+
+/* The same two steps with each robot's global plan and each scene's custom obstacles in their own frames, as defined at
+ * TebFrameArgs. frames == NULL, or all four of its transform / vertex pointers NULL, is the call without _tf, bit for
+ * bit. Argument errors of TebFrameArgs (only one of costmap_to_plan / plan_to_costmap; custom_vertices without
+ * custom_to_costmap; custom_vertices without obst_vertices or PV_cap; PV_cap < 0; a misaligned custom array) return
+ * TEBGPU_ERR_INVALID_ARG before anything is launched. tebgpu_costmap_obstacles_tf also refuses a custom Line / Pill /
+ * Polygon row whose vertices lie outside 0 .. PV_cap or are not given (custom_vertices == NULL); the _device form answers
+ * that scene with obst_count = needed = -1 instead. tebgpu_costmap_obstacles_tf copies back the moved vertices of every
+ * row it wrote, into frames->obst_vertices (HOST). */
+int32_t tebgpu_local_plan_tf(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args,
+                             const TebFrameArgs* frames);
+int32_t tebgpu_local_plan_tf_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebLocalPlanArgs* args,
+                                    const TebFrameArgs* frames, void* cuda_stream);
+int32_t tebgpu_costmap_obstacles_tf(tebgpu_ctx* ctx, const TebCostmapArgs* args, const TebFrameArgs* frames);
+int32_t tebgpu_costmap_obstacles_tf_device(tebgpu_ctx* ctx, const TebCostmapArgs* args, const TebFrameArgs* frames,
+                                           void* cuda_stream);
 
 /* The two controller steps around plan(), as defined at TebCycleArgs. One thread per band, so that the detector's sums
  * run in the reference's order (tebgpu_get_info key 17). A fleet cycle on one stream: tebgpu_costmap_obstacles_device,

@@ -72,6 +72,16 @@ def load_library(build_if_missing=False):
     L.tebgpu_local_plan.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs)]
     L.tebgpu_local_plan_device.restype = C.c_int32
     L.tebgpu_local_plan_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs), vp]
+    L.tebgpu_costmap_obstacles_tf.restype = C.c_int32
+    L.tebgpu_costmap_obstacles_tf.argtypes = [vp, C.POINTER(abi.TebCostmapArgs), C.POINTER(abi.TebFrameArgs)]
+    L.tebgpu_costmap_obstacles_tf_device.restype = C.c_int32
+    L.tebgpu_costmap_obstacles_tf_device.argtypes = [vp, C.POINTER(abi.TebCostmapArgs), C.POINTER(abi.TebFrameArgs), vp]
+    L.tebgpu_local_plan_tf.restype = C.c_int32
+    L.tebgpu_local_plan_tf.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs),
+                                       C.POINTER(abi.TebFrameArgs)]
+    L.tebgpu_local_plan_tf_device.restype = C.c_int32
+    L.tebgpu_local_plan_tf_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs),
+                                              C.POINTER(abi.TebFrameArgs), vp]
     for name in ("tebgpu_backup_modes", "tebgpu_finish_cycle"):
         getattr(L, name).restype = C.c_int32
         getattr(L, name).argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebCycleArgs)]
@@ -324,12 +334,15 @@ class TebGpu:
                     "tebgpu_read_trajectory_device")
 
     def costmap_obstacles(self, cost, grid, origin, robot, M_cap, behind_robot_dist=1.5, include=True, custom=None,
-                          custom_count=None):
+                          custom_count=None, custom_to_costmap=None, custom_vertices=None):
         """Each scene's obstacle table from its local costmap (tebgpu_costmap_obstacles), host buffers: cost [S][cell_cap]
         uint8 (scene s's char map in its first sx * sy bytes, row my = mx + my * sx), grid [S][2] (sx, sy), origin [S][3]
         (ox, oy, resolution), robot [S][3] (x, y, yaw), custom [S][C_cap] abi.OBST_DTYPE rows appended after the points,
         custom_count [S]. Returns (obstacles [S][M_cap] abi.OBST_DTYPE, zero past each scene's written rows, obst_count
-        [S]: the rows, or -1 when they do not fit M_cap, needed [S]: the rows the scene has)."""
+        [S]: the rows, or -1 when they do not fit M_cap, needed [S]: the rows the scene has).
+        custom_to_costmap [S][7] (see abi.TebFrameArgs): the custom rows are in their own frame and are moved into the
+        costmap's (tebgpu_costmap_obstacles_tf); custom_vertices [S][PV_cap][2] their Line / Pill / Polygon vertices in
+        that frame, whose moved copy [S][PV_cap][2] (zero where no row moved a vertex) is then returned fourth."""
         import numpy as np
         cost = np.ascontiguousarray(cost, dtype=np.uint8)
         S = cost.shape[0]
@@ -350,27 +363,43 @@ class TebGpu:
                   else np.ascontiguousarray(custom_count, dtype=np.int32).reshape(S))
             ca.C_cap, ca.custom, ca.custom_count = custom.shape[1], abi.ptr(custom), abi.ptr(cc)
         ca.obstacles, ca.obst_count, ca.needed = abi.ptr(obst), abi.ptr(cnt), abi.ptr(need)
-        self._check(self.lib.tebgpu_costmap_obstacles(self.ctx, C.byref(ca)), "tebgpu_costmap_obstacles")
-        return obst, cnt, need
+        if custom_to_costmap is None and custom_vertices is None:
+            self._check(self.lib.tebgpu_costmap_obstacles(self.ctx, C.byref(ca)), "tebgpu_costmap_obstacles")
+            return obst, cnt, need
+        tf = None if custom_to_costmap is None else np.ascontiguousarray(custom_to_costmap, dtype=np.float64).reshape(S, 7)
+        cv = None if custom_vertices is None else np.ascontiguousarray(custom_vertices, dtype=np.float64).reshape(S, -1, 2)
+        ov = None if cv is None else np.zeros_like(cv)
+        fr = abi.make_frame_args(custom_to_costmap=abi.ptr(tf), custom_vertices=abi.ptr(cv), obst_vertices=abi.ptr(ov),
+                                 PV_cap=0 if cv is None else cv.shape[1])
+        self._check(self.lib.tebgpu_costmap_obstacles_tf(self.ctx, C.byref(ca), C.byref(fr)), "tebgpu_costmap_obstacles_tf")
+        return (obst, cnt, need) if ov is None else (obst, cnt, need, ov)
 
-    def costmap_obstacles_device(self, args, stream=None):
+    def costmap_obstacles_device(self, args, stream=None, frames=None):
         """tebgpu_costmap_obstacles_device: the same conversion over DEVICE memory (args: an abi.TebCostmapArgs of device
         pointers, e.g. the obstacles / obst_count of the batch it feeds). Stream ordered on `stream` (a cudaStream_t
-        handle; None: the context's stream); does not synchronise."""
-        self._check(self.lib.tebgpu_costmap_obstacles_device(self.ctx, C.byref(args), stream),
-                    "tebgpu_costmap_obstacles_device")
+        handle; None: the context's stream); does not synchronise. frames: an abi.TebFrameArgs of device pointers
+        (custom_to_costmap, custom_vertices, obst_vertices: the batch's vertex pool), or None: the custom rows verbatim."""
+        if frames is None:
+            self._check(self.lib.tebgpu_costmap_obstacles_device(self.ctx, C.byref(args), stream),
+                        "tebgpu_costmap_obstacles_device")
+        else:
+            self._check(self.lib.tebgpu_costmap_obstacles_tf_device(self.ctx, C.byref(args), C.byref(frames), stream),
+                        "tebgpu_costmap_obstacles_tf_device")
 
     def last_costmap_grid(self):
         """grid in CTAs (one per scene) of the last costmap conversion, 0 before the first"""
         return self.info(15)
 
     def local_plan(self, global_plan, plan_begin, plan_end, robot, robot_vel, grid, origin, P_cap, V_cap=None,
-                   scene_id=None, via_count=None, infeasible_count=None, since_infeasible=None, **scalars):
+                   scene_id=None, via_count=None, infeasible_count=None, since_infeasible=None, costmap_to_plan=None,
+                   plan_to_costmap=None, **scalars):
         """Each robot's local plan, goal and via-points from its global plan (tebgpu_local_plan), host buffers:
         global_plan [B][G_cap][3] (x, y, yaw), plan_begin / plan_end [B] (its live rows), robot [B][3], robot_vel [B][3]
         (vx, vy, omega), grid [S][2] and origin [S][3] of the costmaps, scene_id [B] (None: all 0). V_cap None: the
         via-points are the caller's own and via_count [B] (or None: 0) holds their counts; otherwise they are extracted
         into [B][V_cap][2]. infeasible_count / since_infeasible [B] or None. scalars: abi.make_local_plan_args' keywords.
+        costmap_to_plan / plan_to_costmap [B][7] (both or neither, see abi.TebFrameArgs and abi.transform_from_se2): the
+        global plans are in their own frame and robot in the costmap's (tebgpu_local_plan_tf).
         Returns a dict: plan_begin (moved by pruning), plan [B][P_cap][3] and via [B][V_cap][2] (NaN past the rows
         written), plan_count, goal_idx (-1 where not written), via_count, result (TEB_LOCAL_PLAN_*), needed [B][2]."""
         import numpy as np
@@ -391,7 +420,10 @@ class TebGpu:
                     sid=np.zeros(B, np.int32) if scene_id is None else i32(scene_id, (B,)),
                     inf=None if infeasible_count is None else i32(infeasible_count, (B,)),
                     since=None if since_infeasible is None else f64(since_infeasible, (B,)))
-        la = abi.make_local_plan_args(G_cap, P_cap, 0 if own else V_cap, **scalars)
+        c2p = None if costmap_to_plan is None else f64(costmap_to_plan, (B, 7))
+        p2c = None if plan_to_costmap is None else f64(plan_to_costmap, (B, 7))
+        la = abi.make_local_plan_args(G_cap, P_cap, 0 if own else V_cap, costmap_to_plan=abi.ptr(c2p),
+                                      plan_to_costmap=abi.ptr(p2c), **scalars)
         la.global_plan, la.plan_begin, la.plan_end = abi.ptr(gp), abi.ptr(out["plan_begin"]), abi.ptr(keep["pe"])
         la.robot, la.robot_vel, la.grid, la.origin = abi.ptr(keep["rb"]), abi.ptr(keep["rv"]), abi.ptr(grid), abi.ptr(keep["org"])
         la.infeasible_count, la.since_infeasible = abi.ptr(keep["inf"]), abi.ptr(keep["since"])
@@ -400,15 +432,27 @@ class TebGpu:
         la.result, la.needed = abi.ptr(out["result"]), abi.ptr(out["needed"])
         bs = abi.TebBatch()
         bs.B, bs.S, bs.scene_id = B, S, abi.ptr(keep["sid"])
-        self._check(self.lib.tebgpu_local_plan(self.ctx, C.byref(bs), C.byref(la)), "tebgpu_local_plan")
+        if la.frames is None:
+            self._check(self.lib.tebgpu_local_plan(self.ctx, C.byref(bs), C.byref(la)), "tebgpu_local_plan")
+        else:
+            self._check(self.lib.tebgpu_local_plan_tf(self.ctx, C.byref(bs), C.byref(la), C.byref(la.frames)),
+                        "tebgpu_local_plan_tf")
         return out
 
-    def local_plan_device(self, batch_struct, args, stream=None):
+    def local_plan_device(self, batch_struct, args, stream=None, frames=None):
         """tebgpu_local_plan_device: the same step over DEVICE memory (batch_struct: an abi.TebBatch whose B, S and
         scene_id are read; args: an abi.TebLocalPlanArgs of device pointers, see abi.make_local_plan_args). Stream
-        ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise."""
-        self._check(self.lib.tebgpu_local_plan_device(self.ctx, C.byref(batch_struct), C.byref(args), stream),
-                    "tebgpu_local_plan_device")
+        ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise. frames: an
+        abi.TebFrameArgs of device pointers, or None: the one make_local_plan_args kept on args (costmap_to_plan /
+        plan_to_costmap), if any (tebgpu_local_plan_tf_device)."""
+        if frames is None:
+            frames = getattr(args, "frames", None)
+        if frames is None:
+            self._check(self.lib.tebgpu_local_plan_device(self.ctx, C.byref(batch_struct), C.byref(args), stream),
+                        "tebgpu_local_plan_device")
+        else:
+            self._check(self.lib.tebgpu_local_plan_tf_device(self.ctx, C.byref(batch_struct), C.byref(args),
+                                                             C.byref(frames), stream), "tebgpu_local_plan_tf_device")
 
     def last_local_plan_grid(self):
         """grid in CTAs (4 bands each) of the last local-plan launch, 0 before the first"""

@@ -203,10 +203,15 @@ TEB_LOCAL_PLAN_PLANNED, TEB_LOCAL_PLAN_GOAL_REACHED, TEB_LOCAL_PLAN_EMPTY, TEB_L
 def make_local_plan_args(G_cap, P_cap, V_cap=0, prune_distance=1.0, max_lookahead_dist=1.0, viapoint_sep=-1.0,
                          xy_goal_tolerance=0.2, yaw_goal_tolerance=0.2, trans_stopped_vel=0.1, theta_stopped_vel=0.1,
                          shrink_horizon_min_duration=10.0, free_goal_vel=False, complete_global_plan=True,
-                         shrink_horizon_backup=True, **arrays) -> TebLocalPlanArgs:
+                         shrink_horizon_backup=True, costmap_to_plan=None, plan_to_costmap=None,
+                         **arrays) -> TebLocalPlanArgs:
     """TebLocalPlanArgs with the scalars set (the defaults are the reference's, teb_config.h:259-298, :381-382) and the
-    arrays given by keyword as addresses (ints, or None for NULL): global_plan=..., plan_begin=..., ..."""
+    arrays given by keyword as addresses (ints, or None for NULL): global_plan=..., plan_begin=..., ...
+    costmap_to_plan / plan_to_costmap (addresses of [B][7] transforms, see TebFrameArgs) are kept on the returned struct
+    as its `frames` (an abi.TebFrameArgs, None when both are None) for the _tf entry points."""
     a = TebLocalPlanArgs()
+    a.frames = (None if costmap_to_plan is None and plan_to_costmap is None
+                else make_frame_args(costmap_to_plan=costmap_to_plan, plan_to_costmap=plan_to_costmap))
     a.G_cap, a.P_cap, a.V_cap = int(G_cap), int(P_cap), int(V_cap)
     a.free_goal_vel, a.complete_global_plan = int(bool(free_goal_vel)), int(bool(complete_global_plan))
     a.shrink_horizon_backup = int(bool(shrink_horizon_backup))
@@ -220,6 +225,37 @@ def make_local_plan_args(G_cap, P_cap, V_cap=0, prune_distance=1.0, max_lookahea
             raise TypeError(f"unknown TebLocalPlanArgs array {k}")
         setattr(a, k, v)
     return a
+
+
+class TebFrameArgs(C.Structure):
+    """The frames of tebgpu_local_plan_tf / tebgpu_costmap_obstacles_tf: per-robot plan transforms [B][7], per-scene
+    custom-obstacle transforms [S][7] (tx, ty, tz, qx, qy, qz, qw) and the custom vertex pools [S][PV_cap][2], as host
+    or device pointers; NULL everywhere is the identity"""
+    _fields_ = [("PV_cap", _i), ("_pad", _i), ("costmap_to_plan", C.c_void_p), ("plan_to_costmap", C.c_void_p),
+                ("custom_to_costmap", C.c_void_p), ("custom_vertices", C.c_void_p), ("obst_vertices", C.c_void_p)]
+
+
+def make_frame_args(costmap_to_plan=None, plan_to_costmap=None, custom_to_costmap=None, custom_vertices=None,
+                    obst_vertices=None, PV_cap=0) -> TebFrameArgs:
+    """TebFrameArgs with the arrays given as addresses (ints, or None for NULL)"""
+    f = TebFrameArgs()
+    f.PV_cap = int(PV_cap)
+    f.costmap_to_plan, f.plan_to_costmap = costmap_to_plan, plan_to_costmap
+    f.custom_to_costmap, f.custom_vertices, f.obst_vertices = custom_to_costmap, custom_vertices, obst_vertices
+    return f
+
+
+def transform_from_se2(x, y, yaw):
+    """The pair of transforms a planar parent -> child pose (x, y, yaw) gives, as the node looks them up for a plan in
+    the parent frame (map) and a costmap in the child frame (odom): (costmap_to_plan, plan_to_costmap), 7 doubles each
+    (tx, ty, tz, qx, qy, qz, qw). costmap_to_plan is the pose itself; plan_to_costmap its inverse, formed in closed form
+    (the device never inverts a transform)."""
+    x, y, yaw = float(x), float(y), float(yaw)
+    c, s = np.cos(yaw), np.sin(yaw)
+    qz, qw = np.sin(yaw / 2), np.cos(yaw / 2)
+    fwd = np.array([x, y, 0.0, 0.0, 0.0, qz, qw])
+    inv = np.array([-(c * x + s * y), s * x - c * y, 0.0, 0.0, 0.0, -qz, qw])
+    return fwd, inv
 
 
 class TebCycleArgs(C.Structure):

@@ -126,6 +126,7 @@ struct tebgpu_ctx {
   uint8_t* d_ccost = nullptr; int32_t* d_cgrid = nullptr; double* d_corigin = nullptr; double* d_crobot = nullptr;
   TebObstacle* d_ccustom = nullptr; int32_t* d_ccount = nullptr; TebObstacle* d_cobst = nullptr; int32_t* d_cocount = nullptr;
   int32_t* d_cneeded = nullptr;
+  char* d_cframe = nullptr; size_t cframe_bytes = 0; /* tebgpu_costmap_obstacles_tf: transforms and vertex pools */
   size_t ccost_bytes = 0, cgrid_bytes = 0, corigin_bytes = 0, crobot_bytes = 0, ccustom_bytes = 0, ccount_bytes = 0,
          cobst_bytes = 0, cocount_bytes = 0, cneeded_bytes = 0;
   long long last_costmap_grid = 0;    /* grid in CTAs of the last k_costmap_obstacles launch */
@@ -231,6 +232,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 9: return (int32_t)sizeof(TebLocalPlanArgs);
     case 10: return (int32_t)sizeof(TebCycleArgs);
     case 11: return (int32_t)sizeof(TebCostmapWorld);
+    case 12: return (int32_t)sizeof(TebFrameArgs);
     default: return -1;
   }
 }
@@ -268,7 +270,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
-                  c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost};
+                  c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1702,33 +1704,65 @@ static int32_t check_costmap_args(tebgpu_ctx* ctx, const TebCostmapArgs* ca) {
   return TEBGPU_OK;
 }
 
-/* k_costmap_obstacles on arguments already checked */
-static int32_t issue_costmap(tebgpu_ctx* ctx, const TebCostmapArgs* ca, cudaStream_t st) {
+/* argument checks of TebFrameArgs (NULL: no frames) */
+static int32_t check_frame_args(tebgpu_ctx* ctx, const TebFrameArgs* fr) {
+  if (!fr) return TEBGPU_OK;
+  if (!fr->costmap_to_plan != !fr->plan_to_costmap) { ctx->err = "only one of costmap_to_plan / plan_to_costmap given"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fr->PV_cap < 0) { ctx->err = "PV_cap < 0"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fr->custom_vertices && !fr->custom_to_costmap) { ctx->err = "custom_vertices without custom_to_costmap"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fr->custom_vertices && (!fr->obst_vertices || fr->PV_cap < 1)) { ctx->err = "custom_vertices without obst_vertices or PV_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_costmap_obstacles on arguments already checked; fr NULL or without custom_to_costmap: the custom rows verbatim */
+static int32_t issue_costmap(tebgpu_ctx* ctx, const TebCostmapArgs* ca, const TebFrameArgs* fr, cudaStream_t st) {
   TebCostmapArgs a = *ca;
   if (!a.custom_count) a.custom = nullptr;
-  k_costmap_obstacles<<<ca->S, COSTMAP_THREADS, 0, st>>>(a);
+  TebFrameArgs f{};
+  if (fr) f = *fr;
+  if (f.custom_to_costmap && a.custom) k_costmap_obstacles<true><<<ca->S, COSTMAP_THREADS, 0, st>>>(a, f);
+  else k_costmap_obstacles<false><<<ca->S, COSTMAP_THREADS, 0, st>>>(a, f);
   ctx->last_costmap_grid = ca->S;
   ctx->launches = 1;
   CUDA_TRY(ctx, cudaGetLastError());
   return TEBGPU_OK;
 }
 
-int32_t tebgpu_costmap_obstacles_device(tebgpu_ctx* ctx, const TebCostmapArgs* ca, void* cuda_stream) {
-  const int32_t rc = check_costmap_args(ctx, ca);
-  if (rc) return rc;
+int32_t tebgpu_costmap_obstacles_tf_device(tebgpu_ctx* ctx, const TebCostmapArgs* ca, const TebFrameArgs* fr,
+                                           void* cuda_stream) {
+  int32_t rc = check_costmap_args(ctx, ca);
+  if (rc || (rc = check_frame_args(ctx, fr))) return rc;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  return issue_costmap(ctx, ca, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+  return issue_costmap(ctx, ca, fr, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_costmap_obstacles_device(tebgpu_ctx* ctx, const TebCostmapArgs* ca, void* cuda_stream) {
+  return tebgpu_costmap_obstacles_tf_device(ctx, ca, nullptr, cuda_stream);
 }
 
 int32_t tebgpu_costmap_obstacles(tebgpu_ctx* ctx, const TebCostmapArgs* ca) {
+  return tebgpu_costmap_obstacles_tf(ctx, ca, nullptr);
+}
+
+int32_t tebgpu_costmap_obstacles_tf(tebgpu_ctx* ctx, const TebCostmapArgs* ca, const TebFrameArgs* fr) {
   int32_t rc = check_costmap_args(ctx, ca);
-  if (rc) return rc;
+  if (rc || (rc = check_frame_args(ctx, fr))) return rc;
+  const bool move = fr && fr->custom_to_costmap && ca->custom_count && ca->C_cap > 0;
   /* the scenes the device entry point would answer with -1 are refused here, before anything runs */
   for (int s = 0; s < ca->S; ++s) {
     const int32_t sx = ca->grid[2 * s], sy = ca->grid[2 * s + 1];
     if (sx < 0 || sy < 0) { ctx->err = "negative costmap size"; return TEBGPU_ERR_INVALID_ARG; }
     if ((long long)sx * sy > ca->cell_cap) { ctx->err = "sx * sy > cell_cap"; return TEBGPU_ERR_INVALID_ARG; }
     if (ca->custom_count && (ca->custom_count[s] < 0 || ca->custom_count[s] > ca->C_cap)) { ctx->err = "custom_count[s] outside 0 .. C_cap"; return TEBGPU_ERR_INVALID_ARG; }
+    for (int k = 0; move && k < ca->custom_count[s]; ++k) {
+      const TebObstacle& o = ca->custom[(size_t)s * ca->C_cap + k];
+      if (o.type != TEB_OBST_LINE && o.type != TEB_OBST_PILL && o.type != TEB_OBST_POLYGON) continue;
+      if (!fr->custom_vertices) { ctx->err = "custom Line / Pill / Polygon rows without custom_vertices"; return TEBGPU_ERR_INVALID_ARG; }
+      if (o.vertex_begin < 0 || o.vertex_count < 1 || o.vertex_begin > fr->PV_cap - o.vertex_count ||
+          (o.type != TEB_OBST_POLYGON && o.vertex_count != 2)) {
+        ctx->err = "custom row vertices outside 0 .. PV_cap"; return TEBGPU_ERR_INVALID_ARG;
+      }
+    }
   }
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
@@ -1756,8 +1790,25 @@ int32_t tebgpu_costmap_obstacles(tebgpu_ctx* ctx, const TebCostmapArgs* ca) {
   da.custom = cu ? ctx->d_ccustom : nullptr;
   da.custom_count = ca->custom_count ? ctx->d_ccount : nullptr;
   da.obstacles = ctx->d_cobst; da.obst_count = ctx->d_cocount; da.needed = ctx->d_cneeded;
-  rc = issue_costmap(ctx, &da, st);
+  /* frames: the transforms and both vertex pools; obst_vertices goes up too, so the vertices no row moves come back as
+   * the caller left them */
+  TebFrameArgs df{};
+  const size_t tf_bytes = S * 7 * sizeof(double), pv_bytes = fr && fr->custom_vertices ? S * fr->PV_cap * 2 * sizeof(double) : 0;
+  if (move) {
+    if ((rc = grow_mirror(ctx, (void**)&ctx->d_cframe, &ctx->cframe_bytes, tf_bytes + 2 * pv_bytes, st))) return rc;
+    df.PV_cap = fr->PV_cap;
+    df.custom_to_costmap = (const double*)ctx->d_cframe;
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_cframe, fr->custom_to_costmap, tf_bytes, cudaMemcpyHostToDevice, st));
+    if (pv_bytes) {
+      df.custom_vertices = (const double*)(ctx->d_cframe + tf_bytes);
+      df.obst_vertices = (double*)(ctx->d_cframe + tf_bytes + pv_bytes);
+      CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_cframe + tf_bytes, fr->custom_vertices, pv_bytes, cudaMemcpyHostToDevice, st));
+      CUDA_TRY(ctx, cudaMemcpyAsync(df.obst_vertices, fr->obst_vertices, pv_bytes, cudaMemcpyHostToDevice, st));
+    }
+  }
+  rc = issue_costmap(ctx, &da, move ? &df : nullptr, st);
   if (rc) return rc;
+  if (pv_bytes && move) CUDA_TRY(ctx, cudaMemcpyAsync(fr->obst_vertices, df.obst_vertices, pv_bytes, cudaMemcpyDeviceToHost, st));
   std::vector<int32_t> need(S);
   CUDA_TRY(ctx, cudaMemcpyAsync(ca->obst_count, ctx->d_cocount, S * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(need.data(), ctx->d_cneeded, S * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1788,27 +1839,44 @@ static int32_t check_local_plan_args(tebgpu_ctx* ctx, const TebBatch* bt, const 
   return TEBGPU_OK;
 }
 
-/* k_local_plan on arguments already checked */
-static int32_t issue_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la, cudaStream_t st) {
+/* k_local_plan on arguments already checked; fr NULL or without plan transforms: the identity transform */
+static int32_t issue_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la, const TebFrameArgs* fr,
+                                cudaStream_t st) {
   const long long grid = ((long long)bt->B * 32 + LPLAN_THREADS - 1) / LPLAN_THREADS;
-  k_local_plan<<<(unsigned)grid, LPLAN_THREADS, 0, st>>>(*la, bt->scene_id, bt->B, bt->S,
-                                                         ctx->params.global_plan_overwrite_orientation);
+  TebFrameArgs f{};
+  if (fr) f = *fr;
+  if (f.costmap_to_plan)
+    k_local_plan<true><<<(unsigned)grid, LPLAN_THREADS, 0, st>>>(*la, f, bt->scene_id, bt->B, bt->S,
+                                                                 ctx->params.global_plan_overwrite_orientation);
+  else
+    k_local_plan<false><<<(unsigned)grid, LPLAN_THREADS, 0, st>>>(*la, f, bt->scene_id, bt->B, bt->S,
+                                                                  ctx->params.global_plan_overwrite_orientation);
   ctx->last_lplan_grid = grid;
   ctx->launches = 1;
   CUDA_TRY(ctx, cudaGetLastError());
   return TEBGPU_OK;
 }
 
-int32_t tebgpu_local_plan_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la, void* cuda_stream) {
-  const int32_t rc = check_local_plan_args(ctx, bt, la);
-  if (rc) return rc;
+int32_t tebgpu_local_plan_tf_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la,
+                                    const TebFrameArgs* fr, void* cuda_stream) {
+  int32_t rc = check_local_plan_args(ctx, bt, la);
+  if (rc || (rc = check_frame_args(ctx, fr))) return rc;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  return issue_local_plan(ctx, bt, la, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+  return issue_local_plan(ctx, bt, la, fr, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_local_plan_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la, void* cuda_stream) {
+  return tebgpu_local_plan_tf_device(ctx, bt, la, nullptr, cuda_stream);
 }
 
 int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la) {
+  return tebgpu_local_plan_tf(ctx, bt, la, nullptr);
+}
+
+int32_t tebgpu_local_plan_tf(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPlanArgs* la, const TebFrameArgs* fr) {
   int32_t rc = check_local_plan_args(ctx, bt, la);
-  if (rc) return rc;
+  if (rc || (rc = check_frame_args(ctx, fr))) return rc;
+  const bool tf = fr && fr->costmap_to_plan;
   /* the bands the device entry point would answer with TEB_LOCAL_PLAN_BAD_INPUT are refused here, before anything runs */
   for (int b = 0; b < bt->B; ++b) {
     if (la->plan_begin[b] < 0 || la->plan_begin[b] > la->plan_end[b] || la->plan_end[b] > la->G_cap) {
@@ -1827,7 +1895,8 @@ int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPla
                o_origin = slot(S * 3 * sizeof(double)), o_sid = slot(B * 4), o_inf = slot(la->infeasible_count ? B * 4 : 0),
                o_since = slot(la->since_infeasible ? B * sizeof(double) : 0), o_plan = slot(B * P * 3 * sizeof(double)),
                o_pcount = slot(B * 4), o_goal = slot(B * 4), o_via = slot(la->via ? B * V * 2 * sizeof(double) : 0),
-               o_vcount = slot(B * 4), o_result = slot(B * 4), o_needed = slot(B * 2 * 4);
+               o_vcount = slot(B * 4), o_result = slot(B * 4), o_needed = slot(B * 2 * 4),
+               o_c2p = slot(tf ? B * 7 * sizeof(double) : 0), o_p2c = slot(tf ? B * 7 * sizeof(double) : 0);
   if ((rc = grow_mirror(ctx, (void**)&ctx->d_lplan, &ctx->lplan_bytes, off, st))) return rc;
   char* d = ctx->d_lplan;
   auto up = [&](size_t o, const void* src, size_t bytes) -> int32_t {
@@ -1843,6 +1912,13 @@ int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPla
       (rc = up(o_goal, la->goal_idx, B * 4)) || (rc = up(o_vcount, la->via_count, B * 4)) ||
       (rc = up(o_needed, la->needed, B * 2 * 4)))
     return rc;
+  TebFrameArgs df{};
+  if (tf) {
+    if ((rc = up(o_c2p, fr->costmap_to_plan, B * 7 * sizeof(double))) || (rc = up(o_p2c, fr->plan_to_costmap, B * 7 * sizeof(double))))
+      return rc;
+    df.costmap_to_plan = (const double*)(d + o_c2p);
+    df.plan_to_costmap = (const double*)(d + o_p2c);
+  }
   TebBatch db = *bt;
   db.scene_id = (const int32_t*)(d + o_sid);
   TebLocalPlanArgs da = *la;
@@ -1858,7 +1934,7 @@ int32_t tebgpu_local_plan(tebgpu_ctx* ctx, const TebBatch* bt, const TebLocalPla
   da.via_count = la->via_count ? (int32_t*)(d + o_vcount) : nullptr;
   da.result = (int32_t*)(d + o_result);
   da.needed = la->needed ? (int32_t*)(d + o_needed) : nullptr;
-  if ((rc = issue_local_plan(ctx, &db, &da, st))) return rc;
+  if ((rc = issue_local_plan(ctx, &db, &da, tf ? &df : nullptr, st))) return rc;
   auto down = [&](void* dst, size_t o, size_t bytes) -> int32_t {
     if (dst && bytes) CUDA_TRY(ctx, cudaMemcpyAsync(dst, d + o, bytes, cudaMemcpyDeviceToHost, st));
     return TEBGPU_OK;

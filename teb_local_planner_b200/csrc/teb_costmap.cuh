@@ -3,7 +3,9 @@
  * converter-less branch of TebLocalPlannerROS::updateObstacleContainerWithCostmap (teb_local_planner_ros.cpp:478-504)
  * followed by the custom obstacles (:552-625). The contract is at TebCostmapArgs in include/teb_b200.h.
  *
- *   k_costmap_obstacles  one CTA per scene
+ *   k_costmap_obstacles<false>  one CTA per scene, custom rows verbatim
+ *   k_costmap_obstacles<true>   the same with the custom rows moved from their own frame (TebFrameArgs, teb_frame.h's
+ *                               Eigen isometry), one thread per row, a polygon finalised again by its thread
  *
  * The reference runs down the columns of a row-major raster (i over x outer, j over y inner), so 32 consecutive cells of
  * its order lie in 32 different rows: read straight from global memory, one sector each. The CTA therefore stages the
@@ -21,6 +23,7 @@
 #include <climits>
 #include <cstdint>
 
+#include "teb_frame.h"
 #include "teb_plan.h"
 
 namespace tebgpu {
@@ -42,7 +45,44 @@ __device__ __forceinline__ void costmap_store_row(TebObstacle* dst, const uint4 
   for (int k = 0; k < 4; ++k) d[k] = q[k];
 }
 
-__global__ void __launch_bounds__(COSTMAP_THREADS) k_costmap_obstacles(TebCostmapArgs a) {
+/* custom row o of scene s moved by custom_to_costmap (TebFrameArgs), its vertices written to obst_vertices; false for a
+ * Line / Pill / Polygon row whose vertices are not given or lie outside 0 .. PV_cap */
+__device__ bool costmap_move_custom(TebObstacle& o, const TebFrameArgs& f, int s) {
+  const double* t = f.custom_to_costmap + 7 * (size_t)s;
+  double m[9];
+  teb_eigen_basis(t + 3, m);
+  const double org[2] = {teb_add(0.0, t[0]), teb_add(0.0, t[1])}; /* Translation3d * Isometry3d: pretranslate of 0 */
+  double p[2];
+  if (o.type == TEB_OBST_POINT || o.type == TEB_OBST_CIRCULAR) {
+    teb_frame_point(m, org, o.x, o.y, 0.0, p);
+    o.x = p[0]; o.y = p[1];
+    return true;
+  }
+  if (o.type != TEB_OBST_LINE && o.type != TEB_OBST_PILL && o.type != TEB_OBST_POLYGON) return true;
+  const int vb = o.vertex_begin, vc = o.vertex_count;
+  if (!f.custom_vertices || vb < 0 || vc < 1 || vb > f.PV_cap - vc || (o.type != TEB_OBST_POLYGON && vc != 2)) return false;
+  const double* src = f.custom_vertices + ((size_t)s * f.PV_cap + vb) * 2;
+  double* dst = f.obst_vertices + ((size_t)s * f.PV_cap + vb) * 2;
+  for (int i = 0; i < vc; ++i) {
+    teb_frame_point(m, org, src[2 * i], src[2 * i + 1], 0.0, p);
+    dst[2 * i] = p[0]; dst[2 * i + 1] = p[1];
+  }
+  if (o.type != TEB_OBST_POLYGON) {
+    o.x = teb_mul(0.5, teb_add(dst[0], dst[2]));
+    o.y = teb_mul(0.5, teb_add(dst[1], dst[3]));
+    return true;
+  }
+  int n = vc; /* finalizePolygon: fixPolygonClosure, then calcCentroid */
+  if (n >= 2 && teb_eigen_is_approx(dst[0], dst[1], dst[2 * n - 2], dst[2 * n - 1])) --n;
+  o.vertex_count = n;
+  teb_polygon_centroid(dst, n, p);
+  o.x = p[0]; o.y = p[1];
+  return true;
+}
+
+/* TF: the custom rows in their own frame (TebFrameArgs' custom_to_costmap != NULL); otherwise f is not read */
+template <bool TF>
+__global__ void __launch_bounds__(COSTMAP_THREADS) k_costmap_obstacles(TebCostmapArgs a, TebFrameArgs f) {
   __shared__ __align__(16) uint8_t sr[COSTMAP_SMEM];
   __shared__ int swarp[COSTMAP_THREADS / 32];
   const int s = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -142,12 +182,28 @@ __global__ void __launch_bounds__(COSTMAP_THREADS) k_costmap_obstacles(TebCostma
       }
     }
   }
-  /* the custom rows, verbatim */
+  /* the custom rows, verbatim, or moved into the costmap frame */
   const TebObstacle* cu = a.custom ? a.custom + (size_t)s * a.C_cap : nullptr;
+  bool bad = false;
   for (int k = tid; k < cc && (long long)base + k < a.M_cap; k += COSTMAP_THREADS) {
     const uint4* src = reinterpret_cast<const uint4*>(cu + k);
-    const uint4 row[4] = {__ldg(src), __ldg(src + 1), __ldg(src + 2), __ldg(src + 3)};
+    uint4 row[4] = {__ldg(src), __ldg(src + 1), __ldg(src + 2), __ldg(src + 3)};
+    if constexpr (TF) {
+      TebObstacle o;
+      memcpy(&o, row, sizeof(o));
+      bad |= !costmap_move_custom(o, f, s);
+      memcpy(row, &o, sizeof(o));
+    }
     costmap_store_row(out + base + k, row);
+  }
+  if constexpr (TF) {
+    if (__syncthreads_or(bad)) {
+      if (tid == 0) {
+        a.obst_count[s] = -1;
+        if (a.needed) a.needed[s] = -1;
+      }
+      return;
+    }
   }
   if (tid == 0) {
     const long long need = (long long)base + cc;
