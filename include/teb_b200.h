@@ -864,6 +864,46 @@ int32_t tebgpu_get_plan_kernel_times(tebgpu_ctx* ctx, double ms_out[2], int64_t 
  * outside 0 .. n_cap gets NaN in every output of its row. */
 int32_t tebgpu_h_signature(tebgpu_ctx* ctx, const TebBatch* batch, int32_t use_timediffs, double* h_out, int32_t device_ptrs);
 
+/* The scene half of the 2-D signature, for scenes of up to 16384 obstacles (tebgpu_sizeof(13)). HSignature's pole
+ * residue A_l = f0(o_l) / prod_{j != l, |o_l - o_j| >= 0.05} (o_l - o_j) (h_signature.h:149-163) splits into the band's
+ * f0 (its map rectangle) and
+ *     Q_l = 1 / prod_{j != l, |o_l - o_j| >= 0.05} (o_l - o_j),
+ * which depends on the scene's rows only. Q_l = (factor[s][l][0] + i factor[s][l][1]) * 2^factor_exp[s][l], exponent
+ * INT32_MIN for 0; factor_count[s] is the obst_count the table was built at, -1 for a count outside 0 .. M_cap. Rows past
+ * factor_count[s] are 0 / INT32_MIN. The table is the caller's to rebuild whenever a scene's rows change, e.g. after
+ * every tebgpu_costmap_obstacles: factor_count only catches a changed count, not moved rows. */
+typedef struct TebHsigFactors {
+  double*  factor;        /* [S][M_cap][2] mantissa (Re, Im) of Q_l */
+  int32_t* factor_exp;    /* [S][M_cap] binary exponent of Q_l */
+  int32_t* factor_count;  /* [S] obst_count the scene's table was built at, or -1 */
+} TebHsigFactors;
+
+/* Builds every scene's factor table; only S, M_cap, obstacles and obst_count of the batch are read. A scene's table
+ * depends on its own rows only (the same bits whatever S, M_cap or the scene's index). NULL arrays, S outside 1 ..
+ * max_scenes or M_cap outside 0 .. max_obstacles return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit) before
+ * anything is launched. tebgpu_hsig_factors: HOST buffers, synchronous, an obst_count outside 0 .. M_cap is refused.
+ * tebgpu_hsig_factors_device: DEVICE buffers, stream ordered as tebgpu_optimize_batch_device, does not synchronise;
+ * such a scene gets factor_count = -1. Partial products live in context scratch, allocated by the first call that needs
+ * it (it synchronises the stream when it grows) and freed by tebgpu_destroy. */
+int32_t tebgpu_hsig_factors(tebgpu_ctx* ctx, const TebBatch* batch, const TebHsigFactors* factors);
+int32_t tebgpu_hsig_factors_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebHsigFactors* factors, void* cuda_stream);
+
+/* The output of tebgpu_h_signature (stride 2 for 2-D, stride max(M_cap, 1) for x-y-t, chosen by
+ * include_dynamic_obstacles) for every M_cap from 0 to max_obstacles (<= 16384). 2-D: A_l = f0(o_l) * Q_l from the
+ * factor table, factors == NULL builds the table in the same call (context scratch); x-y-t does not read factors. The
+ * per-band work is O(n M) and a band is split over CTAs of 256 obstacles; its sum does not depend on the batch around it.
+ * f0 is applied after the product instead of before it, so the 2-D values are not the bits of tebgpu_h_signature; both
+ * stay within 1e-12 sum_{k,l} |A_l| |L_kl| of the long double signature. tebgpu_h_signature_scenes: HOST buffers
+ * (factors too), checked as tebgpu_h_signature's, synchronous. tebgpu_h_signature_scenes_device: DEVICE buffers, stream
+ * ordered, does not synchronise; a band whose scene_id, n or scene obst_count is out of range (obst_count -1 from an
+ * overflowing tebgpu_costmap_obstacles_device) gets NaN in every output of its row, and so does a 2-D band whose
+ * scene's factor_count differs from obst_count (a table built for other rows). Calls of one context share its scratch:
+ * issue them on one stream. */
+int32_t tebgpu_h_signature_scenes(tebgpu_ctx* ctx, const TebBatch* batch, const TebHsigFactors* factors,
+                                  int32_t use_timediffs, double* h_out);
+int32_t tebgpu_h_signature_scenes_device(tebgpu_ctx* ctx, const TebBatch* batch, const TebHsigFactors* factors,
+                                         int32_t use_timediffs, double* h_out, void* cuda_stream);
+
 /* Number of kernels launched by the last optimize call (for bench.py's gpu_launches). */
 int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
 /* Introspection for measurement scripts. which: 0 speculation width used by the last optimize call, 1 kernel-A variant,

@@ -125,6 +125,15 @@ def load_library(build_if_missing=False):
     L.tebgpu_compute_cost.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebOptimizeArgs)]
     L.tebgpu_h_signature.restype = C.c_int32
     L.tebgpu_h_signature.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, C.c_int32]
+    L.tebgpu_hsig_factors.restype = C.c_int32
+    L.tebgpu_hsig_factors.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebHsigFactors)]
+    L.tebgpu_hsig_factors_device.restype = C.c_int32
+    L.tebgpu_hsig_factors_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebHsigFactors), vp]
+    L.tebgpu_h_signature_scenes.restype = C.c_int32
+    L.tebgpu_h_signature_scenes.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebHsigFactors), C.c_int32, vp]
+    L.tebgpu_h_signature_scenes_device.restype = C.c_int32
+    L.tebgpu_h_signature_scenes_device.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebHsigFactors), C.c_int32,
+                                                   vp, vp]
     L.tebgpu_build_system.restype = C.c_int32
     L.tebgpu_build_system.argtypes = [vp, C.POINTER(abi.TebBatch), C.c_int32, vp, vp, C.c_int32]
     L.tebgpu_build_system_graph.restype = C.c_int32
@@ -588,6 +597,47 @@ class TebGpu:
                     "tebgpu_h_signature")
         # the 2-D rows are (Re, Im) pairs: viewed, not composed as Re + 1j * Im, which turns an infinite Im into a NaN Re
         return out if three_d else out.view(np.complex128)[:, 0].copy()
+
+    def hsig_factors(self, hb):
+        """every scene's factor table of the 2-D signature (tebgpu_hsig_factors) from hb's obstacle tables:
+        (factor [S][M_cap][2] float64, factor_exp [S][M_cap] int32, factor_count [S] int32)"""
+        import numpy as np
+        f = (np.zeros((hb.S, hb.M_cap, 2)), np.zeros((hb.S, hb.M_cap), np.int32), np.zeros(hb.S, np.int32))
+        bs = hb.struct()
+        fs = abi.make_hsig_factors(*(x.ctypes.data for x in f))
+        self._check(self.lib.tebgpu_hsig_factors(self.ctx, C.byref(bs), C.byref(fs)), "tebgpu_hsig_factors")
+        return f
+
+    def h_signature_scenes(self, hb, factors=None, use_timediffs=True):
+        """h_signature for scenes of up to 16384 obstacles (tebgpu_h_signature_scenes), same return shapes. factors: the
+        tuple hsig_factors returned for hb's scenes, or None: the table is built in the call"""
+        import numpy as np
+        three_d = bool(self.params.include_dynamic_obstacles) if hasattr(self, "params") else False
+        out = np.zeros((hb.B, max(hb.M_cap, 1) if three_d else 2))
+        bs = hb.struct()
+        fs = None
+        if factors is not None:
+            f = [np.ascontiguousarray(x, dtype=dt) for x, dt in zip(factors, (np.float64, np.int32, np.int32))]
+            fs = C.byref(abi.make_hsig_factors(*(x.ctypes.data for x in f)))
+        self._check(self.lib.tebgpu_h_signature_scenes(self.ctx, C.byref(bs), fs, int(use_timediffs), out.ctypes.data),
+                    "tebgpu_h_signature_scenes")
+        return out if three_d else out.view(np.complex128)[:, 0].copy()
+
+    def hsig_factors_device(self, batch_struct, factors, stream=None):
+        """tebgpu_hsig_factors_device: the factor tables over DEVICE memory (batch_struct: an abi.TebBatch of device
+        pointers, of which S, M_cap, obstacles and obst_count are read; factors: an abi.TebHsigFactors of device
+        pointers). Stream ordered on `stream` (a cudaStream_t handle; None: the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_hsig_factors_device(self.ctx, C.byref(batch_struct), C.byref(factors), stream),
+                    "tebgpu_hsig_factors_device")
+
+    def h_signature_scenes_device(self, batch_struct, h_out, factors=None, use_timediffs=True, stream=None):
+        """tebgpu_h_signature_scenes_device: the signatures over DEVICE memory into h_out (a device address or a tensor
+        of B x 2 or B x max(M_cap, 1) float64). factors: an abi.TebHsigFactors of device pointers, or None: built in
+        the call. Stream ordered as hsig_factors_device; does not synchronise."""
+        out = h_out.data_ptr() if hasattr(h_out, "data_ptr") else h_out
+        fs = None if factors is None else C.byref(factors)
+        self._check(self.lib.tebgpu_h_signature_scenes_device(self.ctx, C.byref(batch_struct), fs, int(use_timediffs),
+                                                              out, stream), "tebgpu_h_signature_scenes_device")
 
     # ---- the one collective (NCCL all-gather of the per-candidate costs), behind the C-ABI
     def comm_get_unique_id(self, out128):

@@ -235,6 +235,20 @@ class TebFrameArgs(C.Structure):
                 ("custom_to_costmap", C.c_void_p), ("custom_vertices", C.c_void_p), ("obst_vertices", C.c_void_p)]
 
 
+class TebHsigFactors(C.Structure):
+    """Every scene's factor table of the 2-D H-signature (tebgpu_hsig_factors): factor [S][M_cap][2] float64, the
+    mantissa of Q_l = 1 / prod_j (o_l - o_j); factor_exp [S][M_cap] int32, its binary exponent (INT32_MIN for 0);
+    factor_count [S] int32, the obst_count the table was built at, or -1. Host or device pointers."""
+    _fields_ = [("factor", C.c_void_p), ("factor_exp", C.c_void_p), ("factor_count", C.c_void_p)]
+
+
+def make_hsig_factors(factor, factor_exp, factor_count) -> TebHsigFactors:
+    """TebHsigFactors with the arrays given as addresses (ints)"""
+    f = TebHsigFactors()
+    f.factor, f.factor_exp, f.factor_count = factor, factor_exp, factor_count
+    return f
+
+
 def make_frame_args(costmap_to_plan=None, plan_to_costmap=None, custom_to_costmap=None, custom_vertices=None,
                     obst_vertices=None, PV_cap=0) -> TebFrameArgs:
     """TebFrameArgs with the arrays given as addresses (ints, or None for NULL)"""

@@ -18,6 +18,7 @@
 #include "teb_solve_warp.cuh"
 #include "teb_solve_lat.cuh"
 #include "teb_hsig.cuh"
+#include "teb_hsig_scene.cuh"
 #include "teb_plan.cuh"
 #include "teb_feasible.cuh"
 #include "teb_costmap.cuh"
@@ -137,6 +138,10 @@ struct tebgpu_ctx {
   /* backup modes / finish cycle: the host-buffer entry points' arrays, staged in one buffer grown as above */
   char* d_cycle = nullptr; size_t cycle_bytes = 0;
   long long last_cycle_grid = 0;      /* grid in CTAs of the last k_backup_modes / k_finish_cycle launch */
+  /* scene H-signatures: the factor table's partial products, the in-call / uploaded factor table, the bands' chunk sums
+   * and the host-buffer entry point's output, each grown by the first call that needs more */
+  char* d_hsf_part = nullptr; char* d_hsf_tab = nullptr; double* d_hs_part = nullptr; double* d_hs_out = nullptr;
+  size_t hsf_part_bytes = 0, hsf_tab_bytes = 0, hs_part_bytes = 0, hs_out_bytes = 0;
   size_t smem_a = 0, smem_b = 0, smem_g = 0;
   /* profiling */
   bool profiling = false;
@@ -233,6 +238,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 10: return (int32_t)sizeof(TebCycleArgs);
     case 11: return (int32_t)sizeof(TebCostmapWorld);
     case 12: return (int32_t)sizeof(TebFrameArgs);
+    case 13: return (int32_t)sizeof(TebHsigFactors);
     default: return -1;
   }
 }
@@ -270,7 +276,8 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_status, c->d_iters, c->plan_status, c->d_start, c->d_goal, c->d_pcount, c->d_cmd, c->d_path,
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
-                  c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe};
+                  c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
+                  c->d_hs_part, c->d_hs_out};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -2159,6 +2166,153 @@ int32_t tebgpu_h_signature(tebgpu_ctx* ctx, const TebBatch* bt, int32_t use_time
     CUDA_TRY(ctx, cudaMemcpyAsync(h_out, d_out, (size_t)B * stride * sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
   }
+  return TEBGPU_OK;
+}
+
+/* argument checks of both factor-table entry points: only S, M_cap, obstacles and obst_count of the batch are read */
+static int32_t check_hsig_factors_args(tebgpu_ctx* ctx, const TebBatch* bt, const TebHsigFactors* f) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!bt || !f) { ctx->err = "batch or factors == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->S < 1 || bt->M_cap < 0) { ctx->err = "bad batch dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (bt->S > ctx->lim.max_scenes || bt->M_cap > ctx->lim.max_obstacles) { ctx->err = "batch exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+  if (!bt->obst_count || (bt->M_cap > 0 && !bt->obstacles)) { ctx->err = "missing required batch array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!f->factor || !f->factor_exp || !f->factor_count) { ctx->err = "missing factor table array"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_hsig_factors + k_hsig_factors_combine on device arrays, arguments already checked */
+static int32_t issue_hsig_factors(tebgpu_ctx* ctx, const TebBatch* d, const TebHsigFactors* f, cudaStream_t st) {
+  const int S = d->S, M_cap = d->M_cap, P_cap = hsig_parts(M_cap), lb = (M_cap + HSF_THREADS - 1) / HSF_THREADS;
+  const size_t cells = (size_t)S * P_cap * M_cap;
+  int32_t rc;
+  ctx->launches = 0;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_hsf_part, &ctx->hsf_part_bytes, cells * (sizeof(double2) + sizeof(int)) + 16, st))) return rc;
+  double2* pm = reinterpret_cast<double2*>(ctx->d_hsf_part);
+  int* pe = reinterpret_cast<int*>(pm + cells);
+  if (M_cap > 0) {
+    k_hsig_factors<<<dim3(S, lb * P_cap), HSF_THREADS, 0, st>>>(d->obstacles, d->obst_count, M_cap, pm, pe);
+    ++ctx->launches;
+  }
+  k_hsig_factors_combine<<<dim3(S, lb > 0 ? lb : 1), HSF_THREADS, 0, st>>>(d->obst_count, M_cap, pm, pe, f->factor,
+                                                                             f->factor_exp, f->factor_count);
+  ++ctx->launches;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+/* the in-call factor table of S x M_cap rows in ctx->d_hsf_tab */
+static int32_t hsig_table_scratch(tebgpu_ctx* ctx, int S, int M_cap, TebHsigFactors* t, cudaStream_t st) {
+  const size_t rows = (size_t)S * M_cap;
+  int32_t rc = grow_mirror(ctx, (void**)&ctx->d_hsf_tab, &ctx->hsf_tab_bytes,
+                           rows * 2 * sizeof(double) + rows * sizeof(int32_t) + (size_t)S * sizeof(int32_t) + 16, st);
+  if (rc) return rc;
+  t->factor = reinterpret_cast<double*>(ctx->d_hsf_tab);
+  t->factor_exp = reinterpret_cast<int32_t*>(t->factor + 2 * rows);
+  t->factor_count = t->factor_exp + rows;
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_hsig_factors_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebHsigFactors* factors, void* cuda_stream) {
+  const int32_t rc = check_hsig_factors_args(ctx, bt, factors);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_hsig_factors(ctx, bt, factors, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_hsig_factors(tebgpu_ctx* ctx, const TebBatch* bt, const TebHsigFactors* factors) {
+  int32_t rc = check_hsig_factors_args(ctx, bt, factors);
+  if (rc) return rc;
+  for (int sc = 0; sc < bt->S; ++sc)
+    if (bt->obst_count[sc] < 0 || bt->obst_count[sc] > bt->M_cap) { ctx->err = "obst_count[s] outside 0 .. M_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t S = bt->S, rows = S * bt->M_cap;
+  if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_obst, bt->obstacles, rows * sizeof(TebObstacle), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ocount, bt->obst_count, S * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  TebBatch d = *bt;
+  d.obstacles = ctx->d_obst; d.obst_count = ctx->d_ocount;
+  TebHsigFactors t{};
+  if ((rc = hsig_table_scratch(ctx, bt->S, bt->M_cap, &t, st))) return rc;
+  if ((rc = issue_hsig_factors(ctx, &d, &t, st))) return rc;
+  if (rows) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(factors->factor, t.factor, rows * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(factors->factor_exp, t.factor_exp, rows * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  }
+  CUDA_TRY(ctx, cudaMemcpyAsync(factors->factor_count, t.factor_count, S * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* the signatures of every band of d (device arrays, batch checked); f: a device factor table, or NULL: built here */
+static int32_t issue_hsig_scenes(tebgpu_ctx* ctx, const TebBatch* d, const TebHsigFactors* f, int32_t use_timediffs,
+                                 double* out, cudaStream_t st) {
+  DevBatch db = make_devbatch(ctx, d);
+  KParams kp = make_kparams(ctx, d, 1.0);
+  const int B = d->B, Mc = d->M_cap > 0 ? d->M_cap : 1;
+  int32_t rc;
+  if (ctx->params.include_dynamic_obstacles) { /* homotopy_class_planner.hpp:50 */
+    const size_t smem = (size_t)3 * d->n_cap * sizeof(double);
+    k_hsig3d_scene<<<dim3(B, (Mc + HS3_ROWS - 1) / HS3_ROWS), 256, smem, st>>>(db, kp, use_timediffs, out);
+    ctx->launches = 1;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return TEBGPU_OK;
+  }
+  TebHsigFactors t{};
+  int64_t launches = 0;
+  if (!f) {
+    if ((rc = hsig_table_scratch(ctx, d->S, d->M_cap, &t, st))) return rc;
+    if ((rc = issue_hsig_factors(ctx, d, &t, st))) return rc;
+    launches = ctx->launches;
+    f = &t;
+  }
+  const int C_cap = (Mc + HS2_ROWS - 1) / HS2_ROWS;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_hs_part, &ctx->hs_part_bytes, (size_t)B * C_cap * 3 * sizeof(double), st))) return rc;
+  const size_t smem = (size_t)2 * d->n_cap * sizeof(double);
+  k_hsig2d_scene<<<dim3(B, C_cap), HS2_ROWS, smem, st>>>(db, kp, f->factor, f->factor_exp, f->factor_count, ctx->d_hs_part);
+  k_hsig2d_scene_sum<<<(B + 127) / 128, 128, 0, st>>>(db, f->factor_count, ctx->d_hs_part, out);
+  ctx->launches = launches + 2;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_h_signature_scenes_device(tebgpu_ctx* ctx, const TebBatch* bt, const TebHsigFactors* factors,
+                                         int32_t use_timediffs, double* h_out, void* cuda_stream) {
+  int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  if (!h_out) { ctx->err = "h_out == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (factors && (!factors->factor || !factors->factor_exp || !factors->factor_count)) { ctx->err = "missing factor table array"; return TEBGPU_ERR_INVALID_ARG; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_hsig_scenes(ctx, bt, factors, use_timediffs, h_out, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_h_signature_scenes(tebgpu_ctx* ctx, const TebBatch* bt, const TebHsigFactors* factors,
+                                  int32_t use_timediffs, double* h_out) {
+  int32_t rc = check_batch(ctx, bt);
+  if (rc) return rc;
+  if (!h_out) { ctx->err = "h_out == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  const bool three_d = ctx->params.include_dynamic_obstacles != 0;
+  if (factors && !three_d && (!factors->factor || !factors->factor_exp || !factors->factor_count)) { ctx->err = "missing factor table array"; return TEBGPU_ERR_INVALID_ARG; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = upload_batch(ctx, bt))) return rc;
+  const TebBatch d = mirror_batch(ctx, bt);
+  cudaStream_t st = ctx->stream;
+  TebHsigFactors t{};
+  const TebHsigFactors* f = nullptr;
+  if (factors && !three_d) { /* the caller's table goes up into the in-call table's place */
+    const size_t S = bt->S, rows = S * bt->M_cap;
+    if ((rc = hsig_table_scratch(ctx, bt->S, bt->M_cap, &t, st))) return rc;
+    if (rows) {
+      CUDA_TRY(ctx, cudaMemcpyAsync(t.factor, factors->factor, rows * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(ctx, cudaMemcpyAsync(t.factor_exp, factors->factor_exp, rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    }
+    CUDA_TRY(ctx, cudaMemcpyAsync(t.factor_count, factors->factor_count, S * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    f = &t;
+  }
+  const size_t stride = three_d ? (size_t)(bt->M_cap > 0 ? bt->M_cap : 1) : 2, bytes = (size_t)bt->B * stride * sizeof(double);
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_hs_out, &ctx->hs_out_bytes, bytes, st))) return rc;
+  if ((rc = issue_hsig_scenes(ctx, &d, f, use_timediffs, ctx->d_hs_out, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(h_out, ctx->d_hs_out, bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
 }
 
