@@ -643,7 +643,7 @@ typedef struct TebCycleArgs {
 
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
- * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs. */
+ * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs, 13 TebHsigFactors, 14 TebFleetArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -800,6 +800,76 @@ int32_t tebgpu_backup_modes_device(tebgpu_ctx* ctx, const TebBatch* batch, const
 int32_t tebgpu_finish_cycle(tebgpu_ctx* ctx, TebBatch* batch, const TebCycleArgs* args);
 int32_t tebgpu_finish_cycle_device(tebgpu_ctx* ctx, TebBatch* batch, const TebCycleArgs* args, void* cuda_stream);
 
+/* The other robots of a fleet as custom obstacle rows of every robot's scene (tebgpu_fleet_obstacles): what a
+ * multi-robot publisher sends on the custom obstacle topic, one circle with a velocity per robot, read the way
+ * TebLocalPlannerROS::updateObstacleContainerWithCustomObstacles reads a circle message (teb_local_planner_ros.cpp:576-581,
+ * setCentroidVelocity obstacles.h:214-233). It runs between tebgpu_finish_cycle of one cycle and
+ * tebgpu_costmap_obstacles(_tf) of the next, so custom and custom_count are the TebCostmapArgs arrays of the next
+ * conversion. HOST pointers for tebgpu_fleet_obstacles, DEVICE pointers for tebgpu_fleet_obstacles_device.
+ *
+ * Robot r has the pose (x, y, theta) = pose[r] in one common frame, the frame of the custom obstacles (usually map);
+ * the body-frame command (vx, vy) = last_cmd[r] (TebCycleArgs.last_cmd, whose omega is not read); radius rho = radius[r];
+ * world w = world[r] (NULL: one world); scene s = scene[r] (NULL: s = r). Every product and sum is rounded on its own
+ * (no FMA contraction).
+ *   1. Neighbours (defined here): q is a neighbour of r when q != r, world[q] == world[r] and dx * dx + dy * dy <=
+ *      range * range (dx = x_q - x_r, dy = y_q - y_r). Coincident robots are neighbours; a NaN distance is not.
+ *      needed[r] = the number of neighbours. They are ordered by (d2, q): nearest first, a tie to the lower index.
+ *   2. Rows: the first written = min(needed, max_rows, C_cap - own) neighbours (own = own_count[s], 0 for NULL) go to
+ *      custom[s][own .. own + written), in order. Neighbour q gives {x_q, y_q, vx, vy, rho_q, dynamic, TEB_OBST_CIRCULAR,
+ *      0, 0, _pad 0}: the publisher's map-frame velocity (vx, vy) = R(theta_q) (cmd vx, cmd vy), i.e. (c vx - s vy,
+ *      s vx + c vy) with c = cos(theta_q), s = sin(theta_q); then setCentroidVelocity's rule, taken of the body command
+ *      whose norm the rotation keeps (so that no decision depends on sin / cos): sqrt(cmd vx * cmd vx + cmd vy * cmd vy)
+ *      < 0.001 gives dynamic 0 and velocity (0, 0), otherwise dynamic 1 with (vx, vy). The rows move with the other custom
+ *      rows under TebFrameArgs.custom_to_costmap; velocities are not rotated there (TebFrameArgs).
+ *   3. custom_count[s] = own + written. Rows custom[s][0 .. own) and past own + written are not touched, so a second
+ *      call with the same inputs writes the same bytes: own_count holds the caller's own rows and must not be
+ *      custom_count.
+ *   4. status[r] = TEB_FLEET_WRITTEN, or TEB_FLEET_TRUNCATED when written < needed[r] (max_rows or C_cap cut the list;
+ *      the nearest neighbours are the ones kept).
+ * sin and cos are the device's (velocities within ~1e-16 relative of the correctly rounded ones); every decision,
+ * position, radius and the order are exact.
+ *
+ * Argument errors return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit) before anything is launched: NULL
+ * args or a required array (pose, last_cmd, radius, custom_count; custom when C_cap > 0), R outside 1 .. max_bands, S
+ * outside 1 .. max_scenes, C_cap < 0, max_rows outside 0 .. TEB_FLEET_MAX_ROWS, a NaN or negative range, scene == NULL
+ * with R > S, own_count == custom_count, a custom pointer that is not 16-byte aligned. tebgpu_fleet_obstacles: HOST
+ * buffers, synchronous; it also refuses a non-finite pose or command, a radius that is negative or not finite, a scene
+ * outside 0 .. S - 1, an own_count outside 0 .. C_cap, and two robots in one scene; its device copies are allocated by
+ * the first call that needs them. tebgpu_fleet_obstacles_device: DEVICE buffers, stream ordered as
+ * tebgpu_optimize_batch_device, does not synchronise; a robot whose scene is outside 0 .. S - 1 or whose own_count is
+ * outside 0 .. C_cap gets TEB_FLEET_BAD_INPUT, one whose scene another robot also maps to gets TEB_FLEET_SHARED_SCENE;
+ * either has needed = -1 and nothing written to its scene. Such robots are still neighbours of the others. The shared
+ * scene check takes context scratch of S int32 (allocated by the first call that needs it, which synchronises the
+ * stream); calls of one context share it, so issue them on one stream.
+ *
+ * One warp per robot, FLEET_WARPS robots per CTA: the CTA stages the fleet's (x, y, world) in shared-memory tiles, the
+ * lanes test the candidates, and the warp keeps its top-max_rows list in registers, one slot per lane
+ * (tebgpu_get_info key 18: the grid in CTAs). All pairs are tested: O(R^2), exact and deterministic. */
+#define TEB_FLEET_MAX_ROWS 32
+#define TEB_FLEET_WRITTEN       0  /* every neighbour in range written */
+#define TEB_FLEET_TRUNCATED     1  /* written < needed: max_rows or C_cap - own_count kept the nearest ones */
+#define TEB_FLEET_BAD_INPUT     2  /* device entry point only: scene or own_count out of range; nothing written */
+#define TEB_FLEET_SHARED_SCENE  3  /* device entry point only: another robot maps to the same scene; nothing written */
+typedef struct TebFleetArgs {
+  int32_t  R;                 /* robots, 1 .. max_bands */
+  int32_t  S;                 /* scenes (rows of custom_count), 1 .. max_scenes */
+  int32_t  C_cap;             /* custom rows per scene (stride of custom, as TebCostmapArgs.C_cap), >= 0 */
+  int32_t  max_rows;          /* neighbour rows per robot, 0 .. TEB_FLEET_MAX_ROWS */
+  double   range;             /* neighbour distance, >= 0 (inf: every robot of the world) */
+  const double*  pose;        /* [R][3] x, y, theta in the custom obstacles' frame */
+  const double*  last_cmd;    /* [R][3] body-frame vx, vy, omega (TebCycleArgs.last_cmd); omega is not read */
+  const double*  radius;      /* [R] the circle each robot is published as */
+  const int32_t* world;       /* [R] or NULL: one world */
+  const int32_t* scene;       /* [R] or NULL: robot r writes scene r */
+  const int32_t* own_count;   /* [S] or NULL: the caller's own custom rows of each scene (0 for NULL) */
+  TebObstacle*   custom;      /* [S][C_cap] in/out: TebCostmapArgs.custom, 16-byte aligned */
+  int32_t*       custom_count;/* [S] out: TebCostmapArgs.custom_count; only the scenes of valid robots are written */
+  int32_t*       needed;      /* [R] out or NULL: neighbours in range, -1 for a robot answered with BAD_INPUT / SHARED */
+  int32_t*       status;      /* [R] out or NULL: TEB_FLEET_* */
+} TebFleetArgs;
+int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* args);
+int32_t tebgpu_fleet_obstacles_device(tebgpu_ctx* ctx, const TebFleetArgs* args, void* cuda_stream);
+
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded
  *   LDL^T with the active window in registers, and the accept / reject chain is replayed in order;
@@ -918,7 +988,8 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * first), 15 grid in CTAs of the last costmap conversion (k_costmap_obstacles, one CTA per scene; 0 before the first),
  * 16 grid in CTAs of the last local-plan launch (k_local_plan, 4 bands per CTA; 0 before the first), 17 grid in CTAs
  * of the last backup-modes or finish-cycle launch (k_backup_modes / k_finish_cycle, 128 bands per CTA; 0 before the
- * first).
+ * first), 18 grid in CTAs of the last fleet-obstacle launch (k_fleet_obstacles, FLEET_WARPS robots per CTA; 0 before
+ * the first).
  * Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */

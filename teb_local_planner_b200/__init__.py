@@ -87,6 +87,10 @@ def load_library(build_if_missing=False):
         getattr(L, name).argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebCycleArgs)]
         getattr(L, name + "_device").restype = C.c_int32
         getattr(L, name + "_device").argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebCycleArgs), vp]
+    L.tebgpu_fleet_obstacles.restype = C.c_int32
+    L.tebgpu_fleet_obstacles.argtypes = [vp, C.POINTER(abi.TebFleetArgs)]
+    L.tebgpu_fleet_obstacles_device.restype = C.c_int32
+    L.tebgpu_fleet_obstacles_device.argtypes = [vp, C.POINTER(abi.TebFleetArgs), vp]
     L.tebgpu_get_plan_kernel_times.restype = C.c_int32
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
@@ -154,7 +158,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
     for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
                                 abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs,
-                                abi.TebLocalPlanArgs, abi.TebCycleArgs, abi.TebCostmapWorld)):
+                                abi.TebLocalPlanArgs, abi.TebCycleArgs, abi.TebCostmapWorld, abi.TebFrameArgs,
+                                abi.TebHsigFactors, abi.TebFleetArgs)):
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -533,6 +538,44 @@ class TebGpu:
         and chi2 are read; n is written). Stream ordered as backup_modes_device; does not synchronise."""
         self._check(self.lib.tebgpu_finish_cycle_device(self.ctx, C.byref(batch_struct), C.byref(args), stream),
                     "tebgpu_finish_cycle_device")
+
+    def fleet_obstacles(self, pose, last_cmd, radius, custom, range, max_rows=8, own_count=None, custom_count=None,
+                        world=None, scene=None):
+        """The other robots of the fleet as custom obstacle rows of every robot's scene (tebgpu_fleet_obstacles), host
+        buffers: pose [R][3] (x, y, theta in the custom obstacles' frame), last_cmd [R][3] (body vx, vy, omega: the
+        controller state's last_cmd), radius [R], custom [S][C_cap] abi.OBST_DTYPE (the caller's own rows first),
+        own_count [S] (None: 0), custom_count [S] (None: own_count; scenes no robot writes keep it), world / scene [R]
+        (None: one world / scene r). Returns (custom [S][C_cap], a new array with the neighbour rows after each scene's
+        own ones, custom_count [S], needed [R], status [R] TEB_FLEET_*)."""
+        import numpy as np
+        pose = np.ascontiguousarray(pose, dtype=np.float64).reshape(-1, 3)
+        R = pose.shape[0]
+        f64 = lambda x, shape: np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.float64)
+        i32 = lambda x, shape: None if x is None else np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.int32)
+        out = np.array(custom, dtype=abi.OBST_DTYPE, order="C")
+        S = out.shape[0]
+        out = out.reshape(S, -1)
+        own = i32(own_count, (S,))
+        cc = (np.zeros(S, np.int32) if own is None else own.copy()) if custom_count is None else i32(custom_count, (S,)).copy()
+        keep = dict(cmd=f64(last_cmd, (R, 3)), rad=f64(radius, (R,)), world=i32(world, (R,)), scene=i32(scene, (R,)))
+        needed, status = np.full(R, -2, np.int32), np.full(R, -1, np.int32)
+        fa = abi.make_fleet_args(R, S, out.shape[1], max_rows, range, pose=pose, last_cmd=keep["cmd"], radius=keep["rad"],
+                                 world=keep["world"], scene=keep["scene"], own_count=own,
+                                 custom=out if out.size else None, custom_count=cc, needed=needed, status=status)
+        self._check(self.lib.tebgpu_fleet_obstacles(self.ctx, C.byref(fa)), "tebgpu_fleet_obstacles")
+        return out, cc, needed, status
+
+    def fleet_obstacles_device(self, args, stream=None):
+        """tebgpu_fleet_obstacles_device: the same step over DEVICE memory (args: an abi.TebFleetArgs of device
+        pointers, see abi.make_fleet_args, which takes the fleet loop's tensors: the robot poses, the cycle state's
+        last_cmd, and the costmap conversion's custom / custom_count). Stream ordered on `stream` (a cudaStream_t handle;
+        None: the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_fleet_obstacles_device(self.ctx, C.byref(args), stream),
+                    "tebgpu_fleet_obstacles_device")
+
+    def last_fleet_grid(self):
+        """grid in CTAs (16 robots each) of the last fleet-obstacle launch, 0 before the first"""
+        return self.info(18)
 
     def last_cycle_grid(self):
         """grid in CTAs (128 bands each) of the last backup-modes or finish-cycle launch, 0 before the first"""

@@ -333,6 +333,38 @@ def make_cycle_state(B, L_cap=50):
                 osc_fill=np.zeros((B, 2), np.int32))
 
 
+class TebFleetArgs(C.Structure):
+    """The other robots of a fleet as custom obstacle rows of every robot's scene (tebgpu_fleet_obstacles): the robots'
+    poses [R][3], body commands [R][3] (TebCycleArgs.last_cmd), radii [R], optional worlds / scenes [R], each scene's
+    own custom rows [S], and the custom rows / counts written, as host or device pointers"""
+    _fields_ = [("R", _i), ("S", _i), ("C_cap", _i), ("max_rows", _i), ("range", _d), ("pose", C.c_void_p),
+                ("last_cmd", C.c_void_p), ("radius", C.c_void_p), ("world", C.c_void_p), ("scene", C.c_void_p),
+                ("own_count", C.c_void_p), ("custom", C.c_void_p), ("custom_count", C.c_void_p), ("needed", C.c_void_p),
+                ("status", C.c_void_p)]
+
+
+TEB_FLEET_MAX_ROWS = 32
+# TEB_FLEET_*: what tebgpu_fleet_obstacles did for a robot
+TEB_FLEET_WRITTEN, TEB_FLEET_TRUNCATED, TEB_FLEET_BAD_INPUT, TEB_FLEET_SHARED_SCENE = range(4)
+
+
+def make_fleet_args(R, S, C_cap, max_rows, range, **arrays) -> TebFleetArgs:
+    """TebFleetArgs with the sizes set and the arrays given by keyword (pose=..., last_cmd=..., ...) as addresses (ints),
+    torch tensors (their data_ptr()), numpy arrays (their buffer; keep them alive) or None for NULL"""
+    a = TebFleetArgs()
+    a.R, a.S, a.C_cap, a.max_rows, a.range = int(R), int(S), int(C_cap), int(max_rows), float(range)
+    names = {f[0] for f in TebFleetArgs._fields_[5:]}
+    for k, v in arrays.items():
+        if k not in names:
+            raise TypeError(f"unknown TebFleetArgs array {k}")
+        if hasattr(v, "data_ptr"):
+            v = v.data_ptr()
+        elif isinstance(v, np.ndarray):
+            v = ptr(v)
+        setattr(a, k, v)
+    return a
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

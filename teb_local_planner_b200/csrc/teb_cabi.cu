@@ -24,6 +24,7 @@
 #include "teb_costmap.cuh"
 #include "teb_local_plan.cuh"
 #include "teb_cycle.cuh"
+#include "teb_fleet.cuh"
 #include "teb_comm.h"
 #include <cstdlib>
 
@@ -138,6 +139,11 @@ struct tebgpu_ctx {
   /* backup modes / finish cycle: the host-buffer entry points' arrays, staged in one buffer grown as above */
   char* d_cycle = nullptr; size_t cycle_bytes = 0;
   long long last_cycle_grid = 0;      /* grid in CTAs of the last k_backup_modes / k_finish_cycle launch */
+  /* fleet obstacles: the robots per scene of the shared-scene check, and the host-buffer entry point's arrays, staged in
+   * one buffer; each grown by the first call that needs more */
+  int32_t* d_fclaim = nullptr; size_t fclaim_bytes = 0;
+  char* d_fleet = nullptr; size_t fleet_bytes = 0;
+  long long last_fleet_grid = 0;      /* grid in CTAs of the last k_fleet_obstacles launch */
   /* scene H-signatures: the factor table's partial products, the in-call / uploaded factor table, the bands' chunk sums
    * and the host-buffer entry point's output, each grown by the first call that needs more */
   char* d_hsf_part = nullptr; char* d_hsf_tab = nullptr; double* d_hs_part = nullptr; double* d_hs_out = nullptr;
@@ -239,6 +245,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 11: return (int32_t)sizeof(TebCostmapWorld);
     case 12: return (int32_t)sizeof(TebFrameArgs);
     case 13: return (int32_t)sizeof(TebHsigFactors);
+    case 14: return (int32_t)sizeof(TebFleetArgs);
     default: return -1;
   }
 }
@@ -266,6 +273,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 15: return ctx->last_costmap_grid;
     case 16: return ctx->last_lplan_grid;
     case 17: return ctx->last_cycle_grid;
+    case 18: return ctx->last_fleet_grid;
     default: return -1;
   }
 }
@@ -277,7 +285,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
                   c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
-                  c->d_hs_part, c->d_hs_out};
+                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -2099,6 +2107,103 @@ int32_t tebgpu_backup_modes(tebgpu_ctx* ctx, const TebBatch* bt, const TebCycleA
 
 int32_t tebgpu_finish_cycle(tebgpu_ctx* ctx, TebBatch* bt, const TebCycleArgs* ca) {
   return run_cycle_host(ctx, bt, ca, true);
+}
+
+/* argument checks of both fleet-obstacle entry points: nothing is launched when one fails */
+static int32_t check_fleet_args(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!fa) { ctx->err = "fleet args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fa->R < 1 || fa->S < 1 || fa->C_cap < 0) { ctx->err = "bad fleet dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fa->R > ctx->lim.max_bands || fa->S > ctx->lim.max_scenes) { ctx->err = "fleet exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+  if (fa->max_rows < 0 || fa->max_rows > TEB_FLEET_MAX_ROWS) { ctx->err = "max_rows outside 0 .. TEB_FLEET_MAX_ROWS"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!(fa->range >= 0.0)) { ctx->err = "range is NaN or negative"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!fa->pose || !fa->last_cmd || !fa->radius || !fa->custom_count || (fa->C_cap > 0 && !fa->custom)) {
+    ctx->err = "missing required fleet array"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  if (!fa->scene && fa->R > fa->S) { ctx->err = "scene == NULL with R > S"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fa->own_count && (const void*)fa->own_count == (const void*)fa->custom_count) {
+    ctx->err = "own_count is custom_count"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  if (reinterpret_cast<uintptr_t>(fa->custom) & 15) { ctx->err = "custom not 16-byte aligned"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_fleet_claim (when scenes are given) and k_fleet_obstacles on arguments already checked */
+static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st) {
+  int32_t rc;
+  const int32_t* claims = nullptr;
+  if (fa->scene) {
+    if ((rc = grow_mirror(ctx, (void**)&ctx->d_fclaim, &ctx->fclaim_bytes, (size_t)fa->S * sizeof(int32_t), st))) return rc;
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_fclaim, 0, (size_t)fa->S * sizeof(int32_t), st));
+    k_fleet_claim<<<(unsigned)((fa->R + CLAIM_THREADS - 1) / CLAIM_THREADS), CLAIM_THREADS, 0, st>>>(*fa, ctx->d_fclaim);
+    claims = ctx->d_fclaim;
+  }
+  const long long grid = ((long long)fa->R + FLEET_WARPS - 1) / FLEET_WARPS;
+  k_fleet_obstacles<<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims);
+  ctx->last_fleet_grid = grid;
+  ctx->launches = fa->scene ? 2 : 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_obstacles_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, void* cuda_stream) {
+  const int32_t rc = check_fleet_args(ctx, fa);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_fleet(ctx, fa, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
+  int32_t rc = check_fleet_args(ctx, fa);
+  if (rc) return rc;
+  const size_t R = fa->R, S = fa->S, C = fa->C_cap;
+  /* the robots the device entry point would answer with BAD_INPUT / SHARED_SCENE, and every non-finite input, are
+   * refused here, before anything runs */
+  std::vector<char> taken(S, 0);
+  for (size_t r = 0; r < R; ++r) {
+    const double* p = fa->pose + 3 * r;
+    const double* c = fa->last_cmd + 3 * r;
+    if (!std::isfinite(p[0]) || !std::isfinite(p[1]) || !std::isfinite(p[2])) { ctx->err = "pose[r] not finite"; return TEBGPU_ERR_INVALID_ARG; }
+    if (!std::isfinite(c[0]) || !std::isfinite(c[1])) { ctx->err = "last_cmd[r] not finite"; return TEBGPU_ERR_INVALID_ARG; }
+    if (!std::isfinite(fa->radius[r]) || fa->radius[r] < 0.0) { ctx->err = "radius[r] negative or not finite"; return TEBGPU_ERR_INVALID_ARG; }
+    const int32_t s = fa->scene ? fa->scene[r] : (int32_t)r;
+    if (s < 0 || (size_t)s >= S) { ctx->err = "scene[r] outside 0 .. S-1"; return TEBGPU_ERR_INVALID_ARG; }
+    if (taken[s]) { ctx->err = "two robots in one scene"; return TEBGPU_ERR_INVALID_ARG; }
+    taken[s] = 1;
+    const int32_t own = fa->own_count ? fa->own_count[s] : 0;
+    if (own < 0 || (size_t)own > C) { ctx->err = "own_count[s] outside 0 .. C_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t I = sizeof(int32_t), D = sizeof(double);
+  enum { POSE, CMD, RAD, WORLD, SCENE, OWN, CUSTOM, CCOUNT, NEED, STATUS, SLOTS };
+  CycleSlot sl[SLOTS] = {
+      {(void*)fa->pose, R * 3 * D, false, 0},      {(void*)fa->last_cmd, R * 3 * D, false, 0},
+      {(void*)fa->radius, R * D, false, 0},        {(void*)fa->world, R * I, false, 0},
+      {(void*)fa->scene, R * I, false, 0},         {(void*)fa->own_count, S * I, false, 0},
+      {fa->custom, S * C * sizeof(TebObstacle), true, 0}, {fa->custom_count, S * I, true, 0},
+      {fa->needed, R * I, true, 0},                {fa->status, R * I, true, 0}};
+  size_t off = 0;
+  for (CycleSlot& c : sl) {
+    c.off = off;
+    if (c.host) off += (c.bytes + 255) & ~(size_t)255;
+  }
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_fleet, &ctx->fleet_bytes, off, st))) return rc;
+  char* d = ctx->d_fleet;
+  /* the outputs go up too, so what the step leaves unwritten comes back as the caller left it */
+  for (const CycleSlot& c : sl)
+    if (c.host && c.bytes) CUDA_TRY(ctx, cudaMemcpyAsync(d + c.off, c.host, c.bytes, cudaMemcpyHostToDevice, st));
+  TebFleetArgs da = *fa;
+  da.pose = (const double*)sl[POSE].dev(d); da.last_cmd = (const double*)sl[CMD].dev(d);
+  da.radius = (const double*)sl[RAD].dev(d); da.world = (const int32_t*)sl[WORLD].dev(d);
+  da.scene = (const int32_t*)sl[SCENE].dev(d); da.own_count = (const int32_t*)sl[OWN].dev(d);
+  da.custom = (TebObstacle*)sl[CUSTOM].dev(d); da.custom_count = (int32_t*)sl[CCOUNT].dev(d);
+  da.needed = (int32_t*)sl[NEED].dev(d); da.status = (int32_t*)sl[STATUS].dev(d);
+  if ((rc = issue_fleet(ctx, &da, st))) return rc;
+  for (const CycleSlot& c : sl)
+    if (c.host && c.out && c.bytes) CUDA_TRY(ctx, cudaMemcpyAsync(c.host, d + c.off, c.bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
 }
 
 int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args) {
