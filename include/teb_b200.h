@@ -643,7 +643,8 @@ typedef struct TebCycleArgs {
 
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
- * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs, 13 TebHsigFactors, 14 TebFleetArgs. */
+ * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs, 13 TebHsigFactors, 14 TebFleetArgs,
+ * 15 TebFleetRow, 16 TebFleetTable. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -869,6 +870,71 @@ typedef struct TebFleetArgs {
 } TebFleetArgs;
 int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* args);
 int32_t tebgpu_fleet_obstacles_device(tebgpu_ctx* ctx, const TebFleetArgs* args, void* cuda_stream);
+
+/* The fleet table: every robot of a fleet as the row it is published as, shared by the contexts and ranks that hold the
+ * fleet's robots, so that each robot gets the robots of other contexts (another robot kind, another TebParams) and of
+ * other GPUs as neighbour rows. A cycle runs, between tebgpu_finish_cycle and tebgpu_costmap_obstacles(_tf):
+ *   1. tebgpu_fleet_publish: every owner writes its R robots as rows first .. first + R - 1 of the table;
+ *   2. sharing: one table in one GPU's memory that every context writes (contexts ordered by one stream or by events),
+ *      or tebgpu_fleet_gather across the ranks of a communicator (tebgpu_comm_init), one ncclAllGather of 64 T bytes;
+ *   3. tebgpu_fleet_obstacles_table: every owner runs TebFleetArgs' step for its R robots with the candidates taken from
+ *      all T rows of the table.
+ * When the owners' robots are contiguous shards of one global robot order (owner g's robot i is global robot
+ * first_g + i - pad_g, padding rows only between shards), the key (d2, table row) orders the candidates as (d2, global
+ * index) does, so the outputs are bit for bit those of one tebgpu_fleet_obstacles call over the whole fleet.
+ *
+ * TebFleetRow: robot q as published. The position, velocity, dynamic flag and radius are those of the custom row
+ * TebFleetArgs step 2 writes for q: (vx, vy) = R(theta_q) (cmd vx, cmd vy), (0, 0) with dynamic 0 when the body command's
+ * norm is below 0.001. live == 0 marks padding, which is never a neighbour; _pad is written as 0. 64 bytes. */
+typedef struct TebFleetRow {
+  double  x, y;               /* position in the custom obstacles' frame */
+  double  vx, vy;             /* map-frame velocity after the 0.001 rule */
+  double  radius;             /* the circle the robot is published as */
+  int32_t world;              /* TebFleetArgs.world (0 when that is NULL) */
+  int32_t dynamic;            /* 1 moving, 0 still */
+  int32_t live;               /* 1 a robot, 0 padding */
+  int32_t _pad[3];
+} TebFleetRow;
+
+typedef struct TebFleetTable {
+  int32_t      T;             /* rows of the table, >= 1 */
+  int32_t      first;         /* this call's robots are rows first .. first + R - 1 */
+  TebFleetRow* rows;          /* [T], 16-byte aligned; HOST or DEVICE as the entry point says */
+} TebFleetTable;
+
+/* tebgpu_fleet_publish(_device): rows[first + r] = robot r, r < args->R, from args->pose, last_cmd, radius and world
+ * (NULL: world 0), with live = 1; no other field of args is read and no other row is written. The velocity and the
+ * dynamic flag come from the same device function as tebgpu_fleet_obstacles' rows. One thread per robot.
+ *
+ * tebgpu_fleet_gather(_device): the in-place all-gather of a table of T = world * cap rows over the context's
+ * communicator: rank g contributes rows [g cap, (g + 1) cap) and every rank ends with all T rows. NCCL has no
+ * all-gather-v, so shards of fewer robots are padded to cap with live = 0 rows (the caller's, written once). Without a
+ * communicator (one rank) it does nothing. table->first is not read. Stream ordered on the context's stream (_device,
+ * or cuda_stream when given), or synchronous on host rows.
+ *
+ * tebgpu_fleet_obstacles_table(_device): TebFleetArgs' step for the call's R robots (robot r is table row first + r),
+ * the candidates being all T rows of the table: q is a neighbour of r when q != first + r, rows[q].live, rows[q].world
+ * == rows[first + r].world and the distance rule holds; they are ordered by (d2, q) and each is written as its row
+ * ({x, y, vx, vy, radius, dynamic} of the row, TEB_OBST_CIRCULAR, 0, 0, _pad 0}). The robot's position and world are
+ * those of its own row; pose, last_cmd, radius and world of args are not read (may be NULL). scene, own_count, custom,
+ * custom_count, needed, status, the cuts and the shared-scene check are TebFleetArgs'. On the device, a robot whose own
+ * row is not live gets TEB_FLEET_BAD_INPUT (needed -1, nothing written); the host entry point refuses it, and refuses a
+ * live row whose x, y, vx, vy or radius is not finite or whose radius is negative. tebgpu_get_info key 18 reports the
+ * grid of its k_fleet_obstacles launch.
+ *
+ * Argument errors return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit) before anything is launched: those
+ * of TebFleetArgs for the arrays each step reads, NULL table or rows, T < 1, first < 0, first + R > T, rows not 16-byte
+ * aligned; in the gather cap < 1 or T != world * cap. The host forms take HOST rows (and HOST args arrays) and
+ * synchronise; their device copies are allocated by the first call that needs them. The _device forms take DEVICE
+ * pointers, are stream ordered as tebgpu_optimize_batch_device and do not synchronise. */
+int32_t tebgpu_fleet_publish(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetTable* table);
+int32_t tebgpu_fleet_publish_device(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetTable* table,
+                                    void* cuda_stream);
+int32_t tebgpu_fleet_gather(tebgpu_ctx* ctx, const TebFleetTable* table, int32_t cap);
+int32_t tebgpu_fleet_gather_device(tebgpu_ctx* ctx, const TebFleetTable* table, int32_t cap, void* cuda_stream);
+int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetTable* table);
+int32_t tebgpu_fleet_obstacles_table_device(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetTable* table,
+                                            void* cuda_stream);
 
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded

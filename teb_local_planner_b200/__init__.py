@@ -91,6 +91,15 @@ def load_library(build_if_missing=False):
     L.tebgpu_fleet_obstacles.argtypes = [vp, C.POINTER(abi.TebFleetArgs)]
     L.tebgpu_fleet_obstacles_device.restype = C.c_int32
     L.tebgpu_fleet_obstacles_device.argtypes = [vp, C.POINTER(abi.TebFleetArgs), vp]
+    for name in ("tebgpu_fleet_publish", "tebgpu_fleet_obstacles_table"):
+        getattr(L, name).restype = C.c_int32
+        getattr(L, name).argtypes = [vp, C.POINTER(abi.TebFleetArgs), C.POINTER(abi.TebFleetTable)]
+        getattr(L, name + "_device").restype = C.c_int32
+        getattr(L, name + "_device").argtypes = [vp, C.POINTER(abi.TebFleetArgs), C.POINTER(abi.TebFleetTable), vp]
+    L.tebgpu_fleet_gather.restype = C.c_int32
+    L.tebgpu_fleet_gather.argtypes = [vp, C.POINTER(abi.TebFleetTable), C.c_int32]
+    L.tebgpu_fleet_gather_device.restype = C.c_int32
+    L.tebgpu_fleet_gather_device.argtypes = [vp, C.POINTER(abi.TebFleetTable), C.c_int32, vp]
     L.tebgpu_get_plan_kernel_times.restype = C.c_int32
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
@@ -156,10 +165,15 @@ def load_library(build_if_missing=False):
     L.tebgpu_select_best.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double]
     L.tebgpu_auto_resize_host.restype = C.c_int32
     L.tebgpu_auto_resize_host.argtypes = [vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
-    for which, st in enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
+    for which, st in tuple(enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
                                 abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs,
                                 abi.TebLocalPlanArgs, abi.TebCycleArgs, abi.TebCostmapWorld, abi.TebFrameArgs,
-                                abi.TebHsigFactors, abi.TebFleetArgs)):
+                                abi.TebHsigFactors, abi.TebFleetArgs))) + ((15, None), (16, abi.TebFleetTable)):
+        if st is None:
+            if L.tebgpu_sizeof(which) != abi.FLEET_ROW_DTYPE.itemsize:
+                raise RuntimeError(f"ABI mismatch for TebFleetRow: C {L.tebgpu_sizeof(which)} vs FLEET_ROW_DTYPE "
+                                   f"{abi.FLEET_ROW_DTYPE.itemsize}")
+            continue
         if L.tebgpu_sizeof(which) != C.sizeof(st):
             raise RuntimeError(f"ABI mismatch for {st.__name__}: C {L.tebgpu_sizeof(which)} vs ctypes {C.sizeof(st)}")
     _lib = L
@@ -572,6 +586,72 @@ class TebGpu:
         None: the context's stream); does not synchronise."""
         self._check(self.lib.tebgpu_fleet_obstacles_device(self.ctx, C.byref(args), stream),
                     "tebgpu_fleet_obstacles_device")
+
+    def fleet_publish(self, pose, last_cmd, radius, rows, first=0, world=None):
+        """Robots r < R as rows first + r of a fleet table (tebgpu_fleet_publish), host buffers: pose [R][3], last_cmd
+        [R][3], radius [R], world [R] (None: 0), rows [T] abi.FLEET_ROW_DTYPE. Returns a new array: rows with the
+        robots' rows written."""
+        import numpy as np
+        pose = np.ascontiguousarray(pose, dtype=np.float64).reshape(-1, 3)
+        R = pose.shape[0]
+        out = np.array(rows, dtype=abi.FLEET_ROW_DTYPE, order="C").reshape(-1)
+        keep = dict(cmd=np.ascontiguousarray(np.broadcast_to(last_cmd, (R, 3)), dtype=np.float64),
+                    rad=np.ascontiguousarray(np.broadcast_to(radius, (R,)), dtype=np.float64),
+                    world=None if world is None else np.ascontiguousarray(np.broadcast_to(world, (R,)), dtype=np.int32))
+        fa = abi.make_fleet_args(R, 1, 0, 0, 0.0, pose=pose, last_cmd=keep["cmd"], radius=keep["rad"], world=keep["world"])
+        tb = abi.make_fleet_table(len(out), first, out if out.size else None)
+        self._check(self.lib.tebgpu_fleet_publish(self.ctx, C.byref(fa), C.byref(tb)), "tebgpu_fleet_publish")
+        return out
+
+    def fleet_publish_device(self, args, table, stream=None):
+        """tebgpu_fleet_publish_device: args (abi.TebFleetArgs: R, pose, last_cmd, radius, world) and table
+        (abi.TebFleetTable) of device pointers. Stream ordered on `stream` (None: the context's); does not synchronise."""
+        self._check(self.lib.tebgpu_fleet_publish_device(self.ctx, C.byref(args), C.byref(table), stream),
+                    "tebgpu_fleet_publish_device")
+
+    def fleet_gather(self, rows, cap):
+        """tebgpu_fleet_gather on a host table of world * cap rows: rank g's rows [g cap, (g + 1) cap) to every rank.
+        Returns a new array (a copy of rows with one rank)."""
+        import numpy as np
+        out = np.array(rows, dtype=abi.FLEET_ROW_DTYPE, order="C").reshape(-1)
+        tb = abi.make_fleet_table(len(out), 0, out if out.size else None)
+        self._check(self.lib.tebgpu_fleet_gather(self.ctx, C.byref(tb), int(cap)), "tebgpu_fleet_gather")
+        return out
+
+    def fleet_gather_device(self, table, cap, stream=None):
+        """tebgpu_fleet_gather_device: the in-place all-gather of a device table (abi.TebFleetTable) on the context's
+        communicator, stream ordered on `stream` (None: the context's); nothing without a communicator"""
+        self._check(self.lib.tebgpu_fleet_gather_device(self.ctx, C.byref(table), int(cap), stream),
+                    "tebgpu_fleet_gather_device")
+
+    def fleet_obstacles_table(self, rows, first, R, custom, range, max_rows=8, own_count=None, custom_count=None,
+                              scene=None):
+        """The neighbour rows of robots first .. first + R - 1 of a fleet table (tebgpu_fleet_obstacles_table), host
+        buffers: rows [T] abi.FLEET_ROW_DTYPE, the rest as fleet_obstacles. Returns (custom, custom_count, needed,
+        status)."""
+        import numpy as np
+        rows = np.ascontiguousarray(rows, dtype=abi.FLEET_ROW_DTYPE).reshape(-1)
+        i32 = lambda x, shape: None if x is None else np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.int32)
+        out = np.array(custom, dtype=abi.OBST_DTYPE, order="C")
+        S = out.shape[0]
+        out = out.reshape(S, -1)
+        own = i32(own_count, (S,))
+        cc = (np.zeros(S, np.int32) if own is None else own.copy()) if custom_count is None else i32(custom_count, (S,)).copy()
+        sc = i32(scene, (int(R),))
+        needed, status = np.full(int(R), -2, np.int32), np.full(int(R), -1, np.int32)
+        fa = abi.make_fleet_args(R, S, out.shape[1], max_rows, range, scene=sc, own_count=own,
+                                 custom=out if out.size else None, custom_count=cc, needed=needed, status=status)
+        tb = abi.make_fleet_table(len(rows), first, rows if rows.size else None)
+        self._check(self.lib.tebgpu_fleet_obstacles_table(self.ctx, C.byref(fa), C.byref(tb)),
+                    "tebgpu_fleet_obstacles_table")
+        return out, cc, needed, status
+
+    def fleet_obstacles_table_device(self, args, table, stream=None):
+        """tebgpu_fleet_obstacles_table_device: args (abi.TebFleetArgs; pose, last_cmd, radius and world are not read)
+        and table (abi.TebFleetTable) of device pointers. Stream ordered on `stream` (None: the context's); does not
+        synchronise."""
+        self._check(self.lib.tebgpu_fleet_obstacles_table_device(self.ctx, C.byref(args), C.byref(table), stream),
+                    "tebgpu_fleet_obstacles_table_device")
 
     def last_fleet_grid(self):
         """grid in CTAs (16 robots each) of the last fleet-obstacle launch, 0 before the first"""

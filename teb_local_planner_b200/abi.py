@@ -365,6 +365,31 @@ def make_fleet_args(R, S, C_cap, max_rows, range, **arrays) -> TebFleetArgs:
     return a
 
 
+# TebFleetRow: one robot of a fleet table as it is published (include/teb_b200.h), 64 bytes
+FLEET_ROW_DTYPE = np.dtype([("x", "f8"), ("y", "f8"), ("vx", "f8"), ("vy", "f8"), ("radius", "f8"), ("world", "i4"),
+                            ("dynamic", "i4"), ("live", "i4"), ("_pad", "i4", (3,))])
+assert FLEET_ROW_DTYPE.itemsize == 64
+
+
+class TebFleetTable(C.Structure):
+    """The fleet table of tebgpu_fleet_publish / _gather / _obstacles_table: T rows (FLEET_ROW_DTYPE), this call's robots
+    at rows first .. first + R - 1, as a host or device pointer"""
+    _fields_ = [("T", _i), ("first", _i), ("rows", C.c_void_p)]
+
+
+def make_fleet_table(T, first, rows) -> TebFleetTable:
+    """TebFleetTable of T rows with the call's robots from row `first`; rows: an address (int), a torch tensor (its
+    data_ptr()), a numpy array (its buffer; keep it alive) or None for NULL"""
+    t = TebFleetTable()
+    t.T, t.first = int(T), int(first)
+    if hasattr(rows, "data_ptr"):
+        rows = rows.data_ptr()
+    elif isinstance(rows, np.ndarray):
+        rows = ptr(rows)
+    t.rows = rows
+    return t
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

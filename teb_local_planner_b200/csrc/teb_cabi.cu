@@ -143,6 +143,7 @@ struct tebgpu_ctx {
    * one buffer; each grown by the first call that needs more */
   int32_t* d_fclaim = nullptr; size_t fclaim_bytes = 0;
   char* d_fleet = nullptr; size_t fleet_bytes = 0;
+  TebFleetRow* d_ftable = nullptr; size_t ftable_bytes = 0;   /* the host-buffer table entry points' table */
   long long last_fleet_grid = 0;      /* grid in CTAs of the last k_fleet_obstacles launch */
   /* scene H-signatures: the factor table's partial products, the in-call / uploaded factor table, the bands' chunk sums
    * and the host-buffer entry point's output, each grown by the first call that needs more */
@@ -246,6 +247,8 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 12: return (int32_t)sizeof(TebFrameArgs);
     case 13: return (int32_t)sizeof(TebHsigFactors);
     case 14: return (int32_t)sizeof(TebFleetArgs);
+    case 15: return (int32_t)sizeof(TebFleetRow);
+    case 16: return (int32_t)sizeof(TebFleetTable);
     default: return -1;
   }
 }
@@ -285,7 +288,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
                   c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
-                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet};
+                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -2109,15 +2112,16 @@ int32_t tebgpu_finish_cycle(tebgpu_ctx* ctx, TebBatch* bt, const TebCycleArgs* c
   return run_cycle_host(ctx, bt, ca, true);
 }
 
-/* argument checks of both fleet-obstacle entry points: nothing is launched when one fails */
-static int32_t check_fleet_args(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
+/* argument checks of both fleet-obstacle entry points: nothing is launched when one fails. arrays: pose, last_cmd and
+ * radius are required (not for the table step, which reads none of them) */
+static int32_t check_fleet_args(tebgpu_ctx* ctx, const TebFleetArgs* fa, bool arrays = true) {
   if (!ctx) return TEBGPU_ERR_INVALID_ARG;
   if (!fa) { ctx->err = "fleet args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
   if (fa->R < 1 || fa->S < 1 || fa->C_cap < 0) { ctx->err = "bad fleet dimensions"; return TEBGPU_ERR_INVALID_ARG; }
   if (fa->R > ctx->lim.max_bands || fa->S > ctx->lim.max_scenes) { ctx->err = "fleet exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
   if (fa->max_rows < 0 || fa->max_rows > TEB_FLEET_MAX_ROWS) { ctx->err = "max_rows outside 0 .. TEB_FLEET_MAX_ROWS"; return TEBGPU_ERR_INVALID_ARG; }
   if (!(fa->range >= 0.0)) { ctx->err = "range is NaN or negative"; return TEBGPU_ERR_INVALID_ARG; }
-  if (!fa->pose || !fa->last_cmd || !fa->radius || !fa->custom_count || (fa->C_cap > 0 && !fa->custom)) {
+  if ((arrays && (!fa->pose || !fa->last_cmd || !fa->radius)) || !fa->custom_count || (fa->C_cap > 0 && !fa->custom)) {
     ctx->err = "missing required fleet array"; return TEBGPU_ERR_INVALID_ARG;
   }
   if (!fa->scene && fa->R > fa->S) { ctx->err = "scene == NULL with R > S"; return TEBGPU_ERR_INVALID_ARG; }
@@ -2128,8 +2132,9 @@ static int32_t check_fleet_args(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
   return TEBGPU_OK;
 }
 
-/* k_fleet_claim (when scenes are given) and k_fleet_obstacles on arguments already checked */
-static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st) {
+/* k_fleet_claim (when scenes are given) and k_fleet_obstacles on arguments already checked; table: the candidates of
+ * tebgpu_fleet_obstacles_table, NULL for the caller's arrays */
+static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st, const TebFleetTable* table = nullptr) {
   int32_t rc;
   const int32_t* claims = nullptr;
   if (fa->scene) {
@@ -2139,7 +2144,8 @@ static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t
     claims = ctx->d_fclaim;
   }
   const long long grid = ((long long)fa->R + FLEET_WARPS - 1) / FLEET_WARPS;
-  k_fleet_obstacles<<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims);
+  if (table) k_fleet_obstacles<true><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table);
+  else k_fleet_obstacles<false><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{});
   ctx->last_fleet_grid = grid;
   ctx->launches = fa->scene ? 2 : 1;
   CUDA_TRY(ctx, cudaGetLastError());
@@ -2152,6 +2158,8 @@ int32_t tebgpu_fleet_obstacles_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, v
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   return issue_fleet(ctx, fa, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
 }
+
+static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table);
 
 int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
   int32_t rc = check_fleet_args(ctx, fa);
@@ -2174,6 +2182,14 @@ int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
     if (own < 0 || (size_t)own > C) { ctx->err = "own_count[s] outside 0 .. C_cap"; return TEBGPU_ERR_INVALID_ARG; }
   }
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return run_fleet_host(ctx, fa, nullptr);
+}
+
+/* the host-buffer fleet steps on arguments already checked: stage the arrays given (NULL ones stay NULL), launch on the
+ * context's stream, copy the outputs back and synchronise. table: the device copy of the candidates' table, or NULL */
+static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table) {
+  int32_t rc;
+  const size_t R = fa->R, S = fa->S, C = fa->C_cap;
   cudaStream_t st = ctx->stream;
   const size_t I = sizeof(int32_t), D = sizeof(double);
   enum { POSE, CMD, RAD, WORLD, SCENE, OWN, CUSTOM, CCOUNT, NEED, STATUS, SLOTS };
@@ -2199,11 +2215,126 @@ int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
   da.scene = (const int32_t*)sl[SCENE].dev(d); da.own_count = (const int32_t*)sl[OWN].dev(d);
   da.custom = (TebObstacle*)sl[CUSTOM].dev(d); da.custom_count = (int32_t*)sl[CCOUNT].dev(d);
   da.needed = (int32_t*)sl[NEED].dev(d); da.status = (int32_t*)sl[STATUS].dev(d);
-  if ((rc = issue_fleet(ctx, &da, st))) return rc;
+  if ((rc = issue_fleet(ctx, &da, st, table))) return rc;
   for (const CycleSlot& c : sl)
     if (c.host && c.out && c.bytes) CUDA_TRY(ctx, cudaMemcpyAsync(c.host, d + c.off, c.bytes, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
+}
+
+/* the table checks of the fleet-table entry points: rows first .. first + R - 1 lie in the table */
+static int32_t check_fleet_table(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
+  if (!t || !t->rows) { ctx->err = "fleet table or its rows == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (t->T < 1 || t->first < 0 || (int64_t)t->first + fa->R > t->T) {
+    ctx->err = "fleet table rows first .. first + R - 1 outside 0 .. T - 1"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  if (reinterpret_cast<uintptr_t>(t->rows) & 15) { ctx->err = "fleet table rows not 16-byte aligned"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+static int32_t check_fleet_publish_args(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!fa) { ctx->err = "fleet args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fa->R < 1) { ctx->err = "bad fleet dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fa->R > ctx->lim.max_bands) { ctx->err = "fleet exceeds the context limits"; return TEBGPU_ERR_CAPACITY; }
+  if (!fa->pose || !fa->last_cmd || !fa->radius) { ctx->err = "missing required fleet array"; return TEBGPU_ERR_INVALID_ARG; }
+  return check_fleet_table(ctx, fa, t);
+}
+
+static int32_t issue_fleet_publish(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t, cudaStream_t st) {
+  k_fleet_publish<<<(unsigned)((fa->R + CLAIM_THREADS - 1) / CLAIM_THREADS), CLAIM_THREADS, 0, st>>>(*fa, *t);
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_publish_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t, void* cuda_stream) {
+  const int32_t rc = check_fleet_publish_args(ctx, fa, t);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_fleet_publish(ctx, fa, t, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_fleet_publish(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
+  int32_t rc = check_fleet_publish_args(ctx, fa, t);
+  if (rc) return rc;
+  const size_t R = fa->R, I = sizeof(int32_t), D = sizeof(double);
+  for (size_t r = 0; r < R; ++r) {
+    const double* p = fa->pose + 3 * r;
+    const double* c = fa->last_cmd + 3 * r;
+    if (!std::isfinite(p[0]) || !std::isfinite(p[1]) || !std::isfinite(p[2])) { ctx->err = "pose[r] not finite"; return TEBGPU_ERR_INVALID_ARG; }
+    if (!std::isfinite(c[0]) || !std::isfinite(c[1])) { ctx->err = "last_cmd[r] not finite"; return TEBGPU_ERR_INVALID_ARG; }
+    if (!std::isfinite(fa->radius[r]) || fa->radius[r] < 0.0) { ctx->err = "radius[r] negative or not finite"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  /* the robots' rows only: the device table is rows first .. first + R - 1 of the caller's */
+  const size_t rows_bytes = R * sizeof(TebFleetRow);
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_ftable, &ctx->ftable_bytes, rows_bytes, st))) return rc;
+  enum { POSE, CMD, RAD, WORLD, SLOTS };
+  CycleSlot sl[SLOTS] = {{(void*)fa->pose, R * 3 * D, false, 0}, {(void*)fa->last_cmd, R * 3 * D, false, 0},
+                         {(void*)fa->radius, R * D, false, 0},   {(void*)fa->world, R * I, false, 0}};
+  size_t off = 0;
+  for (CycleSlot& c : sl) {
+    c.off = off;
+    if (c.host) off += (c.bytes + 255) & ~(size_t)255;
+  }
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_fleet, &ctx->fleet_bytes, off, st))) return rc;
+  char* d = ctx->d_fleet;
+  for (const CycleSlot& c : sl)
+    if (c.host && c.bytes) CUDA_TRY(ctx, cudaMemcpyAsync(d + c.off, c.host, c.bytes, cudaMemcpyHostToDevice, st));
+  TebFleetArgs da = *fa;
+  da.pose = (const double*)sl[POSE].dev(d); da.last_cmd = (const double*)sl[CMD].dev(d);
+  da.radius = (const double*)sl[RAD].dev(d); da.world = (const int32_t*)sl[WORLD].dev(d);
+  const TebFleetTable dt = {(int32_t)R, 0, ctx->d_ftable};
+  if ((rc = issue_fleet_publish(ctx, &da, &dt, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(t->rows + t->first, ctx->d_ftable, rows_bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_obstacles_table_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t,
+                                            void* cuda_stream) {
+  int32_t rc = check_fleet_args(ctx, fa, false);
+  if (rc || (rc = check_fleet_table(ctx, fa, t))) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_fleet(ctx, fa, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream, t);
+}
+
+int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
+  int32_t rc = check_fleet_args(ctx, fa, false);
+  if (rc || (rc = check_fleet_table(ctx, fa, t))) return rc;
+  const size_t R = fa->R, S = fa->S, C = fa->C_cap, T = t->T;
+  /* what the device entry point would answer with BAD_INPUT / SHARED_SCENE, and every non-finite live row, are refused
+   * here, before anything runs */
+  for (size_t q = 0; q < T; ++q) {
+    const TebFleetRow& w = t->rows[q];
+    if (!w.live) continue;
+    if (!std::isfinite(w.x) || !std::isfinite(w.y) || !std::isfinite(w.vx) || !std::isfinite(w.vy)) {
+      ctx->err = "live fleet row not finite"; return TEBGPU_ERR_INVALID_ARG;
+    }
+    if (!std::isfinite(w.radius) || w.radius < 0.0) { ctx->err = "live fleet row radius negative or not finite"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  std::vector<char> taken(S, 0);
+  for (size_t r = 0; r < R; ++r) {
+    if (!t->rows[t->first + r].live) { ctx->err = "the robot's own fleet row is not live"; return TEBGPU_ERR_INVALID_ARG; }
+    const int32_t s = fa->scene ? fa->scene[r] : (int32_t)r;
+    if (s < 0 || (size_t)s >= S) { ctx->err = "scene[r] outside 0 .. S-1"; return TEBGPU_ERR_INVALID_ARG; }
+    if (taken[s]) { ctx->err = "two robots in one scene"; return TEBGPU_ERR_INVALID_ARG; }
+    taken[s] = 1;
+    const int32_t own = fa->own_count ? fa->own_count[s] : 0;
+    if (own < 0 || (size_t)own > C) { ctx->err = "own_count[s] outside 0 .. C_cap"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t bytes = T * sizeof(TebFleetRow);
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_ftable, &ctx->ftable_bytes, bytes, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ftable, t->rows, bytes, cudaMemcpyHostToDevice, st));
+  const TebFleetTable dt = {t->T, t->first, ctx->d_ftable};
+  TebFleetArgs ha = *fa;
+  ha.pose = ha.last_cmd = ha.radius = nullptr;
+  ha.world = nullptr;
+  return run_fleet_host(ctx, &ha, &dt);
 }
 
 int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args) {
@@ -2897,6 +3028,43 @@ int32_t tebgpu_optimize_batch_gather(tebgpu_ctx* ctx, const TebBatch* bt, const 
   cudaStream_t st = ctx->stream;
   NCCL_TRY(ctx, nccl_api().AllGather(ctx->d_cost, ctx->d_gather, (size_t)bt->B, ncclDouble, ctx->comm, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(cost_all, ctx->d_gather, (size_t)bt->B * ctx->world * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* the second collective: the fleet table, rank g's rows [g cap, (g + 1) cap) to every rank, in place */
+static int32_t check_fleet_gather(tebgpu_ctx* ctx, const TebFleetTable* t, int32_t cap) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!t || !t->rows) { ctx->err = "fleet table or its rows == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (cap < 1 || (int64_t)t->T != (int64_t)ctx->world * cap) { ctx->err = "fleet gather needs cap >= 1 and T == world * cap"; return TEBGPU_ERR_INVALID_ARG; }
+  if (reinterpret_cast<uintptr_t>(t->rows) & 15) { ctx->err = "fleet table rows not 16-byte aligned"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_gather_device(tebgpu_ctx* ctx, const TebFleetTable* t, int32_t cap, void* cuda_stream) {
+  const int32_t rc = check_fleet_gather(ctx, t, cap);
+  if (rc) return rc;
+  if (!ctx->comm) return TEBGPU_OK;          /* one rank: the table is whole */
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  const size_t bytes = (size_t)cap * sizeof(TebFleetRow);
+  NCCL_TRY(ctx, nccl_api().AllGather((const char*)t->rows + (size_t)ctx->rank * bytes, t->rows, bytes, ncclChar, ctx->comm, st));
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_gather(tebgpu_ctx* ctx, const TebFleetTable* t, int32_t cap) {
+  int32_t rc = check_fleet_gather(ctx, t, cap);
+  if (rc) return rc;
+  if (!ctx->comm) return TEBGPU_OK;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t bytes = (size_t)cap * sizeof(TebFleetRow), all = bytes * ctx->world;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_ftable, &ctx->ftable_bytes, all, st))) return rc;
+  char* d = (char*)ctx->d_ftable;
+  const size_t mine = (size_t)ctx->rank * bytes;
+  CUDA_TRY(ctx, cudaMemcpyAsync(d + mine, (const char*)t->rows + mine, bytes, cudaMemcpyHostToDevice, st));
+  NCCL_TRY(ctx, nccl_api().AllGather(d + mine, d, bytes, ncclChar, ctx->comm, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(t->rows, d, all, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
 }

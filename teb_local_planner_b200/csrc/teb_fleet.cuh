@@ -3,9 +3,12 @@
  * _device). The contract is at TebFleetArgs in include/teb_b200.h.
  *
  *   k_fleet_claim      one thread per robot: counts the robots of every scene (only when TebFleetArgs.scene is given)
- *   k_fleet_obstacles  one warp per robot, FLEET_WARPS robots per CTA: all pairs, tiled through shared memory
+ *   k_fleet_obstacles  one warp per robot, FLEET_WARPS robots per CTA: all pairs, tiled through shared memory; TABLE
+ *                      false takes the candidates from the caller's arrays (tebgpu_fleet_obstacles), true from the
+ *                      rows of a TebFleetTable (tebgpu_fleet_obstacles_table)
+ *   k_fleet_publish    one thread per robot: the robot's TebFleetRow (tebgpu_fleet_publish)
  *
- * The CTA stages FLEET_TILE robots' (x, y, world) at a time; lane l of a warp tests candidates l, l + 32, ... of the
+ * The CTA stages FLEET_TILE robots' (x, y, world) at a time (the table build (x, y, world, live)); lane l of a warp tests candidates l, l + 32, ... of the
  * tile against its robot, and the warp keeps the nearest min(max_rows, C_cap - own) neighbours as a list sorted by
  * (d2, index), slot i in lane i. A candidate enters the list only when it is below the list's last slot, so after the
  * first few tiles almost every ballot is empty and the scan costs the distance test alone. The list is a total order
@@ -28,6 +31,31 @@ __device__ __forceinline__ bool fleet_less(double da, int qa, double db, int qb)
   return da < db || (da == db && qa < qb);
 }
 
+/* the row robot q is published as, from its pose (x, y, theta), body command (vx, vy) and radius: the publisher's
+ * map-frame velocity R(theta) (vx, vy), then setCentroidVelocity's rule (obstacles.h:214-233), Eigen's norm() =
+ * sqrt(squaredNorm()), of the body command: the rotation keeps the norm, and so the decision does not depend on the last
+ * bits of sin / cos. Both the array build of k_fleet_obstacles and k_fleet_publish write their rows from here. */
+__device__ __forceinline__ TebFleetRow fleet_row(const double* pose, const double* cmd, const double* radius, int world) {
+  const double th = pose[2], bx = cmd[0], by = cmd[1];
+  double sn, cs;
+  sincos(th, &sn, &cs);
+  double vx = __dsub_rn(__dmul_rn(cs, bx), __dmul_rn(sn, by));
+  double vy = __dadd_rn(__dmul_rn(sn, bx), __dmul_rn(cs, by));
+  const bool moving = !(sqrt(__dadd_rn(__dmul_rn(bx, bx), __dmul_rn(by, by))) < 0.001);
+  if (!moving) vx = vy = 0.0;
+  TebFleetRow w;
+  w.x = pose[0];
+  w.y = pose[1];
+  w.vx = vx;
+  w.vy = vy;
+  w.radius = *radius;
+  w.world = world;
+  w.dynamic = moving ? 1 : 0;
+  w.live = 1;
+  w._pad[0] = w._pad[1] = w._pad[2] = 0;
+  return w;
+}
+
 __global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_claim(const TebFleetArgs a, int32_t* claims) {
   const int r = blockIdx.x * CLAIM_THREADS + threadIdx.x;
   if (r >= a.R) return;
@@ -35,24 +63,39 @@ __global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_claim(const TebFleetArg
   if (s >= 0 && s < a.S) atomicAdd(&claims[s], 1);
 }
 
-/* claims: [S] robots per scene from k_fleet_claim, or NULL when TebFleetArgs.scene is NULL (scene r, never shared) */
-__global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFleetArgs a, const int32_t* claims) {
+/* claims: [S] robots per scene from k_fleet_claim, or NULL when TebFleetArgs.scene is NULL (scene r, never shared).
+ * TABLE: robot r is row t.first + r of t and the candidates are its T rows; otherwise t is not read. */
+template <bool TABLE>
+__global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFleetArgs a, const int32_t* claims,
+                                                                   const TebFleetTable t) {
   __shared__ double sx[FLEET_TILE], sy[FLEET_TILE];
   __shared__ int sw[FLEET_TILE];
+  __shared__ int sl[TABLE ? FLEET_TILE : 1];
   constexpr unsigned FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const int r = blockIdx.x * FLEET_WARPS + (threadIdx.x >> 5);
   const bool live = r < a.R;
+  const int self = TABLE ? t.first + r : r;    /* the robot's own candidate index */
+  const int N = TABLE ? t.T : a.R;             /* candidates */
 
   double xr = 0.0, yr = 0.0;
   int wr = 0, s = -1, own = 0, K = 0, st = TEB_FLEET_BAD_INPUT;
   bool valid = false;
   if (live) {
-    xr = a.pose[3 * (size_t)r];
-    yr = a.pose[3 * (size_t)r + 1];
-    wr = a.world ? a.world[r] : 0;
+    bool ok = true;
+    if constexpr (TABLE) {
+      const TebFleetRow& me = t.rows[self];
+      xr = me.x;
+      yr = me.y;
+      wr = me.world;
+      ok = me.live != 0;
+    } else {
+      xr = a.pose[3 * (size_t)r];
+      yr = a.pose[3 * (size_t)r + 1];
+      wr = a.world ? a.world[r] : 0;
+    }
     s = a.scene ? a.scene[r] : r;
-    if (s >= 0 && s < a.S) {
+    if (ok && s >= 0 && s < a.S) {
       own = a.own_count ? a.own_count[s] : 0;
       if (own >= 0 && own <= a.C_cap) {
         if (claims && claims[s] != 1) st = TEB_FLEET_SHARED_SCENE;
@@ -67,14 +110,22 @@ __global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFlee
   int kq = INT_MAX, tq = INT_MAX;
   int needed = 0;
 
-  for (int base = 0; base < a.R; base += FLEET_TILE) {
-    const int nt = min(FLEET_TILE, a.R - base);
+  for (int base = 0; base < N; base += FLEET_TILE) {
+    const int nt = min(FLEET_TILE, N - base);
     __syncthreads();
     if ((int)threadIdx.x < nt) {
       const size_t q = (size_t)base + threadIdx.x;
-      sx[threadIdx.x] = a.pose[3 * q];
-      sy[threadIdx.x] = a.pose[3 * q + 1];
-      sw[threadIdx.x] = a.world ? a.world[q] : 0;
+      if constexpr (TABLE) {
+        const TebFleetRow& w = t.rows[q];
+        sx[threadIdx.x] = w.x;
+        sy[threadIdx.x] = w.y;
+        sw[threadIdx.x] = w.world;
+        sl[threadIdx.x] = w.live;
+      } else {
+        sx[threadIdx.x] = a.pose[3 * q];
+        sy[threadIdx.x] = a.pose[3 * q + 1];
+        sw[threadIdx.x] = a.world ? a.world[q] : 0;
+      }
     }
     __syncthreads();
     if (!valid) continue;                 /* warp-uniform: one robot per warp */
@@ -82,7 +133,7 @@ __global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFlee
       const int j = j0 + lane, q = base + j;
       bool in = false;
       double d2 = 0.0;
-      if (j < nt && q != r && sw[j] == wr) {
+      if (j < nt && q != self && sw[j] == wr && (!TABLE || sl[j] != 0)) {
         const double dx = __dsub_rn(sx[j], xr), dy = __dsub_rn(sy[j], yr);
         d2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
         in = d2 <= range2;
@@ -119,22 +170,15 @@ __global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFlee
   const int written = min(needed, K);
   if (lane < written) {
     const size_t q = (size_t)kq;
-    const double th = a.pose[3 * q + 2], bx = a.last_cmd[3 * q], by = a.last_cmd[3 * q + 1];
-    double sn, cs;
-    sincos(th, &sn, &cs);
-    double vx = __dsub_rn(__dmul_rn(cs, bx), __dmul_rn(sn, by));
-    double vy = __dadd_rn(__dmul_rn(sn, bx), __dmul_rn(cs, by));
-    /* setCentroidVelocity (obstacles.h:214-233), Eigen's norm() = sqrt(squaredNorm()), of the body command: the rotation
-     * keeps the norm, and so the decision does not depend on the last bits of sin / cos */
-    const bool moving = !(sqrt(__dadd_rn(__dmul_rn(bx, bx), __dmul_rn(by, by))) < 0.001);
-    if (!moving) vx = vy = 0.0;
+    /* the neighbour's row: copied from the table as it was published, or made here from the caller's arrays */
+    const TebFleetRow w = TABLE ? t.rows[q] : fleet_row(a.pose + 3 * q, a.last_cmd + 3 * q, a.radius + q, 0);
     TebObstacle o;
-    o.x = a.pose[3 * q];
-    o.y = a.pose[3 * q + 1];
-    o.vx = vx;
-    o.vy = vy;
-    o.radius = a.radius[q];
-    o.dynamic = moving ? 1 : 0;
+    o.x = w.x;
+    o.y = w.y;
+    o.vx = w.vx;
+    o.vy = w.vy;
+    o.radius = w.radius;
+    o.dynamic = w.dynamic;
     o.type = TEB_OBST_CIRCULAR;
     o.vertex_begin = 0;
     o.vertex_count = 0;
@@ -146,6 +190,13 @@ __global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFlee
     if (a.needed) a.needed[r] = needed;
     if (a.status) a.status[r] = written < needed ? TEB_FLEET_TRUNCATED : TEB_FLEET_WRITTEN;
   }
+}
+
+__global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_publish(const TebFleetArgs a, const TebFleetTable t) {
+  const int r = blockIdx.x * CLAIM_THREADS + threadIdx.x;
+  if (r >= a.R) return;
+  t.rows[(size_t)t.first + r] = fleet_row(a.pose + 3 * (size_t)r, a.last_cmd + 3 * (size_t)r, a.radius + r,
+                                          a.world ? a.world[r] : 0);
 }
 
 }  // namespace tebgpu

@@ -9,7 +9,9 @@ stream, include/teb_b200.h). This module only
   * bootstraps the communicator: rank 0 creates the 128-byte NCCL id, `torch.distributed` (any backend) carries it to
     the other ranks (`init_comm`) - the same job MPI or a file would do for a C++ host,
   * restates selectBestTeb for whole request batches (`select_best_per_request`),
-  * offers the same gather over a torch process group for CPU tests (`gather_costs_torch`, gloo).
+  * offers the same gather over a torch process group for CPU tests (`gather_costs_torch`, gloo),
+  * lays out the fleet table of a sharded fleet (`fleet_layout`) and gathers it over a torch process group
+    (`gather_fleet_table_torch`), as tebgpu_fleet_gather does over NCCL.
 """
 import ctypes as C
 
@@ -82,3 +84,30 @@ def select_best_per_request(all_cost, candidates, params=None, last_best=None, i
         ip = -1 if initial_plan is None else int(initial_plan[r])
         out[r] = select_best(all_cost[r], lb, ip, hyst, pref)
     return out
+
+
+def fleet_layout(counts, world):
+    """The fleet table of a fleet whose rank g holds counts[g] robots: every rank's shard padded to cap rows (NCCL has no
+    all-gather-v), so the table has T = world * cap rows and rank g's robots are rows first[g] .. first[g] + counts[g] - 1.
+    Returns (cap, first per rank)."""
+    counts = [int(c) for c in counts]
+    if len(counts) != world or min(counts) < 0:
+        raise ValueError("one non-negative robot count per rank")
+    cap = max(1, max(counts))
+    return cap, [g * cap for g in range(world)]
+
+
+def gather_fleet_table_torch(rows, cap, rank, world=None, group=None):
+    """tebgpu_fleet_gather over a torch process group (gloo on CPU): rows is the rank's [world * cap] fleet table
+    (abi.FLEET_ROW_DTYPE numpy array) with its shard at rows [rank cap, (rank + 1) cap); returns the gathered table."""
+    import torch
+    import torch.distributed as dist
+    from . import abi
+    world = dist.get_world_size(group) if world is None else world
+    rows = np.ascontiguousarray(rows, dtype=abi.FLEET_ROW_DTYPE).reshape(-1)
+    if len(rows) != world * cap:
+        raise ValueError("the fleet table must have world * cap rows")
+    mine = torch.from_numpy(rows[rank * cap:(rank + 1) * cap].copy().view(np.uint8))
+    out = torch.empty(world * mine.numel(), dtype=torch.uint8)
+    dist.all_gather_into_tensor(out, mine, group=group)
+    return out.numpy().view(abi.FLEET_ROW_DTYPE).copy()
