@@ -840,12 +840,21 @@ int32_t tebgpu_finish_cycle_device(tebgpu_ctx* ctx, TebBatch* batch, const TebCy
  * tebgpu_optimize_batch_device, does not synchronise; a robot whose scene is outside 0 .. S - 1 or whose own_count is
  * outside 0 .. C_cap gets TEB_FLEET_BAD_INPUT, one whose scene another robot also maps to gets TEB_FLEET_SHARED_SCENE;
  * either has needed = -1 and nothing written to its scene. Such robots are still neighbours of the others. The shared
- * scene check takes context scratch of S int32 (allocated by the first call that needs it, which synchronises the
- * stream); calls of one context share it, so issue them on one stream.
+ * scene check takes context scratch of S int32, and the grid search (below) bucket counts and starts, the candidate
+ * indices and the far list, sized to the largest candidate count seen; each is allocated by the first call that needs
+ * it, which synchronises the stream. Calls of one context share this scratch, so issue them on one stream.
  *
- * One warp per robot, FLEET_WARPS robots per CTA: the CTA stages the fleet's (x, y, world) in shared-memory tiles, the
- * lanes test the candidates, and the warp keeps its top-max_rows list in registers, one slot per lane
- * (tebgpu_get_info key 18: the grid in CTAs). All pairs are tested: O(R^2), exact and deterministic. */
+ * One warp per robot, FLEET_WARPS robots per CTA, keeps its top-max_rows list in registers, one slot per lane
+ * (tebgpu_get_info key 18: the grid in CTAs). The candidates come from one of two searches (tebgpu_set_fleet_search;
+ * key 19 reports the one the last step ran), which write the same bytes on every input:
+ *   all pairs  the CTA stages the fleet's (x, y, world) in shared-memory tiles and the lanes test every candidate:
+ *              O(R^2);
+ *   grid       the candidates are binned into square cells of side h = max(range (1 + 2^-16), 2^-500) per world,
+ *              hashed into buckets; each robot tests the candidates of its 3 x 3 cells, and those past the cell
+ *              coordinate bound 2^24 (a far list): O(R) for a fleet of bounded density.
+ * The automatic search takes the grid from 4096 candidates on when range is above 2^-500 and range * range is finite;
+ * below that, and at range inf, all pairs. The kept list is ordered by (d2, index), a total order, so it does not depend
+ * on the order the candidates are met in, and both searches are exact and deterministic. */
 #define TEB_FLEET_MAX_ROWS 32
 #define TEB_FLEET_WRITTEN       0  /* every neighbour in range written */
 #define TEB_FLEET_TRUNCATED     1  /* written < needed: max_rows or C_cap - own_count kept the nearest ones */
@@ -919,8 +928,9 @@ typedef struct TebFleetTable {
  * those of its own row; pose, last_cmd, radius and world of args are not read (may be NULL). scene, own_count, custom,
  * custom_count, needed, status, the cuts and the shared-scene check are TebFleetArgs'. On the device, a robot whose own
  * row is not live gets TEB_FLEET_BAD_INPUT (needed -1, nothing written); the host entry point refuses it, and refuses a
- * live row whose x, y, vx, vy or radius is not finite or whose radius is negative. tebgpu_get_info key 18 reports the
- * grid of its k_fleet_obstacles launch.
+ * live row whose x, y, vx, vy or radius is not finite or whose radius is negative. The candidates are the T rows, found
+ * by all pairs or by the grid as in TebFleetArgs' step (4096 rows and up: the grid), so each owner pays O(R T) or
+ * O(R + T); tebgpu_get_info keys 18 / 19 report the launch's grid and search.
  *
  * Argument errors return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit) before anything is launched: those
  * of TebFleetArgs for the arrays each step reads, NULL table or rows, T < 1, first < 0, first + R > T, rows not 16-byte
@@ -946,6 +956,15 @@ int32_t tebgpu_set_solver(tebgpu_ctx* ctx, int32_t solver);
  * registers; 1 the first-generation kernel: one 128-thread CTA per 32-pose tile, one thread per band row. Same
  * arithmetic, different summation order (results agree to round-off); variant 1 is kept as an independent cross-check. */
 int32_t tebgpu_set_linearize_variant(tebgpu_ctx* ctx, int32_t variant);
+/* The neighbour search of the fleet steps (tebgpu_fleet_obstacles(_device), tebgpu_fleet_obstacles_table(_device)):
+ * TEBGPU_FLEET_SEARCH_AUTO (default) the grid from 4096 candidates on with a finite range above 2^-500, else all pairs;
+ * _ALL_PAIRS always all pairs; _GRID always the grid; _ONE_BUCKET the grid with every cell hashed to one bucket (a test
+ * of the bucket collisions). Every mode writes the same bytes. Another mode returns TEBGPU_ERR_INVALID_ARG. */
+#define TEBGPU_FLEET_SEARCH_AUTO 0
+#define TEBGPU_FLEET_SEARCH_ALL_PAIRS 1
+#define TEBGPU_FLEET_SEARCH_GRID 2
+#define TEBGPU_FLEET_SEARCH_ONE_BUCKET 3
+int32_t tebgpu_set_fleet_search(tebgpu_ctx* ctx, int32_t mode);
 /* Speculation width of solver 2: how many consecutive LM damping trials are solved per round (2, 4, 6 or 8; 0 = auto).
  * Results do not depend on it (the accept / reject chain is replayed in order), only latency and traffic do. */
 int32_t tebgpu_set_speculation(tebgpu_ctx* ctx, int32_t k);
@@ -1054,8 +1073,9 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * first), 15 grid in CTAs of the last costmap conversion (k_costmap_obstacles, one CTA per scene; 0 before the first),
  * 16 grid in CTAs of the last local-plan launch (k_local_plan, 4 bands per CTA; 0 before the first), 17 grid in CTAs
  * of the last backup-modes or finish-cycle launch (k_backup_modes / k_finish_cycle, 128 bands per CTA; 0 before the
- * first), 18 grid in CTAs of the last fleet-obstacle launch (k_fleet_obstacles, FLEET_WARPS robots per CTA; 0 before
- * the first).
+ * first), 18 grid in CTAs of the last fleet-obstacle launch (k_fleet_obstacles or k_fleet_obstacles_grid, FLEET_WARPS
+ * robots per CTA; 0 before the first), 19 the search that launch ran (TEBGPU_FLEET_SEARCH_ALL_PAIRS, _GRID or
+ * _ONE_BUCKET; -1 before the first).
  * Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */

@@ -104,6 +104,8 @@ def load_library(build_if_missing=False):
     L.tebgpu_get_plan_kernel_times.argtypes = [vp, C.POINTER(C.c_double * 2), C.POINTER(C.c_int64 * 2)]
     L.tebgpu_set_linearize_variant.restype = C.c_int32
     L.tebgpu_set_linearize_variant.argtypes = [vp, C.c_int32]
+    L.tebgpu_set_fleet_search.restype = C.c_int32
+    L.tebgpu_set_fleet_search.argtypes = [vp, C.c_int32]
     L.tebgpu_set_speculation.restype = C.c_int32
     L.tebgpu_set_speculation.argtypes = [vp, C.c_int32]
     L.tebgpu_set_solver.restype = C.c_int32
@@ -656,6 +658,18 @@ class TebGpu:
     def last_fleet_grid(self):
         """grid in CTAs (16 robots each) of the last fleet-obstacle launch, 0 before the first"""
         return self.info(18)
+
+    FLEET_SEARCHES = {abi.TEBGPU_FLEET_SEARCH_ALL_PAIRS: "all_pairs", abi.TEBGPU_FLEET_SEARCH_GRID: "grid",
+                      abi.TEBGPU_FLEET_SEARCH_ONE_BUCKET: "one_bucket"}
+
+    def set_fleet_search(self, mode):
+        """neighbour search of the fleet steps (abi.TEBGPU_FLEET_SEARCH_*): 0 automatic (default), 1 all pairs, 2 the
+        grid, 3 the grid with every cell in one bucket. Every mode writes the same bytes."""
+        self._check(self.lib.tebgpu_set_fleet_search(self.ctx, int(mode)), "tebgpu_set_fleet_search")
+
+    def last_fleet_search(self):
+        """the search the last fleet step ran: one of FLEET_SEARCHES' names, or None before the first"""
+        return self.FLEET_SEARCHES.get(self.info(abi.TEBGPU_INFO_FLEET_SEARCH))
 
     def last_cycle_grid(self):
         """grid in CTAs (128 bands each) of the last backup-modes or finish-cycle launch, 0 before the first"""

@@ -344,6 +344,14 @@ class TebFleetArgs(C.Structure):
 
 
 TEB_FLEET_MAX_ROWS = 32
+# TEBGPU_FLEET_SEARCH_*: tebgpu_set_fleet_search's modes, and tebgpu_get_info key 19's values (-1 before the first step)
+(TEBGPU_FLEET_SEARCH_AUTO, TEBGPU_FLEET_SEARCH_ALL_PAIRS, TEBGPU_FLEET_SEARCH_GRID,
+ TEBGPU_FLEET_SEARCH_ONE_BUCKET) = range(4)
+TEBGPU_INFO_FLEET_GRID, TEBGPU_INFO_FLEET_SEARCH = 18, 19
+# the automatic search takes the grid from this many candidates on (FLEET_GRID_N0 in csrc/teb_cabi.cu) ...
+FLEET_GRID_N0 = 4096
+# ... when range is above the cell side's floor and range * range is finite (csrc/teb_fleet.cuh)
+FLEET_H_MARGIN, FLEET_H_FLOOR, FLEET_CELL_BOUND = 1.0 + 2.0 ** -16, 2.0 ** -500, 2.0 ** 24
 # TEB_FLEET_*: what tebgpu_fleet_obstacles did for a robot
 TEB_FLEET_WRITTEN, TEB_FLEET_TRUNCATED, TEB_FLEET_BAD_INPUT, TEB_FLEET_SHARED_SCENE = range(4)
 

@@ -3,6 +3,7 @@
  * No CPU fallback: every entry point that optimises needs a CUDA device and fails loudly otherwise.
  */
 #include <cuda_runtime.h>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -144,7 +145,12 @@ struct tebgpu_ctx {
   int32_t* d_fclaim = nullptr; size_t fclaim_bytes = 0;
   char* d_fleet = nullptr; size_t fleet_bytes = 0;
   TebFleetRow* d_ftable = nullptr; size_t ftable_bytes = 0;   /* the host-buffer table entry points' table */
-  long long last_fleet_grid = 0;      /* grid in CTAs of the last k_fleet_obstacles launch */
+  long long last_fleet_grid = 0;      /* grid in CTAs of the last k_fleet_obstacles(_grid) launch */
+  int fleet_search = TEBGPU_FLEET_SEARCH_AUTO; /* tebgpu_set_fleet_search */
+  int last_fleet_search = -1;         /* the search the last fleet step ran (TEBGPU_FLEET_SEARCH_*), -1 before the first */
+  /* the fleet grid: bucket counts and starts, candidate keys, ranks and indices, the far list and the scan's
+   * temporary storage, in one buffer grown by the first call that needs more */
+  char* d_fgrid = nullptr; size_t fgrid_bytes = 0;
   /* scene H-signatures: the factor table's partial products, the in-call / uploaded factor table, the bands' chunk sums
    * and the host-buffer entry point's output, each grown by the first call that needs more */
   char* d_hsf_part = nullptr; char* d_hsf_tab = nullptr; double* d_hs_part = nullptr; double* d_hs_out = nullptr;
@@ -277,6 +283,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 16: return ctx->last_lplan_grid;
     case 17: return ctx->last_cycle_grid;
     case 18: return ctx->last_fleet_grid;
+    case 19: return ctx->last_fleet_search;
     default: return -1;
   }
 }
@@ -288,7 +295,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
                   c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
-                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable};
+                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1181,6 +1188,12 @@ int32_t tebgpu_get_plan_kernel_times(tebgpu_ctx* ctx, double ms_out[2], int64_t 
 int32_t tebgpu_set_linearize_variant(tebgpu_ctx* ctx, int32_t v) {
   if (!ctx || v < 0 || v > 1) return TEBGPU_ERR_INVALID_ARG;
   ctx->linearize_variant = v;
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_set_fleet_search(tebgpu_ctx* ctx, int32_t mode) {
+  if (!ctx || mode < TEBGPU_FLEET_SEARCH_AUTO || mode > TEBGPU_FLEET_SEARCH_ONE_BUCKET) return TEBGPU_ERR_INVALID_ARG;
+  ctx->fleet_search = mode;
   return TEBGPU_OK;
 }
 
@@ -2132,10 +2145,67 @@ static int32_t check_fleet_args(tebgpu_ctx* ctx, const TebFleetArgs* fa, bool ar
   return TEBGPU_OK;
 }
 
-/* k_fleet_claim (when scenes are given) and k_fleet_obstacles on arguments already checked; table: the candidates of
- * tebgpu_fleet_obstacles_table, NULL for the caller's arrays */
+/* The automatic search takes the grid from FLEET_GRID_N0 candidates (R for the array step, T for the table step) on.
+ * tools/fleet_grid.py on one H100 80GB HBM3 at 700 W (DESIGN §8), the uniform square fleet at range 3 m: all pairs
+ * 30 us against the grid's 38 us at 2048 robots, 56 us against 35 us at 4096. */
+constexpr int64_t FLEET_GRID_N0 = 4096;
+constexpr int64_t FLEET_GRID_MAX_N = (int64_t)1 << 28;   /* the grid's buckets are counted in int32 */
+
+/* the search a fleet step over N candidates runs (TEBGPU_FLEET_SEARCH_ALL_PAIRS, _GRID or _ONE_BUCKET) */
+static int fleet_search(const tebgpu_ctx* ctx, const TebFleetArgs* fa, int64_t N) {
+  if (ctx->fleet_search != TEBGPU_FLEET_SEARCH_AUTO) return ctx->fleet_search;
+  const bool pays = N >= FLEET_GRID_N0 && N <= FLEET_GRID_MAX_N && fa->range > FLEET_H_FLOOR &&
+                    std::isfinite(fa->range * fa->range);
+  return pays ? TEBGPU_FLEET_SEARCH_GRID : TEBGPU_FLEET_SEARCH_ALL_PAIRS;
+}
+
+/* the grid of a step over N candidates: scratch grown to fit, counts cleared, then k_fleet_bin, the scan of the counts
+ * and k_fleet_scatter; the search kernel follows on the same stream */
+static int32_t issue_fleet_grid(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st, const TebFleetTable* table,
+                                int64_t N, bool one_bucket, FleetGrid* g) {
+  int32_t rc;
+  if (N > FLEET_GRID_MAX_N) { ctx->err = "the fleet grid holds at most 2^28 candidates"; return TEBGPU_ERR_CAPACITY; }
+  size_t H = 1;
+  while (H < 2 * (size_t)N) H <<= 1;
+  size_t scan_bytes = 0;
+  CUDA_TRY(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t*)nullptr, (int32_t*)nullptr, (int)(H + 1), st));
+  const size_t I = sizeof(int32_t);
+  const size_t parts[] = {(H + 2) * I, (H + 1) * I, N * I, N * I, N * I, N * I, scan_bytes};
+  size_t off[8] = {0}, total = 0;
+  for (int k = 0; k < 7; ++k) {
+    off[k] = total;
+    total += (parts[k] + 255) & ~(size_t)255;
+  }
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_fgrid, &ctx->fgrid_bytes, total, st))) return rc;
+  char* d = ctx->d_fgrid;
+  g->count = (int32_t*)(d + off[0]);
+  g->nfar = g->count + H + 1;
+  g->start = (int32_t*)(d + off[1]);
+  g->key = (int32_t*)(d + off[2]);
+  g->rank = (int32_t*)(d + off[3]);
+  g->idx = (int32_t*)(d + off[4]);
+  g->far = (int32_t*)(d + off[5]);
+  g->mask = one_bucket ? 0u : (unsigned)(H - 1);
+  g->h = fleet_cell_side(fa->range);
+  g->fin2 = fa->range * fa->range < INFINITY;
+  const unsigned blocks = (unsigned)((N + CLAIM_THREADS - 1) / CLAIM_THREADS);
+  CUDA_TRY(ctx, cudaMemsetAsync(g->count, 0, (H + 2) * I, st));
+  if (table) k_fleet_bin<true><<<blocks, CLAIM_THREADS, 0, st>>>(*fa, *table, *g);
+  else k_fleet_bin<false><<<blocks, CLAIM_THREADS, 0, st>>>(*fa, TebFleetTable{}, *g);
+  CUDA_TRY(ctx, cub::DeviceScan::ExclusiveSum(d + off[6], scan_bytes, g->count, g->start, (int)(H + 1), st));
+  k_fleet_scatter<<<blocks, CLAIM_THREADS, 0, st>>>((int)N, *g);
+  return TEBGPU_OK;
+}
+
+/* k_fleet_claim (when scenes are given), then k_fleet_obstacles or the grid and k_fleet_obstacles_grid, on arguments
+ * already checked; table: the candidates of tebgpu_fleet_obstacles_table, NULL for the caller's arrays */
 static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st, const TebFleetTable* table = nullptr) {
   int32_t rc;
+  const int64_t N = table ? table->T : fa->R;
+  const int search = fleet_search(ctx, fa, N);
+  FleetGrid g{};
+  if (search != TEBGPU_FLEET_SEARCH_ALL_PAIRS &&
+      (rc = issue_fleet_grid(ctx, fa, st, table, N, search == TEBGPU_FLEET_SEARCH_ONE_BUCKET, &g))) return rc;
   const int32_t* claims = nullptr;
   if (fa->scene) {
     if ((rc = grow_mirror(ctx, (void**)&ctx->d_fclaim, &ctx->fclaim_bytes, (size_t)fa->S * sizeof(int32_t), st))) return rc;
@@ -2144,10 +2214,17 @@ static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t
     claims = ctx->d_fclaim;
   }
   const long long grid = ((long long)fa->R + FLEET_WARPS - 1) / FLEET_WARPS;
-  if (table) k_fleet_obstacles<true><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table);
-  else k_fleet_obstacles<false><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{});
+  if (search == TEBGPU_FLEET_SEARCH_ALL_PAIRS) {
+    if (table) k_fleet_obstacles<true><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table);
+    else k_fleet_obstacles<false><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{});
+  } else {
+    if (table) k_fleet_obstacles_grid<true><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, g);
+    else k_fleet_obstacles_grid<false><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, g);
+  }
   ctx->last_fleet_grid = grid;
-  ctx->launches = fa->scene ? 2 : 1;
+  ctx->last_fleet_search = search;
+  /* the grid: k_fleet_bin, DeviceScan's init and scan kernels, k_fleet_scatter */
+  ctx->launches = (fa->scene ? 2 : 1) + (search == TEBGPU_FLEET_SEARCH_ALL_PAIRS ? 0 : 4);
   CUDA_TRY(ctx, cudaGetLastError());
   return TEBGPU_OK;
 }
