@@ -644,7 +644,7 @@ typedef struct TebCycleArgs {
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
  * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs, 13 TebHsigFactors, 14 TebFleetArgs,
- * 15 TebFleetRow, 16 TebFleetTable. */
+ * 15 TebFleetRow, 16 TebFleetTable, 17 TebFleetShapes. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -945,6 +945,94 @@ int32_t tebgpu_fleet_gather_device(tebgpu_ctx* ctx, const TebFleetTable* table, 
 int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetTable* table);
 int32_t tebgpu_fleet_obstacles_table_device(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetTable* table,
                                             void* cuda_stream);
+
+/* Every neighbour as its own footprint (the _shaped fleet steps): what a multi-robot publisher sends when it sends each
+ * robot's footprint polygon, line or circles instead of one enclosing circle, read the way
+ * updateObstacleContainerWithCustomObstacles reads such a message (teb_local_planner_ros.cpp:574-623: one point with a
+ * radius a CircularObstacle, one point a PointObstacle, two a LineObstacle, more a PolygonObstacle with
+ * finalizePolygon), each obstacle given the robot's velocity by setCentroidVelocity. A shape library says how each robot
+ * kind is published; kind ids are fleet-wide, so every context and rank passes the same library.
+ *
+ * The library (HOST arrays in every entry point, validated and copied into the launch; the device copy is context
+ * memory, re-sent on the call's stream only when the library changes, so issue a context's shaped steps, host and
+ * _device forms, on one stream, as its fleet-grid scratch asks): K kinds; kind k is parts kind_parts[k] .. kind_parts[k + 1] - 1,
+ * 1 .. TEB_FLEET_MAX_PARTS of them; part p has the type part_type[p] and the body-frame points vertices[part_vertices[p]
+ * .. part_vertices[p + 1]) (x forward, y left, at the robot's position and heading):
+ *   TEB_OBST_POINT     1 point;
+ *   TEB_OBST_CIRCULAR  1 point, the centre, and part_radius[p] > 0 (the only part whose radius is read);
+ *   TEB_OBST_LINE      2 points;
+ *   TEB_OBST_POLYGON   3 or more points, not closed (the last is not Eigen-isApprox(1e-12) equal to the first).
+ * A kind has at most TEB_FLEET_MAX_KIND_VERTICES points in all (TebCostmapWorld's footprint limit). Every point and
+ * radius is finite.
+ *
+ * The neighbours of every robot, their order and the list of min(max_rows, C_cap - own) kept are exactly those of the
+ * circle steps on the same inputs (same world, d2 <= range^2 on the centres, (d2, q) order, either search). Then, with
+ * own = own_count[s] and vown = own_vertex_count[s] (0 for NULL): the longest prefix q_1 .. q_n of the kept list whose
+ * parts fit in C_cap - own rows and whose Line / Polygon points fit in PV_cap - vown vertices is written (a neighbour
+ * that does not fit ends the list: a smaller one behind it is not taken). Neighbour q_i's parts go, in library order, to
+ * the next rows from custom[s][own], its Line / Polygon points, in library order, to the next vertices from
+ * custom_vertices[s][vown] (vertex_begin / vertex_count of the row point at them). A body point u is placed at
+ * p + R(theta) u: x + (c ux - s uy), y + (s ux + c uy), every product and sum rounded on its own, with the sin / cos of
+ * the circle rows' velocity; u = (0, 0) exactly gives p unchanged. A row's (x, y) is its placed point (Point, Circular),
+ * the midpoint 0.5 (a + b) of its placed ends (Line: LineObstacle::calcCentroid), or finalizePolygon of its placed
+ * points (Polygon: the closure check and calcCentroid of TebFrameArgs, vertex_count the points it keeps); radius the
+ * part's (Circular) or 0; vx, vy and dynamic are the robot's circle row's, the same for all its parts (the reference's
+ * constant-velocity model). Rows past own + written parts and vertices past vown + written points are not touched.
+ * custom_count[s] = own + rows written; needed[r] as the circle steps; status TEB_FLEET_TRUNCATED when fewer neighbours
+ * than needed[r] were written. A kind of one Circular part at (0, 0) of radius rho writes the bytes the circle step
+ * writes for radius rho.
+ *
+ * Per-robot arrays (HOST for the host forms, DEVICE for the _device forms): kind[R] the kind of robot r of the array step
+ * and of the publish step; own_vertex_count[S] (or NULL) and custom_vertices[S][PV_cap][2] in / out, the pool
+ * TebFrameArgs.custom_vertices reads (NULL allowed when no kind has a Line or Polygon part); heading[T] and row_kind[T],
+ * the table's companions: the heading and kind of every row, written by the publish step and read by the table step.
+ * A neighbour whose kind is outside 0 .. K - 1 (the device forms do not read device arrays to check it) ends its list as
+ * one that does not fit would; a robot whose own_vertex_count is outside 0 .. PV_cap gets TEB_FLEET_BAD_INPUT.
+ *
+ * Argument errors return TEBGPU_ERR_INVALID_ARG before anything is launched: those of the matching circle step (radius is
+ * not read, except by the publish step, which writes the rows tebgpu_fleet_publish writes), NULL shapes, K outside
+ * 1 .. TEB_FLEET_MAX_KINDS, a malformed library (the rules above), PV_cap < 0, a Line or Polygon part of more points than
+ * PV_cap (the steps that write rows), a NULL per-robot array the step reads; the host forms also refuse a kind or own_vertex_count out of range and
+ * a non-finite heading. */
+#define TEB_FLEET_MAX_KINDS 256
+#define TEB_FLEET_MAX_PARTS 8
+#define TEB_FLEET_MAX_KIND_VERTICES 64
+typedef struct TebFleetShapes {
+  int32_t  K;                  /* kinds, 1 .. TEB_FLEET_MAX_KINDS */
+  int32_t  PV_cap;             /* vertices per scene (stride of custom_vertices, TebFrameArgs.PV_cap), >= 0 */
+  const int32_t* kind_parts;   /* [K + 1] HOST: kind k is parts kind_parts[k] .. kind_parts[k + 1] - 1; kind_parts[0] = 0 */
+  const int32_t* part_type;    /* [P] HOST: TEB_OBST_POINT, _CIRCULAR, _LINE or _POLYGON */
+  const int32_t* part_vertices;/* [P + 1] HOST: part p is points part_vertices[p] .. part_vertices[p + 1] - 1; [0] = 0 */
+  const double*  part_radius;  /* [P] HOST: the Circular parts' radii */
+  const double*  vertices;     /* [V][2] HOST: the points, body frame */
+  const int32_t* kind;         /* [R] the robots' kinds (array and publish steps) */
+  const int32_t* own_vertex_count; /* [S] or NULL: the caller's own vertices of each scene (0 for NULL) */
+  double*        custom_vertices;  /* [S][PV_cap][2] in/out: TebFrameArgs.custom_vertices */
+  double*        heading;      /* [T] the table's headings (publish writes, table step reads) */
+  int32_t*       row_kind;     /* [T] the table's kinds (publish writes, table step reads) */
+} TebFleetShapes;
+
+/* tebgpu_fleet_obstacles_shaped(_device): TebFleetArgs' step, each neighbour written as its kind's parts; radius is not
+ * read. tebgpu_fleet_publish_shaped(_device): tebgpu_fleet_publish's rows, and heading[first + r] = pose[r][2],
+ * row_kind[first + r] = kind[r]. tebgpu_fleet_gather_shaped(_device): tebgpu_fleet_gather of the rows and both
+ * companions (cap entries per rank each), as one NCCL group; nothing with one rank. tebgpu_fleet_obstacles_table_shaped
+ * (_device): tebgpu_fleet_obstacles_table's step, neighbour q written as kind row_kind[q] at its row's position,
+ * heading[q], and its row's velocity and dynamic flag. Host and stream-ordered device forms as the circle steps. */
+int32_t tebgpu_fleet_obstacles_shaped(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetShapes* shapes);
+int32_t tebgpu_fleet_obstacles_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetShapes* shapes,
+                                             void* cuda_stream);
+int32_t tebgpu_fleet_publish_shaped(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetShapes* shapes,
+                                    const TebFleetTable* table);
+int32_t tebgpu_fleet_publish_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetShapes* shapes,
+                                           const TebFleetTable* table, void* cuda_stream);
+int32_t tebgpu_fleet_gather_shaped(tebgpu_ctx* ctx, const TebFleetShapes* shapes, const TebFleetTable* table, int32_t cap);
+int32_t tebgpu_fleet_gather_shaped_device(tebgpu_ctx* ctx, const TebFleetShapes* shapes, const TebFleetTable* table,
+                                          int32_t cap, void* cuda_stream);
+int32_t tebgpu_fleet_obstacles_table_shaped(tebgpu_ctx* ctx, const TebFleetArgs* args, const TebFleetShapes* shapes,
+                                            const TebFleetTable* table);
+int32_t tebgpu_fleet_obstacles_table_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs* args,
+                                                   const TebFleetShapes* shapes, const TebFleetTable* table,
+                                                   void* cuda_stream);
 
 /* Linear solver / scheduling of the LM step (replaces LinearSolverCSparse, optimal_planner.h:75-79):
  * 2 (default) speculative: the next 4 damping trials are solved concurrently, one thread per (band, trial), banded

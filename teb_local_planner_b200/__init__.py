@@ -96,6 +96,14 @@ def load_library(build_if_missing=False):
         getattr(L, name).argtypes = [vp, C.POINTER(abi.TebFleetArgs), C.POINTER(abi.TebFleetTable)]
         getattr(L, name + "_device").restype = C.c_int32
         getattr(L, name + "_device").argtypes = [vp, C.POINTER(abi.TebFleetArgs), C.POINTER(abi.TebFleetTable), vp]
+    FA, FS, FT = C.POINTER(abi.TebFleetArgs), C.POINTER(abi.TebFleetShapes), C.POINTER(abi.TebFleetTable)
+    for name, args in (("tebgpu_fleet_obstacles_shaped", [vp, FA, FS]), ("tebgpu_fleet_publish_shaped", [vp, FA, FS, FT]),
+                       ("tebgpu_fleet_gather_shaped", [vp, FS, FT, C.c_int32]),
+                       ("tebgpu_fleet_obstacles_table_shaped", [vp, FA, FS, FT])):
+        getattr(L, name).restype = C.c_int32
+        getattr(L, name).argtypes = args
+        getattr(L, name + "_device").restype = C.c_int32
+        getattr(L, name + "_device").argtypes = args + [vp]
     L.tebgpu_fleet_gather.restype = C.c_int32
     L.tebgpu_fleet_gather.argtypes = [vp, C.POINTER(abi.TebFleetTable), C.c_int32]
     L.tebgpu_fleet_gather_device.restype = C.c_int32
@@ -170,7 +178,8 @@ def load_library(build_if_missing=False):
     for which, st in tuple(enumerate((abi.TebParams, abi.TebObstacle, abi.TebBatch, abi.TebOptimizeArgs, abi.TebGpuLimits,
                                 abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs,
                                 abi.TebLocalPlanArgs, abi.TebCycleArgs, abi.TebCostmapWorld, abi.TebFrameArgs,
-                                abi.TebHsigFactors, abi.TebFleetArgs))) + ((15, None), (16, abi.TebFleetTable)):
+                                abi.TebHsigFactors, abi.TebFleetArgs))) + ((15, None), (16, abi.TebFleetTable),
+                                                                (17, abi.TebFleetShapes)):
         if st is None:
             if L.tebgpu_sizeof(which) != abi.FLEET_ROW_DTYPE.itemsize:
                 raise RuntimeError(f"ABI mismatch for TebFleetRow: C {L.tebgpu_sizeof(which)} vs FLEET_ROW_DTYPE "
@@ -654,6 +663,124 @@ class TebGpu:
         synchronise."""
         self._check(self.lib.tebgpu_fleet_obstacles_table_device(self.ctx, C.byref(args), C.byref(table), stream),
                     "tebgpu_fleet_obstacles_table_device")
+
+    def fleet_obstacles_shaped(self, kinds, kind, pose, last_cmd, custom, range, max_rows=8, own_count=None,
+                               custom_count=None, world=None, scene=None, custom_vertices=None, own_vertex_count=None):
+        """fleet_obstacles with every neighbour written as its kind's footprint (tebgpu_fleet_obstacles_shaped), host
+        buffers: kinds the shape library (abi.make_fleet_shapes' list), kind [R] each robot's kind, custom_vertices
+        [S][PV_cap][2] the scenes' vertex pools (None: PV_cap 0), own_vertex_count [S] (None: 0); the rest as
+        fleet_obstacles. Returns (custom, custom_count, needed, status, custom_vertices), new arrays."""
+        import numpy as np
+        pose = np.ascontiguousarray(pose, dtype=np.float64).reshape(-1, 3)
+        R = pose.shape[0]
+        i32 = lambda x, shape: None if x is None else np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.int32)
+        out = np.array(custom, dtype=abi.OBST_DTYPE, order="C")
+        S = out.shape[0]
+        out = out.reshape(S, -1)
+        cv = np.zeros((S, 0, 2)) if custom_vertices is None else np.array(custom_vertices, np.float64, order="C").reshape(S, -1, 2)
+        own = i32(own_count, (S,))
+        cc = (np.zeros(S, np.int32) if own is None else own.copy()) if custom_count is None else i32(custom_count, (S,)).copy()
+        keep = dict(cmd=np.ascontiguousarray(np.broadcast_to(last_cmd, (R, 3)), dtype=np.float64), world=i32(world, (R,)),
+                    scene=i32(scene, (R,)), kind=i32(kind, (R,)), ownv=i32(own_vertex_count, (S,)))
+        needed, status = np.full(R, -2, np.int32), np.full(R, -1, np.int32)
+        fa = abi.make_fleet_args(R, S, out.shape[1], max_rows, range, pose=pose, last_cmd=keep["cmd"], world=keep["world"],
+                                 scene=keep["scene"], own_count=own, custom=out if out.size else None, custom_count=cc,
+                                 needed=needed, status=status)
+        sh = abi.make_fleet_shapes(kinds, cv.shape[1], kind=keep["kind"], own_vertex_count=keep["ownv"],
+                                   custom_vertices=cv if cv.size else None)
+        self._check(self.lib.tebgpu_fleet_obstacles_shaped(self.ctx, C.byref(fa), C.byref(sh)),
+                    "tebgpu_fleet_obstacles_shaped")
+        return out, cc, needed, status, cv
+
+    def fleet_obstacles_shaped_device(self, args, shapes, stream=None):
+        """tebgpu_fleet_obstacles_shaped_device: args (abi.TebFleetArgs, radius not read) and the per-robot arrays of
+        shapes (abi.make_fleet_shapes: kind, own_vertex_count, custom_vertices) of device pointers. Stream ordered on
+        `stream` (None: the context's); does not synchronise."""
+        self._check(self.lib.tebgpu_fleet_obstacles_shaped_device(self.ctx, C.byref(args), C.byref(shapes), stream),
+                    "tebgpu_fleet_obstacles_shaped_device")
+
+    def fleet_publish_shaped(self, kinds, kind, pose, last_cmd, radius, rows, heading, row_kind, first=0, world=None):
+        """fleet_publish with the table's companions (tebgpu_fleet_publish_shaped), host buffers: heading [T] float64
+        and row_kind [T] int32 get the robots' headings and kinds at first .. first + R - 1. Returns new (rows, heading,
+        row_kind)."""
+        import numpy as np
+        pose = np.ascontiguousarray(pose, dtype=np.float64).reshape(-1, 3)
+        R = pose.shape[0]
+        out = np.array(rows, dtype=abi.FLEET_ROW_DTYPE, order="C").reshape(-1)
+        hd = np.array(heading, np.float64, order="C").reshape(-1)
+        rk = np.array(row_kind, np.int32, order="C").reshape(-1)
+        keep = dict(cmd=np.ascontiguousarray(np.broadcast_to(last_cmd, (R, 3)), dtype=np.float64),
+                    rad=np.ascontiguousarray(np.broadcast_to(radius, (R,)), dtype=np.float64),
+                    world=None if world is None else np.ascontiguousarray(np.broadcast_to(world, (R,)), dtype=np.int32),
+                    kind=np.ascontiguousarray(np.broadcast_to(kind, (R,)), dtype=np.int32))
+        fa = abi.make_fleet_args(R, 1, 0, 0, 0.0, pose=pose, last_cmd=keep["cmd"], radius=keep["rad"], world=keep["world"])
+        sh = abi.make_fleet_shapes(kinds, 0, kind=keep["kind"], heading=hd if hd.size else None,
+                                   row_kind=rk if rk.size else None)
+        tb = abi.make_fleet_table(len(out), first, out if out.size else None)
+        self._check(self.lib.tebgpu_fleet_publish_shaped(self.ctx, C.byref(fa), C.byref(sh), C.byref(tb)),
+                    "tebgpu_fleet_publish_shaped")
+        return out, hd, rk
+
+    def fleet_publish_shaped_device(self, args, shapes, table, stream=None):
+        """tebgpu_fleet_publish_shaped_device: args, shapes (kind, heading, row_kind) and table of device pointers.
+        Stream ordered on `stream` (None: the context's); does not synchronise."""
+        self._check(self.lib.tebgpu_fleet_publish_shaped_device(self.ctx, C.byref(args), C.byref(shapes), C.byref(table),
+                                                                stream), "tebgpu_fleet_publish_shaped_device")
+
+    def fleet_gather_shaped(self, kinds, rows, heading, row_kind, cap):
+        """tebgpu_fleet_gather_shaped on a host table and its companions. Returns new (rows, heading, row_kind)."""
+        import numpy as np
+        out = np.array(rows, dtype=abi.FLEET_ROW_DTYPE, order="C").reshape(-1)
+        hd = np.array(heading, np.float64, order="C").reshape(-1)
+        rk = np.array(row_kind, np.int32, order="C").reshape(-1)
+        sh = abi.make_fleet_shapes(kinds, 0, heading=hd if hd.size else None, row_kind=rk if rk.size else None)
+        tb = abi.make_fleet_table(len(out), 0, out if out.size else None)
+        self._check(self.lib.tebgpu_fleet_gather_shaped(self.ctx, C.byref(sh), C.byref(tb), int(cap)),
+                    "tebgpu_fleet_gather_shaped")
+        return out, hd, rk
+
+    def fleet_gather_shaped_device(self, shapes, table, cap, stream=None):
+        """tebgpu_fleet_gather_shaped_device: the in-place all-gather of a device table and its companions (shapes'
+        heading and row_kind) as one NCCL group; nothing without a communicator"""
+        self._check(self.lib.tebgpu_fleet_gather_shaped_device(self.ctx, C.byref(shapes), C.byref(table), int(cap), stream),
+                    "tebgpu_fleet_gather_shaped_device")
+
+    def fleet_obstacles_table_shaped(self, kinds, rows, heading, row_kind, first, R, custom, range, max_rows=8,
+                                     own_count=None, custom_count=None, scene=None, custom_vertices=None,
+                                     own_vertex_count=None):
+        """fleet_obstacles_table with every neighbour written as its kind's footprint
+        (tebgpu_fleet_obstacles_table_shaped), host buffers: heading [T], row_kind [T] the table's companions, the rest
+        as fleet_obstacles_shaped / fleet_obstacles_table. Returns (custom, custom_count, needed, status,
+        custom_vertices)."""
+        import numpy as np
+        rows = np.ascontiguousarray(rows, dtype=abi.FLEET_ROW_DTYPE).reshape(-1)
+        hd = np.ascontiguousarray(heading, np.float64).reshape(-1)
+        rk = np.ascontiguousarray(row_kind, np.int32).reshape(-1)
+        i32 = lambda x, shape: None if x is None else np.ascontiguousarray(np.broadcast_to(x, shape), dtype=np.int32)
+        out = np.array(custom, dtype=abi.OBST_DTYPE, order="C")
+        S = out.shape[0]
+        out = out.reshape(S, -1)
+        cv = np.zeros((S, 0, 2)) if custom_vertices is None else np.array(custom_vertices, np.float64, order="C").reshape(S, -1, 2)
+        own = i32(own_count, (S,))
+        cc = (np.zeros(S, np.int32) if own is None else own.copy()) if custom_count is None else i32(custom_count, (S,)).copy()
+        sc, ownv = i32(scene, (int(R),)), i32(own_vertex_count, (S,))
+        needed, status = np.full(int(R), -2, np.int32), np.full(int(R), -1, np.int32)
+        fa = abi.make_fleet_args(R, S, out.shape[1], max_rows, range, scene=sc, own_count=own,
+                                 custom=out if out.size else None, custom_count=cc, needed=needed, status=status)
+        sh = abi.make_fleet_shapes(kinds, cv.shape[1], own_vertex_count=ownv, custom_vertices=cv if cv.size else None,
+                                   heading=hd if hd.size else None, row_kind=rk if rk.size else None)
+        tb = abi.make_fleet_table(len(rows), first, rows if rows.size else None)
+        self._check(self.lib.tebgpu_fleet_obstacles_table_shaped(self.ctx, C.byref(fa), C.byref(sh), C.byref(tb)),
+                    "tebgpu_fleet_obstacles_table_shaped")
+        return out, cc, needed, status, cv
+
+    def fleet_obstacles_table_shaped_device(self, args, shapes, table, stream=None):
+        """tebgpu_fleet_obstacles_table_shaped_device: args, shapes (own_vertex_count, custom_vertices, heading,
+        row_kind) and table of device pointers. Stream ordered on `stream` (None: the context's); does not
+        synchronise."""
+        self._check(self.lib.tebgpu_fleet_obstacles_table_shaped_device(self.ctx, C.byref(args), C.byref(shapes),
+                                                                        C.byref(table), stream),
+                    "tebgpu_fleet_obstacles_table_shaped_device")
 
     def last_fleet_grid(self):
         """grid in CTAs (16 robots each) of the last fleet-obstacle launch, 0 before the first"""

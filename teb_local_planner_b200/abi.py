@@ -398,6 +398,81 @@ def make_fleet_table(T, first, rows) -> TebFleetTable:
     return t
 
 
+class TebFleetShapes(C.Structure):
+    """The shape library of the _shaped fleet steps (include/teb_b200.h): K kinds of parts (Point, Circular, Line,
+    Polygon) in the robot's body frame as HOST arrays, and the per-robot arrays (kind [R], own_vertex_count [S],
+    custom_vertices [S][PV_cap][2], the table's heading [T] / row_kind [T]) as host or device pointers"""
+    _fields_ = [("K", _i), ("PV_cap", _i), ("kind_parts", C.c_void_p), ("part_type", C.c_void_p),
+                ("part_vertices", C.c_void_p), ("part_radius", C.c_void_p), ("vertices", C.c_void_p),
+                ("kind", C.c_void_p), ("own_vertex_count", C.c_void_p), ("custom_vertices", C.c_void_p),
+                ("heading", C.c_void_p), ("row_kind", C.c_void_p)]
+
+
+TEB_FLEET_MAX_KINDS, TEB_FLEET_MAX_PARTS, TEB_FLEET_MAX_KIND_VERTICES = 256, 8, 64
+
+
+def _addr(v):
+    if hasattr(v, "data_ptr"):
+        return v.data_ptr()
+    if isinstance(v, np.ndarray):
+        return ptr(v)
+    return v
+
+
+def make_fleet_shapes(kinds, PV_cap=0, **arrays) -> TebFleetShapes:
+    """TebFleetShapes of the library `kinds`: a list of kinds, each a list of parts (type, points, radius=0.0), type a
+    TEB_OBST_POINT / _CIRCULAR / _LINE / _POLYGON, points [n][2] in the body frame (x forward, y left). The per-robot
+    arrays are given by keyword (kind=..., own_vertex_count=..., custom_vertices=..., heading=..., row_kind=...) as
+    addresses (ints), torch tensors (their data_ptr()), numpy arrays (their buffer; keep them alive) or None for NULL. The
+    returned struct keeps the library's arrays alive."""
+    kind_parts, part_type, part_vertices, part_radius, verts = [0], [], [0], [], []
+    for parts in kinds:
+        for part in parts:
+            typ, pts = part[0], np.asarray(part[1], np.float64).reshape(-1, 2)
+            part_type.append(int(typ))
+            part_radius.append(float(part[2]) if len(part) > 2 else 0.0)
+            verts.append(pts)
+            part_vertices.append(part_vertices[-1] + len(pts))
+        kind_parts.append(len(part_type))
+    lib = dict(kind_parts=np.asarray(kind_parts, np.int32), part_type=np.asarray(part_type, np.int32),
+               part_vertices=np.asarray(part_vertices, np.int32), part_radius=np.asarray(part_radius, np.float64),
+               vertices=np.ascontiguousarray(np.concatenate(verts) if verts else np.zeros((0, 2))))
+    sh = TebFleetShapes()
+    sh.K, sh.PV_cap = len(kinds), int(PV_cap)
+    for k, v in lib.items():
+        setattr(sh, k, ptr(v) if v.size else None)
+    names = {f[0] for f in TebFleetShapes._fields_[7:]}
+    for k, v in arrays.items():
+        if k not in names:
+            raise TypeError(f"unknown TebFleetShapes array {k}")
+        setattr(sh, k, _addr(v))
+    sh._keep = lib
+    return sh
+
+
+def fleet_shape_from_params(params):
+    """The kind (a list of parts for make_fleet_shapes) of a robot with the footprint model of `params` (TebParams):
+    Point: one point; Circular: one circle of footprint_radius; TwoCircles: circles at (+front_offset, 0) and
+    (-rear_offset, 0) of their radii (a radius of 0 gives a point); Line: its two ends; Polygon: its vertices."""
+    t = params.footprint_type
+    if t == TEB_FOOTPRINT_POINT:
+        return [(TEB_OBST_POINT, [[0.0, 0.0]])]
+    if t == TEB_FOOTPRINT_CIRCULAR:
+        return [(TEB_OBST_CIRCULAR, [[0.0, 0.0]], params.footprint_radius)]
+    if t == TEB_FOOTPRINT_TWO_CIRCLES:
+        circle = lambda x, r: (TEB_OBST_CIRCULAR, [[x, 0.0]], r) if r > 0 else (TEB_OBST_POINT, [[x, 0.0]])
+        return [circle(params.footprint_front_offset, params.footprint_front_radius),
+                circle(-params.footprint_rear_offset, params.footprint_rear_radius)]
+    if t == TEB_FOOTPRINT_LINE:
+        ln = list(params.footprint_line)
+        return [(TEB_OBST_LINE, [ln[0:2], ln[2:4]])]
+    if t == TEB_FOOTPRINT_POLYGON:
+        n = params.footprint_vertex_count
+        v = list(params.footprint_vertices)
+        return [(TEB_OBST_POLYGON, [v[2 * i:2 * i + 2] for i in range(n)])]
+    raise ValueError(f"unknown footprint type {t}")
+
+
 class TebGpuLimits(C.Structure):
     _fields_ = [("max_bands", _i), ("max_poses", _i), ("max_scenes", _i), ("max_obstacles", _i),
                 ("max_viapoints", _i), ("max_obst_vertices", _i)]

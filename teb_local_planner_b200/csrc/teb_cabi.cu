@@ -151,6 +151,10 @@ struct tebgpu_ctx {
   /* the fleet grid: bucket counts and starts, candidate keys, ranks and indices, the far list and the scan's
    * temporary storage, in one buffer grown by the first call that needs more */
   char* d_fgrid = nullptr; size_t fgrid_bytes = 0;
+  /* the shaped fleet steps' library: the device copy of the last library sent, and its bytes on the host, compared
+   * with each call's so that an unchanged library is not sent again */
+  char* d_fshape = nullptr; size_t fshape_bytes = 0;
+  std::vector<char> fshape_sent;
   /* scene H-signatures: the factor table's partial products, the in-call / uploaded factor table, the bands' chunk sums
    * and the host-buffer entry point's output, each grown by the first call that needs more */
   char* d_hsf_part = nullptr; char* d_hsf_tab = nullptr; double* d_hs_part = nullptr; double* d_hs_out = nullptr;
@@ -255,6 +259,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 14: return (int32_t)sizeof(TebFleetArgs);
     case 15: return (int32_t)sizeof(TebFleetRow);
     case 16: return (int32_t)sizeof(TebFleetTable);
+    case 17: return (int32_t)sizeof(TebFleetShapes);
     default: return -1;
   }
 }
@@ -295,7 +300,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
                   c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
-                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid};
+                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid, c->d_fshape};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -2198,8 +2203,12 @@ static int32_t issue_fleet_grid(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStr
 }
 
 /* k_fleet_claim (when scenes are given), then k_fleet_obstacles or the grid and k_fleet_obstacles_grid, on arguments
- * already checked; table: the candidates of tebgpu_fleet_obstacles_table, NULL for the caller's arrays */
-static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st, const TebFleetTable* table = nullptr) {
+ * already checked; table: the candidates of tebgpu_fleet_obstacles_table, NULL for the caller's arrays; writer: what the
+ * kept lists become (FleetCircles or FleetShaped) */
+extern "C++" {
+template <class W = FleetCircles>
+static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st, const TebFleetTable* table = nullptr,
+                           const W& writer = W{}) {
   int32_t rc;
   const int64_t N = table ? table->T : fa->R;
   const int search = fleet_search(ctx, fa, N);
@@ -2215,11 +2224,11 @@ static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t
   }
   const long long grid = ((long long)fa->R + FLEET_WARPS - 1) / FLEET_WARPS;
   if (search == TEBGPU_FLEET_SEARCH_ALL_PAIRS) {
-    if (table) k_fleet_obstacles<true><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table);
-    else k_fleet_obstacles<false><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{});
+    if (table) k_fleet_obstacles<true, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, writer);
+    else k_fleet_obstacles<false, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, writer);
   } else {
-    if (table) k_fleet_obstacles_grid<true><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, g);
-    else k_fleet_obstacles_grid<false><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, g);
+    if (table) k_fleet_obstacles_grid<true, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, g, writer);
+    else k_fleet_obstacles_grid<false, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, g, writer);
   }
   ctx->last_fleet_grid = grid;
   ctx->last_fleet_search = search;
@@ -2228,6 +2237,7 @@ static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t
   CUDA_TRY(ctx, cudaGetLastError());
   return TEBGPU_OK;
 }
+}  // extern "C++"
 
 int32_t tebgpu_fleet_obstacles_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, void* cuda_stream) {
   const int32_t rc = check_fleet_args(ctx, fa);
@@ -2236,11 +2246,11 @@ int32_t tebgpu_fleet_obstacles_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, v
   return issue_fleet(ctx, fa, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
 }
 
-static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table);
+static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table,
+                              const TebFleetShapes* sh = nullptr, const FleetLib* lib = nullptr);
 
-int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
-  int32_t rc = check_fleet_args(ctx, fa);
-  if (rc) return rc;
+/* the host form's checks of its arrays, on arguments that passed check_fleet_args */
+static int32_t check_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
   const size_t R = fa->R, S = fa->S, C = fa->C_cap;
   /* the robots the device entry point would answer with BAD_INPUT / SHARED_SCENE, and every non-finite input, are
    * refused here, before anything runs */
@@ -2258,24 +2268,38 @@ int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
     const int32_t own = fa->own_count ? fa->own_count[s] : 0;
     if (own < 0 || (size_t)own > C) { ctx->err = "own_count[s] outside 0 .. C_cap"; return TEBGPU_ERR_INVALID_ARG; }
   }
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
+  int32_t rc = check_fleet_args(ctx, fa);
+  if (rc || (rc = check_fleet_host(ctx, fa))) return rc;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   return run_fleet_host(ctx, fa, nullptr);
 }
 
 /* the host-buffer fleet steps on arguments already checked: stage the arrays given (NULL ones stay NULL), launch on the
- * context's stream, copy the outputs back and synchronise. table: the device copy of the candidates' table, or NULL */
-static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table) {
+ * context's stream, copy the outputs back and synchronise. table: the device copy of the candidates' table, or NULL.
+ * sh, lib: the shaped steps' host arrays and their library already on the device, or NULL for the circle steps */
+static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table,
+                              const TebFleetShapes* sh, const FleetLib* lib) {
   int32_t rc;
   const size_t R = fa->R, S = fa->S, C = fa->C_cap;
+  const size_t T = table ? table->T : 0, PV = sh ? sh->PV_cap : 0;
   cudaStream_t st = ctx->stream;
   const size_t I = sizeof(int32_t), D = sizeof(double);
-  enum { POSE, CMD, RAD, WORLD, SCENE, OWN, CUSTOM, CCOUNT, NEED, STATUS, SLOTS };
+  enum { POSE, CMD, RAD, WORLD, SCENE, OWN, CUSTOM, CCOUNT, NEED, STATUS, KIND, OWNV, CVERT, HEAD, RKIND, SLOTS };
   CycleSlot sl[SLOTS] = {
       {(void*)fa->pose, R * 3 * D, false, 0},      {(void*)fa->last_cmd, R * 3 * D, false, 0},
       {(void*)fa->radius, R * D, false, 0},        {(void*)fa->world, R * I, false, 0},
       {(void*)fa->scene, R * I, false, 0},         {(void*)fa->own_count, S * I, false, 0},
       {fa->custom, S * C * sizeof(TebObstacle), true, 0}, {fa->custom_count, S * I, true, 0},
-      {fa->needed, R * I, true, 0},                {fa->status, R * I, true, 0}};
+      {fa->needed, R * I, true, 0},                {fa->status, R * I, true, 0},
+      {sh && !table ? (void*)sh->kind : nullptr, R * I, false, 0},
+      {sh ? (void*)sh->own_vertex_count : nullptr, S * I, false, 0},
+      {sh ? (void*)sh->custom_vertices : nullptr, S * PV * 2 * D, true, 0},
+      {sh && table ? (void*)sh->heading : nullptr, T * D, false, 0},
+      {sh && table ? (void*)sh->row_kind : nullptr, T * I, false, 0}};
   size_t off = 0;
   for (CycleSlot& c : sl) {
     c.off = off;
@@ -2292,7 +2316,15 @@ static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const Teb
   da.scene = (const int32_t*)sl[SCENE].dev(d); da.own_count = (const int32_t*)sl[OWN].dev(d);
   da.custom = (TebObstacle*)sl[CUSTOM].dev(d); da.custom_count = (int32_t*)sl[CCOUNT].dev(d);
   da.needed = (int32_t*)sl[NEED].dev(d); da.status = (int32_t*)sl[STATUS].dev(d);
-  if ((rc = issue_fleet(ctx, &da, st, table))) return rc;
+  if (lib) {
+    FleetShaped w{*lib};
+    w.L.kind = (const int32_t*)sl[KIND].dev(d); w.L.own_v = (const int32_t*)sl[OWNV].dev(d);
+    w.L.cv = (double*)sl[CVERT].dev(d); w.L.heading = (double*)sl[HEAD].dev(d); w.L.row_kind = (int32_t*)sl[RKIND].dev(d);
+    rc = issue_fleet(ctx, &da, st, table, w);
+  } else {
+    rc = issue_fleet(ctx, &da, st, table);
+  }
+  if (rc) return rc;
   for (const CycleSlot& c : sl)
     if (c.host && c.out && c.bytes) CUDA_TRY(ctx, cudaMemcpyAsync(c.host, d + c.off, c.bytes, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
@@ -2378,9 +2410,8 @@ int32_t tebgpu_fleet_obstacles_table_device(tebgpu_ctx* ctx, const TebFleetArgs*
   return issue_fleet(ctx, fa, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream, t);
 }
 
-int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
-  int32_t rc = check_fleet_args(ctx, fa, false);
-  if (rc || (rc = check_fleet_table(ctx, fa, t))) return rc;
+/* the host table form's checks of its arrays and rows, on arguments that passed check_fleet_args / check_fleet_table */
+static int32_t check_fleet_table_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
   const size_t R = fa->R, S = fa->S, C = fa->C_cap, T = t->T;
   /* what the device entry point would answer with BAD_INPUT / SHARED_SCENE, and every non-finite live row, are refused
    * here, before anything runs */
@@ -2402,16 +2433,234 @@ int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* fa, co
     const int32_t own = fa->own_count ? fa->own_count[s] : 0;
     if (own < 0 || (size_t)own > C) { ctx->err = "own_count[s] outside 0 .. C_cap"; return TEBGPU_ERR_INVALID_ARG; }
   }
+  return TEBGPU_OK;
+}
+
+/* the host table forms on checked arguments: the table up, then run_fleet_host */
+static int32_t run_fleet_table_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t,
+                                    const TebFleetShapes* sh = nullptr, const FleetLib* lib = nullptr) {
+  int32_t rc;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const size_t bytes = T * sizeof(TebFleetRow);
+  const size_t bytes = (size_t)t->T * sizeof(TebFleetRow);
   if ((rc = grow_mirror(ctx, (void**)&ctx->d_ftable, &ctx->ftable_bytes, bytes, st))) return rc;
   CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_ftable, t->rows, bytes, cudaMemcpyHostToDevice, st));
   const TebFleetTable dt = {t->T, t->first, ctx->d_ftable};
   TebFleetArgs ha = *fa;
   ha.pose = ha.last_cmd = ha.radius = nullptr;
   ha.world = nullptr;
-  return run_fleet_host(ctx, &ha, &dt);
+  return run_fleet_host(ctx, &ha, &dt, sh, lib);
+}
+
+int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
+  int32_t rc = check_fleet_args(ctx, fa, false);
+  if (rc || (rc = check_fleet_table(ctx, fa, t)) || (rc = check_fleet_table_host(ctx, fa, t))) return rc;
+  return run_fleet_table_host(ctx, fa, t);
+}
+
+/* the shaped fleet steps' library (TebFleetShapes): checked, laid out as the device reads it (FleetLib: the parts, the
+ * kinds' part and written-point ranges, the written points) and sent to the context's copy when it differs from the
+ * last library sent. Nothing is launched before it; lib gets the device pointers, K and PV_cap. kind / companions: the
+ * step reads those arrays; rows: it writes rows and vertices (not the publish step), so PV_cap must hold every part */
+static int32_t check_fleet_shape_arrays(tebgpu_ctx* ctx, const TebFleetShapes* sh, bool kind, bool companions,
+                                        bool vertices);
+
+static int32_t stage_fleet_shapes(tebgpu_ctx* ctx, const TebFleetShapes* sh, cudaStream_t st, FleetLib* lib, bool kind,
+                                  bool companions, bool rows = true) {
+  if (!sh) { ctx->err = "fleet shapes == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (sh->K < 1 || sh->K > TEB_FLEET_MAX_KINDS) { ctx->err = "shapes K outside 1 .. TEB_FLEET_MAX_KINDS"; return TEBGPU_ERR_INVALID_ARG; }
+  if (sh->PV_cap < 0) { ctx->err = "shapes PV_cap < 0"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!sh->kind_parts || !sh->part_type || !sh->part_vertices || !sh->vertices) {
+    ctx->err = "missing fleet shape library array"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  const int K = sh->K;
+  if (sh->kind_parts[0] != 0 || sh->part_vertices[0] != 0) { ctx->err = "shape library ranges do not start at 0"; return TEBGPU_ERR_INVALID_ARG; }
+  for (int k = 0; k < K; ++k) {
+    const int n = sh->kind_parts[k + 1] - sh->kind_parts[k];
+    if (n < 1 || n > TEB_FLEET_MAX_PARTS) { ctx->err = "a kind has no parts or more than TEB_FLEET_MAX_PARTS"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  const int P = sh->kind_parts[K];
+  std::vector<FleetPart> parts(P);
+  std::vector<int32_t> kpart(K + 1), kvert(K + 1, 0);
+  std::vector<double> wv;
+  for (int k = 0; k < K; ++k) {
+    kpart[k] = sh->kind_parts[k];
+    int points = 0;
+    for (int p = sh->kind_parts[k]; p < sh->kind_parts[k + 1]; ++p) {
+      const int v0 = sh->part_vertices[p], n = sh->part_vertices[p + 1] - v0, type = sh->part_type[p];
+      const bool one = type == TEB_OBST_POINT || type == TEB_OBST_CIRCULAR;
+      if (v0 < 0 || !((one && n == 1) || (type == TEB_OBST_LINE && n == 2) || (type == TEB_OBST_POLYGON && n >= 3))) {
+        ctx->err = "a part's type or point count is not Point / Circular 1, Line 2, Polygon >= 3"; return TEBGPU_ERR_INVALID_ARG;
+      }
+      points += n;
+      if (points > TEB_FLEET_MAX_KIND_VERTICES) { ctx->err = "a kind has more than TEB_FLEET_MAX_KIND_VERTICES points"; return TEBGPU_ERR_INVALID_ARG; }
+      const double* u = sh->vertices + 2 * (size_t)v0;
+      for (int i = 0; i < 2 * n; ++i)
+        if (!std::isfinite(u[i])) { ctx->err = "a shape point is not finite"; return TEBGPU_ERR_INVALID_ARG; }
+      FleetPart& f = parts[p];
+      f = FleetPart{0.0, 0.0, 0.0, type, 0, 0, 0};
+      if (one) {
+        f.cx = u[0];
+        f.cy = u[1];
+        if (type == TEB_OBST_CIRCULAR) {
+          if (!sh->part_radius || !std::isfinite(sh->part_radius[p]) || !(sh->part_radius[p] > 0.0)) {
+            ctx->err = "a Circular part's radius is not finite and > 0"; return TEBGPU_ERR_INVALID_ARG;
+          }
+          f.radius = sh->part_radius[p];
+        }
+        continue;
+      }
+      if (rows && n > sh->PV_cap) { ctx->err = "a Line / Polygon part has more points than PV_cap"; return TEBGPU_ERR_INVALID_ARG; }
+      if (type == TEB_OBST_POLYGON && teb_eigen_is_approx(u[0], u[1], u[2 * n - 2], u[2 * n - 1])) {
+        ctx->err = "a Polygon part repeats its first point at its end"; return TEBGPU_ERR_INVALID_ARG;
+      }
+      f.nv = n;
+      f.woff = (int32_t)(wv.size() / 2) - kvert[k];
+      wv.insert(wv.end(), u, u + 2 * n);
+    }
+    kvert[k + 1] = (int32_t)(wv.size() / 2);
+  }
+  kpart[K] = P;
+  int32_t rc;
+  if ((rc = check_fleet_shape_arrays(ctx, sh, kind, companions, rows && !wv.empty()))) return rc;
+  /* one buffer: parts, kpart, kvert, points, each 16-byte aligned */
+  auto up16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+  const size_t o1 = up16(P * sizeof(FleetPart)), o2 = o1 + up16((K + 1) * sizeof(int32_t)),
+               o3 = o2 + up16((K + 1) * sizeof(int32_t)), bytes = o3 + wv.size() * sizeof(double);
+  std::vector<char> blob(bytes, 0);
+  std::memcpy(blob.data(), parts.data(), P * sizeof(FleetPart));
+  std::memcpy(blob.data() + o1, kpart.data(), (K + 1) * sizeof(int32_t));
+  std::memcpy(blob.data() + o2, kvert.data(), (K + 1) * sizeof(int32_t));
+  if (!wv.empty()) std::memcpy(blob.data() + o3, wv.data(), wv.size() * sizeof(double));
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  if (blob != ctx->fshape_sent) {
+    if ((rc = grow_mirror(ctx, (void**)&ctx->d_fshape, &ctx->fshape_bytes, bytes, st))) return rc;
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_fshape, blob.data(), bytes, cudaMemcpyHostToDevice, st));
+    ctx->fshape_sent.swap(blob);
+  }
+  const char* d = ctx->d_fshape;
+  *lib = FleetLib{};
+  lib->part = (const FleetPart*)d;
+  lib->kpart = (const int32_t*)(d + o1);
+  lib->kvert = (const int32_t*)(d + o2);
+  lib->wv = (const double*)(d + o3);
+  lib->K = K;
+  lib->PV_cap = sh->PV_cap;
+  lib->kind = sh->kind;
+  lib->own_v = sh->own_vertex_count;
+  lib->cv = sh->custom_vertices;
+  lib->heading = sh->heading;
+  lib->row_kind = sh->row_kind;
+  return TEBGPU_OK;
+}
+
+/* the shapes' per-robot arrays a shaped step reads: kind (array and publish steps), the companions (table, publish and
+ * gather steps), custom_vertices (when some kind writes points) */
+static int32_t check_fleet_shape_arrays(tebgpu_ctx* ctx, const TebFleetShapes* sh, bool kind, bool companions,
+                                        bool vertices) {
+  if ((kind && !sh->kind) || (companions && (!sh->heading || !sh->row_kind)) || (vertices && !sh->custom_vertices)) {
+    ctx->err = "missing fleet shapes array"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  return TEBGPU_OK;
+}
+
+/* the host forms' checks of the per-robot arrays: kinds in 0 .. K - 1 (n of them), own_vertex_count of the robots'
+ * scenes in 0 .. PV_cap */
+static int32_t check_fleet_shape_values(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh,
+                                        const int32_t* kinds, size_t n) {
+  for (size_t q = 0; q < n; ++q)
+    if (kinds[q] < 0 || kinds[q] >= sh->K) { ctx->err = "kind outside 0 .. K - 1"; return TEBGPU_ERR_INVALID_ARG; }
+  if (fa && sh->own_vertex_count)
+    for (int r = 0; r < fa->R; ++r) {
+      const int32_t s = fa->scene ? fa->scene[r] : r;
+      if (s < 0 || s >= fa->S) { ctx->err = "scene[r] outside 0 .. S-1"; return TEBGPU_ERR_INVALID_ARG; }
+      const int32_t v = sh->own_vertex_count[s];
+      if (v < 0 || v > sh->PV_cap) { ctx->err = "own_vertex_count[s] outside 0 .. PV_cap"; return TEBGPU_ERR_INVALID_ARG; }
+    }
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_obstacles_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh,
+                                             void* cuda_stream) {
+  int32_t rc = check_fleet_args(ctx, fa, false);
+  if (rc) return rc;
+  if (!fa->pose || !fa->last_cmd) { ctx->err = "missing required fleet array"; return TEBGPU_ERR_INVALID_ARG; }
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  FleetLib lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, st, &lib, true, false))) return rc;
+  return issue_fleet(ctx, fa, st, nullptr, FleetShaped{lib});
+}
+
+int32_t tebgpu_fleet_obstacles_shaped(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh) {
+  /* the circle step's checks with a radius that is not read */
+  if (!fa) return check_fleet_args(ctx, fa);
+  const size_t R = fa->R > 0 ? fa->R : 0;
+  std::vector<double> zero(R, 0.0);
+  TebFleetArgs ca = *fa;
+  ca.radius = zero.data();
+  int32_t rc = check_fleet_args(ctx, &ca);
+  if (rc || (rc = check_fleet_host(ctx, &ca))) return rc;     /* scenes and own counts first: the checks below read them */
+  FleetLib lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, ctx->stream, &lib, true, false))) return rc;
+  if ((rc = check_fleet_shape_values(ctx, fa, sh, sh->kind, R))) return rc;
+  ca.radius = nullptr;
+  return run_fleet_host(ctx, &ca, nullptr, sh, &lib);
+}
+
+int32_t tebgpu_fleet_publish_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh,
+                                           const TebFleetTable* t, void* cuda_stream) {
+  int32_t rc = check_fleet_publish_args(ctx, fa, t);
+  if (rc) return rc;
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  FleetLib lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, st, &lib, true, true, false))) return rc;
+  k_fleet_publish_shaped<<<(unsigned)((fa->R + CLAIM_THREADS - 1) / CLAIM_THREADS), CLAIM_THREADS, 0, st>>>(*fa, *t, lib);
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_publish_shaped(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh,
+                                    const TebFleetTable* t) {
+  int32_t rc = check_fleet_publish_args(ctx, fa, t);
+  if (rc) return rc;
+  FleetLib lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, ctx->stream, &lib, true, true, false))) return rc;
+  if ((rc = check_fleet_shape_values(ctx, nullptr, sh, sh->kind, fa->R))) return rc;
+  /* the rows are tebgpu_fleet_publish's (k_fleet_publish_shaped writes them through the same fleet_row); the companions
+   * are copies of the inputs */
+  if ((rc = tebgpu_fleet_publish(ctx, fa, t))) return rc;
+  for (int r = 0; r < fa->R; ++r) {
+    sh->heading[t->first + r] = fa->pose[3 * (size_t)r + 2];
+    sh->row_kind[t->first + r] = sh->kind[r];
+  }
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_obstacles_table_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh,
+                                                   const TebFleetTable* t, void* cuda_stream) {
+  int32_t rc = check_fleet_args(ctx, fa, false);
+  if (rc || (rc = check_fleet_table(ctx, fa, t))) return rc;
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  FleetLib lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, st, &lib, false, true))) return rc;
+  return issue_fleet(ctx, fa, st, t, FleetShaped{lib});
+}
+
+int32_t tebgpu_fleet_obstacles_table_shaped(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh,
+                                            const TebFleetTable* t) {
+  int32_t rc = check_fleet_args(ctx, fa, false);
+  if (rc || (rc = check_fleet_table(ctx, fa, t)) || (rc = check_fleet_table_host(ctx, fa, t))) return rc;
+  FleetLib lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, ctx->stream, &lib, false, true))) return rc;
+  std::vector<int32_t> live_kinds;
+  for (int q = 0; q < t->T; ++q) {
+    if (!t->rows[q].live) continue;
+    if (!std::isfinite(sh->heading[q])) { ctx->err = "live fleet row heading not finite"; return TEBGPU_ERR_INVALID_ARG; }
+    live_kinds.push_back(sh->row_kind[q]);
+  }
+  if ((rc = check_fleet_shape_values(ctx, fa, sh, live_kinds.data(), live_kinds.size()))) return rc;
+  return run_fleet_table_host(ctx, fa, t, sh, &lib);
 }
 
 int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args) {
@@ -3142,6 +3391,56 @@ int32_t tebgpu_fleet_gather(tebgpu_ctx* ctx, const TebFleetTable* t, int32_t cap
   CUDA_TRY(ctx, cudaMemcpyAsync(d + mine, (const char*)t->rows + mine, bytes, cudaMemcpyHostToDevice, st));
   NCCL_TRY(ctx, nccl_api().AllGather(d + mine, d, bytes, ncclChar, ctx->comm, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(t->rows, d, all, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* tebgpu_fleet_gather with the table's companions: the rows, headings and kinds of every rank, as one NCCL group */
+static int32_t check_fleet_gather_shaped(tebgpu_ctx* ctx, const TebFleetShapes* sh, const TebFleetTable* t, int32_t cap) {
+  const int32_t rc = check_fleet_gather(ctx, t, cap);
+  if (rc) return rc;
+  if (!sh || !sh->heading || !sh->row_kind) { ctx->err = "fleet shapes or their heading / row_kind == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_gather_shaped_device(tebgpu_ctx* ctx, const TebFleetShapes* sh, const TebFleetTable* t, int32_t cap,
+                                          void* cuda_stream) {
+  const int32_t rc = check_fleet_gather_shaped(ctx, sh, t, cap);
+  if (rc) return rc;
+  if (!ctx->comm) return TEBGPU_OK;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  const size_t n = (size_t)cap, mine = (size_t)ctx->rank * n;
+  NcclApi& api = nccl_api();
+  NCCL_TRY(ctx, api.GroupStart());
+  NCCL_TRY(ctx, api.AllGather(t->rows + mine, t->rows, n * sizeof(TebFleetRow), ncclChar, ctx->comm, st));
+  NCCL_TRY(ctx, api.AllGather(sh->heading + mine, sh->heading, n, ncclDouble, ctx->comm, st));
+  NCCL_TRY(ctx, api.AllGather(sh->row_kind + mine, sh->row_kind, n, ncclInt32, ctx->comm, st));
+  NCCL_TRY(ctx, api.GroupEnd());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_fleet_gather_shaped(tebgpu_ctx* ctx, const TebFleetShapes* sh, const TebFleetTable* t, int32_t cap) {
+  int32_t rc = check_fleet_gather_shaped(ctx, sh, t, cap);
+  if (rc) return rc;
+  if (!ctx->comm) return TEBGPU_OK;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t n = (size_t)cap, T = n * ctx->world, mine = (size_t)ctx->rank * n;
+  const size_t rows_b = (T * sizeof(TebFleetRow) + 255) & ~(size_t)255, head_b = (T * sizeof(double) + 255) & ~(size_t)255;
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_fleet, &ctx->fleet_bytes, rows_b + head_b + T * sizeof(int32_t), st))) return rc;
+  TebFleetTable dt = *t;
+  dt.rows = (TebFleetRow*)ctx->d_fleet;
+  TebFleetShapes ds = *sh;
+  ds.heading = (double*)(ctx->d_fleet + rows_b);
+  ds.row_kind = (int32_t*)(ctx->d_fleet + rows_b + head_b);
+  CUDA_TRY(ctx, cudaMemcpyAsync(dt.rows + mine, t->rows + mine, n * sizeof(TebFleetRow), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ds.heading + mine, sh->heading + mine, n * sizeof(double), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(ds.row_kind + mine, sh->row_kind + mine, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if ((rc = tebgpu_fleet_gather_shaped_device(ctx, &ds, &dt, cap, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(t->rows, dt.rows, T * sizeof(TebFleetRow), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(sh->heading, ds.heading, T * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(sh->row_kind, ds.row_kind, T * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
 }

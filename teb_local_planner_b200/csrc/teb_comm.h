@@ -24,6 +24,8 @@ struct NcclApi {
   ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
   ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
   ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*GroupStart)() = nullptr;
+  ncclResult_t (*GroupEnd)() = nullptr;
   const char* (*GetErrorString)(ncclResult_t) = nullptr;
   ncclResult_t (*GetVersion)(int*) = nullptr;
   std::string error;
@@ -49,6 +51,8 @@ inline NcclApi& nccl_api() {
     api.CommInitRank = reinterpret_cast<decltype(api.CommInitRank)>(sym("ncclCommInitRank"));
     api.CommDestroy = reinterpret_cast<decltype(api.CommDestroy)>(sym("ncclCommDestroy"));
     api.AllGather = reinterpret_cast<decltype(api.AllGather)>(sym("ncclAllGather"));
+    api.GroupStart = reinterpret_cast<decltype(api.GroupStart)>(sym("ncclGroupStart"));
+    api.GroupEnd = reinterpret_cast<decltype(api.GroupEnd)>(sym("ncclGroupEnd"));
     api.GetErrorString = reinterpret_cast<decltype(api.GetErrorString)>(sym("ncclGetErrorString"));
     api.GetVersion = reinterpret_cast<decltype(api.GetVersion)>(sym("ncclGetVersion"));
   });

@@ -11,6 +11,11 @@
  *   k_fleet_obstacles_grid  one warp per robot, as k_fleet_obstacles: the candidates of the buckets of the robot's 3 x 3
  *                           cells and of the far list
  *   k_fleet_publish         one thread per robot: the robot's TebFleetRow (tebgpu_fleet_publish)
+ *   k_fleet_publish_shaped  the same, and the row's heading and kind in the table's companions
+ *
+ * Both search kernels take a writer, what the kept list becomes: FleetCircles, one TEB_OBST_CIRCULAR row per neighbour
+ * (the circle steps), or FleetShaped, each neighbour as its kind's parts from a TebFleetShapes library (the _shaped
+ * steps). The contract is at TebFleetShapes in include/teb_b200.h.
  *
  * The CTA stages FLEET_TILE robots' (x, y, world) at a time (the table build (x, y, world, live)); lane l of a warp tests candidates l, l + 32, ... of the
  * tile against its robot, and the warp keeps the nearest min(max_rows, C_cap - own) neighbours as a list sorted by
@@ -32,6 +37,8 @@
 #include <climits>
 #include <cmath>
 
+#include "teb_frame.h"
+
 namespace tebgpu {
 
 constexpr int FLEET_WARPS = 16;                    /* robots per CTA */
@@ -47,26 +54,32 @@ __device__ __forceinline__ bool fleet_less(double da, int qa, double db, int qb)
   return da < db || (da == db && qa < qb);
 }
 
-/* the row robot q is published as, from its pose (x, y, theta), body command (vx, vy) and radius: the publisher's
- * map-frame velocity R(theta) (vx, vy), then setCentroidVelocity's rule (obstacles.h:214-233), Eigen's norm() =
+/* the map-frame velocity a robot is published with, from its body command (bx, by) and sn, cs = sin, cos of its
+ * heading: R(theta) (bx, by), then setCentroidVelocity's rule (obstacles.h:214-233), Eigen's norm() =
  * sqrt(squaredNorm()), of the body command: the rotation keeps the norm, and so the decision does not depend on the last
- * bits of sin / cos. Both the array build of k_fleet_obstacles and k_fleet_publish write their rows from here. */
+ * bits of sin / cos. dyn: 1 moving, 0 still with (0, 0). */
+__device__ __forceinline__ void fleet_velocity(double bx, double by, double sn, double cs, double& vx, double& vy,
+                                               int& dyn) {
+  vx = __dsub_rn(__dmul_rn(cs, bx), __dmul_rn(sn, by));
+  vy = __dadd_rn(__dmul_rn(sn, bx), __dmul_rn(cs, by));
+  const bool moving = !(sqrt(__dadd_rn(__dmul_rn(bx, bx), __dmul_rn(by, by))) < 0.001);
+  if (!moving) vx = vy = 0.0;
+  dyn = moving ? 1 : 0;
+}
+
+/* the row robot q is published as, from its pose (x, y, theta), body command (vx, vy) and radius, with fleet_velocity.
+ * The array build of k_fleet_obstacles, k_fleet_publish and k_fleet_publish_shaped write their rows from here, and the
+ * shaped writer takes its velocities from fleet_velocity with the same sincos. */
 __device__ __forceinline__ TebFleetRow fleet_row(const double* pose, const double* cmd, const double* radius, int world) {
   const double th = pose[2], bx = cmd[0], by = cmd[1];
   double sn, cs;
   sincos(th, &sn, &cs);
-  double vx = __dsub_rn(__dmul_rn(cs, bx), __dmul_rn(sn, by));
-  double vy = __dadd_rn(__dmul_rn(sn, bx), __dmul_rn(cs, by));
-  const bool moving = !(sqrt(__dadd_rn(__dmul_rn(bx, bx), __dmul_rn(by, by))) < 0.001);
-  if (!moving) vx = vy = 0.0;
   TebFleetRow w;
+  fleet_velocity(bx, by, sn, cs, w.vx, w.vy, w.dynamic);
   w.x = pose[0];
   w.y = pose[1];
-  w.vx = vx;
-  w.vy = vy;
   w.radius = *radius;
   w.world = world;
-  w.dynamic = moving ? 1 : 0;
   w.live = 1;
   w._pad[0] = w._pad[1] = w._pad[2] = 0;
   return w;
@@ -155,11 +168,214 @@ __device__ __forceinline__ FleetRobot fleet_robot(const TebFleetArgs& a, const i
     }                                                                                        \
   } while (0)
 
-/* the outputs of the warp's robot r < R: the first min(needed, K) slots of its list (kq, slot `lane`) as rows of its
- * scene, custom_count, needed and status; a robot that does not write gets needed -1 and its status */
-template <bool TABLE>
+/* the writers of fleet_finish: what a kept list becomes. FleetCircles: each neighbour one TEB_OBST_CIRCULAR row of its
+ * radius (the circle steps); FleetShaped: each neighbour its kind's parts (the _shaped steps). */
+struct FleetCircles {
+  static constexpr int MIN_CTAS = 0;   /* __launch_bounds__' minimum CTAs per SM: 0 leaves it to ptxas (40 registers) */
+  /* the first min(needed, K) slots of the list (kq, slot `lane`) as rows of the robot's scene, custom_count, needed and
+   * status */
+  template <bool TABLE>
+  __device__ __forceinline__ void write(const TebFleetArgs& a, const TebFleetTable& t, const FleetRobot& m, int r,
+                                        int lane, int kq, int needed) const {
+    const int written = min(needed, m.K);
+    if (lane < written) {
+      const size_t q = (size_t)kq;
+      /* the neighbour's row: copied from the table as it was published, or made here from the caller's arrays */
+      const TebFleetRow w = TABLE ? t.rows[q] : fleet_row(a.pose + 3 * q, a.last_cmd + 3 * q, a.radius + q, 0);
+      TebObstacle o;
+      o.x = w.x;
+      o.y = w.y;
+      o.vx = w.vx;
+      o.vy = w.vy;
+      o.radius = w.radius;
+      o.dynamic = w.dynamic;
+      o.type = TEB_OBST_CIRCULAR;
+      o.vertex_begin = 0;
+      o.vertex_count = 0;
+      o._pad = 0.0;
+      a.custom[(size_t)m.s * a.C_cap + m.own + lane] = o;
+    }
+    if (lane == 0) {
+      a.custom_count[m.s] = m.own + written;
+      if (a.needed) a.needed[r] = needed;
+      if (a.status) a.status[r] = written < needed ? TEB_FLEET_TRUNCATED : TEB_FLEET_WRITTEN;
+    }
+  }
+};
+
+/* one part of a shape library as the device reads it: its type, the radius (Circular), the body point (Point, Circular),
+ * and for Line / Polygon its point count and offset among its kind's written points */
+struct FleetPart {
+  double cx, cy, radius;
+  int32_t type, nv, woff, _pad;
+};
+
+/* a TebFleetShapes library on the device (the context's copy, built by the launcher in teb_cabi.cu) and the call's
+ * per-robot arrays */
+struct FleetLib {
+  const FleetPart* part;       /* [P] */
+  const int32_t* kpart;        /* [K + 1] kind k is parts kpart[k] .. kpart[k + 1] - 1 */
+  const int32_t* kvert;        /* [K + 1] kind k writes the points wv[kvert[k] .. kvert[k + 1]) */
+  const double* wv;            /* [.][2] the Line / Polygon points of every kind, kind by kind, part by part */
+  int K, PV_cap;
+  const int32_t* kind;         /* TebFleetShapes' per-robot arrays */
+  const int32_t* own_v;
+  double* cv;
+  double* heading;
+  int32_t* row_kind;
+};
+
+constexpr int FLEET_NO_FIT = 1 << 20;   /* the parts of a neighbour of an unknown kind: more than any scene holds */
+
+/* body point (ux, uy) of a robot at (x, y) with sin / cos (sn, cs) of its heading: p + R(theta) u, every operation
+ * rounded on its own; (0, 0) gives p unchanged */
+__device__ __forceinline__ void fleet_place(double x, double y, double sn, double cs, double ux, double uy, double& px,
+                                            double& py) {
+  if (ux == 0.0 && uy == 0.0) {
+    px = x;
+    py = y;
+    return;
+  }
+  px = __dadd_rn(x, __dsub_rn(__dmul_rn(cs, ux), __dmul_rn(sn, uy)));
+  py = __dadd_rn(y, __dadd_rn(__dmul_rn(sn, ux), __dmul_rn(cs, uy)));
+}
+
+struct FleetShaped {
+  /* one CTA per SM: under ptxas' default bound of 64 registers for 512 threads the writer spills; with one CTA the
+   * instantiations take 118 / 120 registers and spill nothing */
+  static constexpr int MIN_CTAS = 1;
+  FleetLib L;
+  /* lane i holds slot i: its kind's part and point counts, inclusive warp scans of both, and the longest prefix of the
+   * kept list that fits the scene's rows and vertices; then neighbour by neighbour, the lanes place its points (lane v
+   * point v) and write its parts (lane p part p); then the Line / Polygon rows take their centroids from the points */
+  template <bool TABLE>
+  __device__ __forceinline__ void write(const TebFleetArgs& a, const TebFleetTable& t, const FleetRobot& m, int r,
+                                        int lane, int kq, int needed) const {
+    constexpr unsigned FULL = 0xffffffffu;
+    const int vown = L.own_v ? L.own_v[m.s] : 0;
+    if (vown < 0 || vown > L.PV_cap) {
+      if (lane == 0) {
+        if (a.needed) a.needed[r] = -1;
+        if (a.status) a.status[r] = TEB_FLEET_BAD_INPUT;
+      }
+      return;
+    }
+    const int listed = min(needed, m.K);
+    /* lane i < listed: its neighbour's kind and the sin / cos of its heading, taken first, while little else is live
+     * across sincos' call to its slow path */
+    int kd = 0, np = 0, nv = 0;
+    double sn = 0.0, cs = 1.0;
+    if (lane < listed) {
+      kd = TABLE ? L.row_kind[kq] : L.kind[kq];
+      sincos(TABLE ? L.heading[kq] : a.pose[3 * (size_t)kq + 2], &sn, &cs);
+      if (kd >= 0 && kd < L.K) {
+        np = __ldg(L.kpart + kd + 1) - __ldg(L.kpart + kd);
+        nv = __ldg(L.kvert + kd + 1) - __ldg(L.kvert + kd);
+      } else {
+        np = FLEET_NO_FIT;
+      }
+    }
+    int sp = np, sv = nv;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int up = __shfl_up_sync(FULL, sp, o), uv = __shfl_up_sync(FULL, sv, o);
+      if (lane >= o) {
+        sp += up;
+        sv += uv;
+      }
+    }
+    /* sp and sv grow with the lane, so the lanes that fit are a prefix */
+    const bool fits = lane < listed && sp <= a.C_cap - m.own && sv <= L.PV_cap - vown;
+    const int n = __popc(__ballot_sync(FULL, fits));
+    /* lane i < n: its neighbour's position and velocity, the circle row's */
+    double x = 0.0, y = 0.0, vx = 0.0, vy = 0.0;
+    int dyn = 0;
+    if (lane < n) {
+      const size_t q = (size_t)kq;
+      if constexpr (TABLE) {
+        const TebFleetRow& w = t.rows[q];
+        x = w.x;
+        y = w.y;
+        vx = w.vx;
+        vy = w.vy;
+        dyn = w.dynamic;
+      } else {
+        x = a.pose[3 * q];
+        y = a.pose[3 * q + 1];
+        fleet_velocity(a.last_cmd[3 * q], a.last_cmd[3 * q + 1], sn, cs, vx, vy, dyn);
+      }
+    }
+    const int rb = m.own + sp - np, vb = vown + sv - nv;
+    const size_t srow = (size_t)m.s * a.C_cap;
+    double* const cv = L.cv + (size_t)m.s * L.PV_cap * 2;
+    for (int j = 0; j < n; ++j) {
+      const double jx = __shfl_sync(FULL, x, j), jy = __shfl_sync(FULL, y, j);
+      const double jsn = __shfl_sync(FULL, sn, j), jcs = __shfl_sync(FULL, cs, j);
+      const int jk = __shfl_sync(FULL, kd, j), jnv = __shfl_sync(FULL, nv, j), jvb = __shfl_sync(FULL, vb, j);
+      const int w0 = __ldg(L.kvert + jk);
+      for (int v = lane; v < jnv; v += 32) {
+        const double2 u = __ldg(reinterpret_cast<const double2*>(L.wv) + w0 + v);
+        double px, py;
+        fleet_place(jx, jy, jsn, jcs, u.x, u.y, px, py);
+        cv[2 * (size_t)(jvb + v)] = px;
+        cv[2 * (size_t)(jvb + v) + 1] = py;
+      }
+      const double jvx = __shfl_sync(FULL, vx, j), jvy = __shfl_sync(FULL, vy, j);
+      const int jdyn = __shfl_sync(FULL, dyn, j), jnp = __shfl_sync(FULL, np, j), jrb = __shfl_sync(FULL, rb, j);
+      if (lane < jnp) {
+        const FleetPart& P = L.part[__ldg(L.kpart + jk) + lane];
+        TebObstacle o;
+        o.vx = jvx;
+        o.vy = jvy;
+        o.radius = 0.0;
+        o.dynamic = jdyn;
+        o.type = __ldg(&P.type);
+        o.vertex_begin = 0;
+        o.vertex_count = 0;
+        o._pad = 0.0;
+        if (o.type == TEB_OBST_POINT || o.type == TEB_OBST_CIRCULAR) {
+          if (o.type == TEB_OBST_CIRCULAR) o.radius = __ldg(&P.radius);
+          fleet_place(jx, jy, jsn, jcs, __ldg(&P.cx), __ldg(&P.cy), o.x, o.y);
+        } else {
+          o.x = o.y = 0.0;   /* the centroid, below */
+          o.vertex_begin = jvb + __ldg(&P.woff);
+          o.vertex_count = __ldg(&P.nv);
+        }
+        a.custom[srow + jrb + lane] = o;
+      }
+    }
+    const int total = n ? __shfl_sync(FULL, sp, n - 1) : 0;
+    /* the Line / Polygon rows' centroids from their placed points, row by row over the lanes: apart from the loop above,
+     * where the calls of the division and the square root would have its state live across them */
+    __syncwarp();
+    for (int i = lane; i < total; i += 32) {
+      TebObstacle& o = a.custom[srow + m.own + i];
+      if (o.type != TEB_OBST_LINE && o.type != TEB_OBST_POLYGON) continue;
+      const double* d = cv + 2 * (size_t)o.vertex_begin;
+      if (o.type == TEB_OBST_LINE) {
+        o.x = teb_mul(0.5, teb_add(d[0], d[2]));
+        o.y = teb_mul(0.5, teb_add(d[1], d[3]));
+        continue;
+      }
+      int k = o.vertex_count;   /* finalizePolygon, as TebFrameArgs' step finalises a moved polygon */
+      if (teb_eigen_is_approx(d[0], d[1], d[2 * k - 2], d[2 * k - 1])) --k;
+      double c[2];
+      teb_polygon_centroid(d, k, c);
+      o.x = c[0];
+      o.y = c[1];
+      o.vertex_count = k;
+    }
+    if (lane == 0) {
+      a.custom_count[m.s] = m.own + total;
+      if (a.needed) a.needed[r] = needed;
+      if (a.status) a.status[r] = n < needed ? TEB_FLEET_TRUNCATED : TEB_FLEET_WRITTEN;
+    }
+  }
+};
+
+/* the outputs of the warp's robot r < R through the writer w; a robot that does not write gets needed -1 and its status */
+template <bool TABLE, class W>
 __device__ __forceinline__ void fleet_finish(const TebFleetArgs& a, const TebFleetTable& t, const FleetRobot& m, int r,
-                                             int lane, int kq, int needed) {
+                                             int lane, int kq, int needed, const W& w) {
   if (!m.valid) {
     if (lane == 0) {
       if (a.needed) a.needed[r] = -1;
@@ -167,36 +383,14 @@ __device__ __forceinline__ void fleet_finish(const TebFleetArgs& a, const TebFle
     }
     return;
   }
-  const int written = min(needed, m.K);
-  if (lane < written) {
-    const size_t q = (size_t)kq;
-    /* the neighbour's row: copied from the table as it was published, or made here from the caller's arrays */
-    const TebFleetRow w = TABLE ? t.rows[q] : fleet_row(a.pose + 3 * q, a.last_cmd + 3 * q, a.radius + q, 0);
-    TebObstacle o;
-    o.x = w.x;
-    o.y = w.y;
-    o.vx = w.vx;
-    o.vy = w.vy;
-    o.radius = w.radius;
-    o.dynamic = w.dynamic;
-    o.type = TEB_OBST_CIRCULAR;
-    o.vertex_begin = 0;
-    o.vertex_count = 0;
-    o._pad = 0.0;
-    a.custom[(size_t)m.s * a.C_cap + m.own + lane] = o;
-  }
-  if (lane == 0) {
-    a.custom_count[m.s] = m.own + written;
-    if (a.needed) a.needed[r] = needed;
-    if (a.status) a.status[r] = written < needed ? TEB_FLEET_TRUNCATED : TEB_FLEET_WRITTEN;
-  }
+  w.template write<TABLE>(a, t, m, r, lane, kq, needed);
 }
 
 /* claims: [S] robots per scene from k_fleet_claim, or NULL when TebFleetArgs.scene is NULL (scene r, never shared).
  * TABLE: robot r is row t.first + r of t and the candidates are its T rows; otherwise t is not read. */
-template <bool TABLE>
-__global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFleetArgs a, const int32_t* claims,
-                                                                   const TebFleetTable t) {
+template <bool TABLE, class W = FleetCircles>
+__global__ void __launch_bounds__(FLEET_THREADS, W::MIN_CTAS) k_fleet_obstacles(const TebFleetArgs a, const int32_t* claims,
+                                                                   const TebFleetTable t, const W writer) {
   __shared__ double sx[FLEET_TILE], sy[FLEET_TILE];
   __shared__ int sw[FLEET_TILE];
   __shared__ int sl[TABLE ? FLEET_TILE : 1];
@@ -269,7 +463,7 @@ __global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles(const TebFlee
     }
   }
   if (!live) return;
-  fleet_finish<TABLE>(a, t, FleetRobot{xr, yr, wr, s, own, K, st, valid}, r, lane, kq, needed);
+  fleet_finish<TABLE>(a, t, FleetRobot{xr, yr, wr, s, own, K, st, valid}, r, lane, kq, needed, writer);
 }
 
 /* the grid of one fleet step: context scratch sized by the launcher (teb_cabi.cu issue_fleet_grid) */
@@ -366,9 +560,10 @@ __global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_scatter(const int N, co
 /* k_fleet_obstacles' step with the candidates taken from the grid: the buckets of the robot's 3 x 3 cells (a bucket two
  * cells share is scanned once, so no candidate is met twice) and the far list; a robot in the far list meets every
  * candidate, one never in range none. Every candidate met takes k_fleet_obstacles' exact test and list. */
-template <bool TABLE>
-__global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles_grid(const TebFleetArgs a, const int32_t* claims,
-                                                                        const TebFleetTable t, const FleetGrid g) {
+template <bool TABLE, class W = FleetCircles>
+__global__ void __launch_bounds__(FLEET_THREADS, W::MIN_CTAS) k_fleet_obstacles_grid(const TebFleetArgs a, const int32_t* claims,
+                                                                        const TebFleetTable t, const FleetGrid g,
+                                                                        const W writer) {
   const int lane = threadIdx.x & 31;
   const int r = blockIdx.x * FLEET_WARPS + (threadIdx.x >> 5);
   if (r >= a.R) return;                    /* warp-uniform */
@@ -414,7 +609,7 @@ __global__ void __launch_bounds__(FLEET_THREADS) k_fleet_obstacles_grid(const Te
       for (int q = lane; q - lane < N; q += 32) meet(q < N ? q : -1);
     }
   }
-  fleet_finish<TABLE>(a, t, m, r, lane, kq, needed);
+  fleet_finish<TABLE>(a, t, m, r, lane, kq, needed, writer);
 }
 
 __global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_publish(const TebFleetArgs a, const TebFleetTable t) {
@@ -422,6 +617,17 @@ __global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_publish(const TebFleetA
   if (r >= a.R) return;
   t.rows[(size_t)t.first + r] = fleet_row(a.pose + 3 * (size_t)r, a.last_cmd + 3 * (size_t)r, a.radius + r,
                                           a.world ? a.world[r] : 0);
+}
+
+/* k_fleet_publish's row, and the row's heading and kind in the table's companions (tebgpu_fleet_publish_shaped) */
+__global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_publish_shaped(const TebFleetArgs a, const TebFleetTable t,
+                                                                        const FleetLib L) {
+  const int r = blockIdx.x * CLAIM_THREADS + threadIdx.x;
+  if (r >= a.R) return;
+  const size_t i = (size_t)t.first + r;
+  t.rows[i] = fleet_row(a.pose + 3 * (size_t)r, a.last_cmd + 3 * (size_t)r, a.radius + r, a.world ? a.world[r] : 0);
+  L.heading[i] = a.pose[3 * (size_t)r + 2];
+  L.row_kind[i] = L.kind[r];
 }
 
 }  // namespace tebgpu

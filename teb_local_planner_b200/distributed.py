@@ -11,7 +11,8 @@ stream, include/teb_b200.h). This module only
   * restates selectBestTeb for whole request batches (`select_best_per_request`),
   * offers the same gather over a torch process group for CPU tests (`gather_costs_torch`, gloo),
   * lays out the fleet table of a sharded fleet (`fleet_layout`) and gathers it over a torch process group
-    (`gather_fleet_table_torch`), as tebgpu_fleet_gather does over NCCL.
+    (`gather_fleet_table_torch`, with the shaped steps' heading / row_kind companions), as tebgpu_fleet_gather(_shaped)
+    does over NCCL.
 """
 import ctypes as C
 
@@ -97,17 +98,26 @@ def fleet_layout(counts, world):
     return cap, [g * cap for g in range(world)]
 
 
-def gather_fleet_table_torch(rows, cap, rank, world=None, group=None):
+def gather_fleet_table_torch(rows, cap, rank, world=None, group=None, heading=None, row_kind=None):
     """tebgpu_fleet_gather over a torch process group (gloo on CPU): rows is the rank's [world * cap] fleet table
-    (abi.FLEET_ROW_DTYPE numpy array) with its shard at rows [rank cap, (rank + 1) cap); returns the gathered table."""
+    (abi.FLEET_ROW_DTYPE numpy array) with its shard at rows [rank cap, (rank + 1) cap); returns the gathered table.
+    heading / row_kind (the shaped steps' companions, [world * cap] float64 / int32): gathered too, as
+    tebgpu_fleet_gather_shaped does, and the return is (rows, heading, row_kind)."""
     import torch
     import torch.distributed as dist
     from . import abi
     world = dist.get_world_size(group) if world is None else world
-    rows = np.ascontiguousarray(rows, dtype=abi.FLEET_ROW_DTYPE).reshape(-1)
-    if len(rows) != world * cap:
-        raise ValueError("the fleet table must have world * cap rows")
-    mine = torch.from_numpy(rows[rank * cap:(rank + 1) * cap].copy().view(np.uint8))
-    out = torch.empty(world * mine.numel(), dtype=torch.uint8)
-    dist.all_gather_into_tensor(out, mine, group=group)
-    return out.numpy().view(abi.FLEET_ROW_DTYPE).copy()
+
+    def gather(a, dtype):
+        a = np.ascontiguousarray(a, dtype=dtype).reshape(-1)
+        if len(a) != world * cap:
+            raise ValueError("the fleet table must have world * cap rows")
+        mine = torch.from_numpy(a[rank * cap:(rank + 1) * cap].copy().view(np.uint8))
+        out = torch.empty(world * mine.numel(), dtype=torch.uint8)
+        dist.all_gather_into_tensor(out, mine, group=group)
+        return out.numpy().view(dtype).copy()
+
+    table = gather(rows, abi.FLEET_ROW_DTYPE)
+    if heading is None and row_kind is None:
+        return table
+    return table, gather(heading, np.float64), gather(row_kind, np.int32)
