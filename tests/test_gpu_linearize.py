@@ -30,6 +30,7 @@ import teb_local_planner_b200 as T
 from teb_local_planner_b200 import abi
 from tests import oracle_binding as O
 from tests import scenarios
+from tests.param_cases import weight_multiplier
 from tests.test_gpu_parity import _report as _write_report
 from tests.test_oracle_graph import _line, _obst, _params
 
@@ -96,7 +97,7 @@ def _oracle(p, hb, b, outer):
            kw["rotdir"], None if kw["obst_vertices"] is None else kw["obst_vertices"].tobytes(), outer,
            max(1, (hb.M_cap + 63) // 64))
     if key not in _oracle_cache:
-        mult = 2.0 ** outer
+        mult = weight_multiplier(p, outer)
         Hd, bd, _ = O.build_system(p, hb.poses[b], n, weight_multiplier=mult, jac_mode=O.JAC_ANALYTIC, **kw)
         fam = O.trial_chi2(p, hb.poses[b], n, hb.poses[b][None, :n], weight_multiplier=mult, **kw)[0]
         gr = O.graph(p, hb.poses[b], n, weight_multiplier=mult, MW=max(1, (hb.M_cap + 63) // 64), **kw)

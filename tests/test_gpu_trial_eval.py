@@ -39,6 +39,7 @@ from teb_local_planner_b200 import abi, scenes
 from tests import banded_reference as R
 from tests import oracle_binding as O
 from tests import scenarios
+from tests.param_cases import weight_multiplier
 from tests.test_gpu_parity import _report as _write_report
 
 pytestmark = pytest.mark.gpu
@@ -162,7 +163,7 @@ def _fam_errors(got, ref):
 def _oracle_b(p, hb, b, outer):
     """the oracle's b of band b at its graph state, in the device's row order (row = oracle row + 3)"""
     n = int(hb.n[b])
-    _, bd, _ = O.build_system(p, hb.poses[b], n, weight_multiplier=2.0 ** outer, jac_mode=O.JAC_ANALYTIC,
+    _, bd, _ = O.build_system(p, hb.poses[b], n, weight_multiplier=weight_multiplier(p, outer), jac_mode=O.JAC_ANALYTIC,
                               **scenarios.band_kwargs(hb, b))
     full = np.zeros(4 * hb.n_cap)
     full[3:3 + bd.size] = bd
@@ -175,7 +176,7 @@ def check_chi2(rd, build, bands=None):
     for b in (rd.bands() if bands is None else bands):
         n, kact = int(hb.n[b]), rd.kact(b)
         trials = np.stack([rd.trial_state(b, k)[:n] for k in range(kact)])
-        ref = O.trial_chi2(p, hb.poses[b], n, trials, weight_multiplier=2.0 ** rd.outer, **scenarios.band_kwargs(hb, b))
+        ref = O.trial_chi2(p, hb.poses[b], n, trials, weight_multiplier=weight_multiplier(p, rd.outer), **scenarios.band_kwargs(hb, b))
         got = rd.out["res"][b, :kact]
         err = _fam_errors(got[:, :4], ref)
         for f, nm in enumerate(("obst", "via", "time", "other")):

@@ -180,7 +180,9 @@ def test_compute_cost_outside_optimize_is_undefined_in_the_reference(oracle):
 
 def _cost_from_oracle(oracle, p, hb, b, args):
     """scaled chi2 by family at the current state: chi2 is linear in the information weights and a zero weight removes
-    the family's edges (optimal_planner.cpp:337, :342, :677), so differences of three oracle builds isolate the families"""
+    the family's edges (optimal_planner.cpp:337, :342, :677), so differences of oracle builds isolate the families. A
+    zero obstacle weight also removes the velocity-obstacle ratio edges (obstacles_per_vertex_ stays empty), which
+    computeCurrentCost does not scale: the obstacle part is taken with the ratio edges switched off on both sides"""
     kw = scenarios.band_kwargs(hb, b)
     n = int(hb.n[b])
 
@@ -188,8 +190,10 @@ def _cost_from_oracle(oracle, p, hb, b, args):
         return oracle.build_system(q, hb.poses[b], n, jac_mode=oracle.JAC_G2O, **kw)[2]
     base = chi(p)
     q = type(p).from_buffer_copy(p)
+    q.weight_velocity_obstacle_ratio = 0
+    no_ratio = chi(q)
     q.weight_obstacle, q.weight_inflation, q.weight_dynamic_obstacle, q.weight_dynamic_obstacle_inflation = 0, 0, 0, 0
-    obst = base - chi(q)
+    obst = no_ratio - chi(q)
     q = type(p).from_buffer_copy(p)
     q.weight_viapoint = 0
     via = base - chi(q)
