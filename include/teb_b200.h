@@ -965,8 +965,34 @@ int32_t tebgpu_fleet_obstacles_table_device(tebgpu_ctx* ctx, const TebFleetArgs*
  * A kind has at most TEB_FLEET_MAX_KIND_VERTICES points in all (TebCostmapWorld's footprint limit). Every point and
  * radius is finite.
  *
- * The neighbours of every robot, their order and the list of min(max_rows, C_cap - own) kept are exactly those of the
- * circle steps on the same inputs (same world, d2 <= range^2 on the centres, (d2, q) order, either search). Then, with
+ * Neighbours (defined here), by select:
+ *   TEB_FLEET_SELECT_CENTRES (0, a zero-initialised struct): the neighbours of every robot, their order and the list of
+ *     min(max_rows, C_cap - own) kept are exactly those of the circle steps on the same inputs (same world, d2 <=
+ *     range^2 on the centres, (d2, q) order, either search).
+ *   TEB_FLEET_SELECT_FOOTPRINTS (1): by the clearance robot r's planner will measure. For robot r and a candidate q of
+ *     the circle steps' candidates (same world, live, q != r):
+ *     a. r's footprint is the footprint model of the context's TebParams (tebgpu_set_params; a new context's default
+ *        is the Point model) at r's pose: pose[r] in the array step, its row's (x, y) and heading[first + r] in the table step;
+ *     b. q's parts are placed exactly as the rows below place them (same sin / cos, a Polygon's closure check);
+ *     c. gap(r, q) = the least, over q's parts, of the optimizer's static distance from r's footprint to the part
+ *        (robot_obstacle_distance_only at t = 0, teb_oracle_distance); velocities are not used. As in that code, a
+ *        NaN pair value (a NaN heading on the device forms) is skipped, so a part all of whose pair values are NaN
+ *        has the distance 1.797e308 less the radii: a neighbour only at range inf. -inf for a kind outside 0 .. K - 1
+ *        on the device forms (such a neighbour is kept first and ends the list as below);
+ *     d. prefilter: q is tested only if d2 <= R'^2 on the centres (rounded as the circle steps), with R' = (range + E_r
+ *        + E_lib)(1 + 2^-16), each operation rounded on its own: E_r the circumscribed radius of the footprint model,
+ *        E_lib the largest |u| + radius of a part point u of the library; the grid's cell side comes from R' as it
+ *        comes from range in the circle steps. DESIGN §4 shows that the prefilter drops no pair with gap <= range while
+ *        both centres lie within the grid's cell bound (|x|, |y| < 2^24 h, h the cell side from R'); past it a pair
+ *        whose gap is within range may fail the prefilter, alike in both searches;
+ *     e. q is a neighbour when it passes the prefilter and gap <= range; needed counts them; they
+ *        are ordered by (gap, q), a total order, and cut at min(max_rows, C_cap - own).
+ *     The gap rests on the device's sin / cos and on the distance code's rounding, so a host restatement may part ways
+ *     with the device on a pair whose gap lies within rounding of range, or on two gaps within rounding of a tie; every
+ *     other decision is the same, and both searches write the same bytes (one out-of-line routine computes the gap).
+ *     A fleet published as circles gets this rule through a kind of one Circular part; the circle steps keep the
+ *     centres' rule.
+ * Then, with
  * own = own_count[s] and vown = own_vertex_count[s] (0 for NULL): the longest prefix q_1 .. q_n of the kept list whose
  * parts fit in C_cap - own rows and whose Line / Polygon points fit in PV_cap - vown vertices is written (a neighbour
  * that does not fit ends the list: a smaller one behind it is not taken). Neighbour q_i's parts go, in library order, to
@@ -992,11 +1018,14 @@ int32_t tebgpu_fleet_obstacles_table_device(tebgpu_ctx* ctx, const TebFleetArgs*
  * Argument errors return TEBGPU_ERR_INVALID_ARG before anything is launched: those of the matching circle step (radius is
  * not read, except by the publish step, which writes the rows tebgpu_fleet_publish writes), NULL shapes, K outside
  * 1 .. TEB_FLEET_MAX_KINDS, a malformed library (the rules above), PV_cap < 0, a Line or Polygon part of more points than
- * PV_cap (the steps that write rows), a NULL per-robot array the step reads; the host forms also refuse a kind or own_vertex_count out of range and
- * a non-finite heading. */
+ * PV_cap (the steps that write rows), a NULL per-robot array the step reads, and in the obstacle steps a select that is
+ * not a TEB_FLEET_SELECT_* or TEB_FLEET_SELECT_FOOTPRINTS on a context without params or with a non-finite footprint;
+ * the host forms also refuse a kind or own_vertex_count out of range and a non-finite heading. */
 #define TEB_FLEET_MAX_KINDS 256
 #define TEB_FLEET_MAX_PARTS 8
 #define TEB_FLEET_MAX_KIND_VERTICES 64
+#define TEB_FLEET_SELECT_CENTRES    0  /* neighbours by d2 <= range^2 on the centres, ordered by (d2, q): the circle steps' */
+#define TEB_FLEET_SELECT_FOOTPRINTS 1  /* neighbours by the gap from the robot's footprint to their parts, by (gap, q) */
 typedef struct TebFleetShapes {
   int32_t  K;                  /* kinds, 1 .. TEB_FLEET_MAX_KINDS */
   int32_t  PV_cap;             /* vertices per scene (stride of custom_vertices, TebFrameArgs.PV_cap), >= 0 */
@@ -1010,6 +1039,7 @@ typedef struct TebFleetShapes {
   double*        custom_vertices;  /* [S][PV_cap][2] in/out: TebFrameArgs.custom_vertices */
   double*        heading;      /* [T] the table's headings (publish writes, table step reads) */
   int32_t*       row_kind;     /* [T] the table's kinds (publish writes, table step reads) */
+  int32_t        select;       /* TEB_FLEET_SELECT_*: how the obstacle steps choose neighbours (0: by centres) */
 } TebFleetShapes;
 
 /* tebgpu_fleet_obstacles_shaped(_device): TebFleetArgs' step, each neighbour written as its kind's parts; radius is not

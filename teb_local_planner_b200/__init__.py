@@ -665,11 +665,13 @@ class TebGpu:
                     "tebgpu_fleet_obstacles_table_device")
 
     def fleet_obstacles_shaped(self, kinds, kind, pose, last_cmd, custom, range, max_rows=8, own_count=None,
-                               custom_count=None, world=None, scene=None, custom_vertices=None, own_vertex_count=None):
+                               custom_count=None, world=None, scene=None, custom_vertices=None, own_vertex_count=None,
+                               select=abi.TEB_FLEET_SELECT_CENTRES):
         """fleet_obstacles with every neighbour written as its kind's footprint (tebgpu_fleet_obstacles_shaped), host
         buffers: kinds the shape library (abi.make_fleet_shapes' list), kind [R] each robot's kind, custom_vertices
-        [S][PV_cap][2] the scenes' vertex pools (None: PV_cap 0), own_vertex_count [S] (None: 0); the rest as
-        fleet_obstacles. Returns (custom, custom_count, needed, status, custom_vertices), new arrays."""
+        [S][PV_cap][2] the scenes' vertex pools (None: PV_cap 0), own_vertex_count [S] (None: 0), select the neighbour
+        rule (abi.TEB_FLEET_SELECT_*; footprints need set_params); the rest as fleet_obstacles. Returns (custom,
+        custom_count, needed, status, custom_vertices), new arrays."""
         import numpy as np
         pose = np.ascontiguousarray(pose, dtype=np.float64).reshape(-1, 3)
         R = pose.shape[0]
@@ -686,7 +688,7 @@ class TebGpu:
         fa = abi.make_fleet_args(R, S, out.shape[1], max_rows, range, pose=pose, last_cmd=keep["cmd"], world=keep["world"],
                                  scene=keep["scene"], own_count=own, custom=out if out.size else None, custom_count=cc,
                                  needed=needed, status=status)
-        sh = abi.make_fleet_shapes(kinds, cv.shape[1], kind=keep["kind"], own_vertex_count=keep["ownv"],
+        sh = abi.make_fleet_shapes(kinds, cv.shape[1], select, kind=keep["kind"], own_vertex_count=keep["ownv"],
                                    custom_vertices=cv if cv.size else None)
         self._check(self.lib.tebgpu_fleet_obstacles_shaped(self.ctx, C.byref(fa), C.byref(sh)),
                     "tebgpu_fleet_obstacles_shaped")
@@ -747,7 +749,7 @@ class TebGpu:
 
     def fleet_obstacles_table_shaped(self, kinds, rows, heading, row_kind, first, R, custom, range, max_rows=8,
                                      own_count=None, custom_count=None, scene=None, custom_vertices=None,
-                                     own_vertex_count=None):
+                                     own_vertex_count=None, select=abi.TEB_FLEET_SELECT_CENTRES):
         """fleet_obstacles_table with every neighbour written as its kind's footprint
         (tebgpu_fleet_obstacles_table_shaped), host buffers: heading [T], row_kind [T] the table's companions, the rest
         as fleet_obstacles_shaped / fleet_obstacles_table. Returns (custom, custom_count, needed, status,
@@ -767,7 +769,7 @@ class TebGpu:
         needed, status = np.full(int(R), -2, np.int32), np.full(int(R), -1, np.int32)
         fa = abi.make_fleet_args(R, S, out.shape[1], max_rows, range, scene=sc, own_count=own,
                                  custom=out if out.size else None, custom_count=cc, needed=needed, status=status)
-        sh = abi.make_fleet_shapes(kinds, cv.shape[1], own_vertex_count=ownv, custom_vertices=cv if cv.size else None,
+        sh = abi.make_fleet_shapes(kinds, cv.shape[1], select, own_vertex_count=ownv, custom_vertices=cv if cv.size else None,
                                    heading=hd if hd.size else None, row_kind=rk if rk.size else None)
         tb = abi.make_fleet_table(len(rows), first, rows if rows.size else None)
         self._check(self.lib.tebgpu_fleet_obstacles_table_shaped(self.ctx, C.byref(fa), C.byref(sh), C.byref(tb)),

@@ -401,14 +401,16 @@ def make_fleet_table(T, first, rows) -> TebFleetTable:
 class TebFleetShapes(C.Structure):
     """The shape library of the _shaped fleet steps (include/teb_b200.h): K kinds of parts (Point, Circular, Line,
     Polygon) in the robot's body frame as HOST arrays, and the per-robot arrays (kind [R], own_vertex_count [S],
-    custom_vertices [S][PV_cap][2], the table's heading [T] / row_kind [T]) as host or device pointers"""
+    custom_vertices [S][PV_cap][2], the table's heading [T] / row_kind [T]) as host or device pointers, and the
+    obstacle steps' selection rule (TEB_FLEET_SELECT_CENTRES or _FOOTPRINTS)"""
     _fields_ = [("K", _i), ("PV_cap", _i), ("kind_parts", C.c_void_p), ("part_type", C.c_void_p),
                 ("part_vertices", C.c_void_p), ("part_radius", C.c_void_p), ("vertices", C.c_void_p),
                 ("kind", C.c_void_p), ("own_vertex_count", C.c_void_p), ("custom_vertices", C.c_void_p),
-                ("heading", C.c_void_p), ("row_kind", C.c_void_p)]
+                ("heading", C.c_void_p), ("row_kind", C.c_void_p), ("select", _i)]
 
 
 TEB_FLEET_MAX_KINDS, TEB_FLEET_MAX_PARTS, TEB_FLEET_MAX_KIND_VERTICES = 256, 8, 64
+TEB_FLEET_SELECT_CENTRES, TEB_FLEET_SELECT_FOOTPRINTS = 0, 1
 
 
 def _addr(v):
@@ -419,12 +421,14 @@ def _addr(v):
     return v
 
 
-def make_fleet_shapes(kinds, PV_cap=0, **arrays) -> TebFleetShapes:
+def make_fleet_shapes(kinds, PV_cap=0, select=TEB_FLEET_SELECT_CENTRES, **arrays) -> TebFleetShapes:
     """TebFleetShapes of the library `kinds`: a list of kinds, each a list of parts (type, points, radius=0.0), type a
     TEB_OBST_POINT / _CIRCULAR / _LINE / _POLYGON, points [n][2] in the body frame (x forward, y left). The per-robot
     arrays are given by keyword (kind=..., own_vertex_count=..., custom_vertices=..., heading=..., row_kind=...) as
-    addresses (ints), torch tensors (their data_ptr()), numpy arrays (their buffer; keep them alive) or None for NULL. The
-    returned struct keeps the library's arrays alive."""
+    addresses (ints), torch tensors (their data_ptr()), numpy arrays (their buffer; keep them alive) or None for NULL.
+    select: how the obstacle steps choose neighbours, by their centres (TEB_FLEET_SELECT_CENTRES) or by the gap from the
+    context's footprint to their parts (TEB_FLEET_SELECT_FOOTPRINTS). The returned struct keeps the library's arrays
+    alive."""
     kind_parts, part_type, part_vertices, part_radius, verts = [0], [], [0], [], []
     for parts in kinds:
         for part in parts:
@@ -438,7 +442,7 @@ def make_fleet_shapes(kinds, PV_cap=0, **arrays) -> TebFleetShapes:
                part_vertices=np.asarray(part_vertices, np.int32), part_radius=np.asarray(part_radius, np.float64),
                vertices=np.ascontiguousarray(np.concatenate(verts) if verts else np.zeros((0, 2))))
     sh = TebFleetShapes()
-    sh.K, sh.PV_cap = len(kinds), int(PV_cap)
+    sh.K, sh.PV_cap, sh.select = len(kinds), int(PV_cap), int(select)
     for k, v in lib.items():
         setattr(sh, k, ptr(v) if v.size else None)
     names = {f[0] for f in TebFleetShapes._fields_[7:]}

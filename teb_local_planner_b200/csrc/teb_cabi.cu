@@ -2206,15 +2206,18 @@ static int32_t issue_fleet_grid(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStr
  * already checked; table: the candidates of tebgpu_fleet_obstacles_table, NULL for the caller's arrays; writer: what the
  * kept lists become (FleetCircles or FleetShaped) */
 extern "C++" {
-template <class W = FleetCircles>
+template <class W = FleetCircles, class S = FleetCentres>
 static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t st, const TebFleetTable* table = nullptr,
-                           const W& writer = W{}) {
+                           const W& writer = W{}, const S& sel = S{}) {
   int32_t rc;
   const int64_t N = table ? table->T : fa->R;
-  const int search = fleet_search(ctx, fa, N);
+  /* the search and the grid's cells are those of the centres' test: range, or the footprints' prefilter R' */
+  TebFleetArgs ga = *fa;
+  if constexpr (S::EXACT) ga.range = sel.pre;
+  const int search = fleet_search(ctx, &ga, N);
   FleetGrid g{};
   if (search != TEBGPU_FLEET_SEARCH_ALL_PAIRS &&
-      (rc = issue_fleet_grid(ctx, fa, st, table, N, search == TEBGPU_FLEET_SEARCH_ONE_BUCKET, &g))) return rc;
+      (rc = issue_fleet_grid(ctx, &ga, st, table, N, search == TEBGPU_FLEET_SEARCH_ONE_BUCKET, &g))) return rc;
   const int32_t* claims = nullptr;
   if (fa->scene) {
     if ((rc = grow_mirror(ctx, (void**)&ctx->d_fclaim, &ctx->fclaim_bytes, (size_t)fa->S * sizeof(int32_t), st))) return rc;
@@ -2224,11 +2227,11 @@ static int32_t issue_fleet(tebgpu_ctx* ctx, const TebFleetArgs* fa, cudaStream_t
   }
   const long long grid = ((long long)fa->R + FLEET_WARPS - 1) / FLEET_WARPS;
   if (search == TEBGPU_FLEET_SEARCH_ALL_PAIRS) {
-    if (table) k_fleet_obstacles<true, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, writer);
-    else k_fleet_obstacles<false, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, writer);
+    if (table) k_fleet_obstacles<true, W, S><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, writer, sel);
+    else k_fleet_obstacles<false, W, S><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, writer, sel);
   } else {
-    if (table) k_fleet_obstacles_grid<true, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, g, writer);
-    else k_fleet_obstacles_grid<false, W><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, g, writer);
+    if (table) k_fleet_obstacles_grid<true, W, S><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, *table, g, writer, sel);
+    else k_fleet_obstacles_grid<false, W, S><<<(unsigned)grid, FLEET_THREADS, 0, st>>>(*fa, claims, TebFleetTable{}, g, writer, sel);
   }
   ctx->last_fleet_grid = grid;
   ctx->last_fleet_search = search;
@@ -2247,7 +2250,8 @@ int32_t tebgpu_fleet_obstacles_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, v
 }
 
 static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table,
-                              const TebFleetShapes* sh = nullptr, const FleetLib* lib = nullptr);
+                              const TebFleetShapes* sh = nullptr, const FleetLib* lib = nullptr,
+                              const FleetFootprints* sel = nullptr);
 
 /* the host form's checks of its arrays, on arguments that passed check_fleet_args */
 static int32_t check_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
@@ -2280,9 +2284,10 @@ int32_t tebgpu_fleet_obstacles(tebgpu_ctx* ctx, const TebFleetArgs* fa) {
 
 /* the host-buffer fleet steps on arguments already checked: stage the arrays given (NULL ones stay NULL), launch on the
  * context's stream, copy the outputs back and synchronise. table: the device copy of the candidates' table, or NULL.
- * sh, lib: the shaped steps' host arrays and their library already on the device, or NULL for the circle steps */
+ * sh, lib: the shaped steps' host arrays and their library already on the device, or NULL for the circle steps; sel:
+ * the footprints' rule (TEB_FLEET_SELECT_FOOTPRINTS), or NULL for the centres' */
 static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* table,
-                              const TebFleetShapes* sh, const FleetLib* lib) {
+                              const TebFleetShapes* sh, const FleetLib* lib, const FleetFootprints* sel) {
   int32_t rc;
   const size_t R = fa->R, S = fa->S, C = fa->C_cap;
   const size_t T = table ? table->T : 0, PV = sh ? sh->PV_cap : 0;
@@ -2320,7 +2325,7 @@ static int32_t run_fleet_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const Teb
     FleetShaped w{*lib};
     w.L.kind = (const int32_t*)sl[KIND].dev(d); w.L.own_v = (const int32_t*)sl[OWNV].dev(d);
     w.L.cv = (double*)sl[CVERT].dev(d); w.L.heading = (double*)sl[HEAD].dev(d); w.L.row_kind = (int32_t*)sl[RKIND].dev(d);
-    rc = issue_fleet(ctx, &da, st, table, w);
+    rc = sel ? issue_fleet(ctx, &da, st, table, w, *sel) : issue_fleet(ctx, &da, st, table, w);
   } else {
     rc = issue_fleet(ctx, &da, st, table);
   }
@@ -2438,7 +2443,8 @@ static int32_t check_fleet_table_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, c
 
 /* the host table forms on checked arguments: the table up, then run_fleet_host */
 static int32_t run_fleet_table_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t,
-                                    const TebFleetShapes* sh = nullptr, const FleetLib* lib = nullptr) {
+                                    const TebFleetShapes* sh = nullptr, const FleetLib* lib = nullptr,
+                                    const FleetFootprints* sel = nullptr) {
   int32_t rc;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
@@ -2449,7 +2455,7 @@ static int32_t run_fleet_table_host(tebgpu_ctx* ctx, const TebFleetArgs* fa, con
   TebFleetArgs ha = *fa;
   ha.pose = ha.last_cmd = ha.radius = nullptr;
   ha.world = nullptr;
-  return run_fleet_host(ctx, &ha, &dt, sh, lib);
+  return run_fleet_host(ctx, &ha, &dt, sh, lib, sel);
 }
 
 int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetTable* t) {
@@ -2461,12 +2467,13 @@ int32_t tebgpu_fleet_obstacles_table(tebgpu_ctx* ctx, const TebFleetArgs* fa, co
 /* the shaped fleet steps' library (TebFleetShapes): checked, laid out as the device reads it (FleetLib: the parts, the
  * kinds' part and written-point ranges, the written points) and sent to the context's copy when it differs from the
  * last library sent. Nothing is launched before it; lib gets the device pointers, K and PV_cap. kind / companions: the
- * step reads those arrays; rows: it writes rows and vertices (not the publish step), so PV_cap must hold every part */
+ * step reads those arrays; rows: it writes rows and vertices (not the publish step), so PV_cap must hold every part;
+ * reach (or NULL): E_lib, the largest |u| + radius of a part point u of the library (DESIGN §4) */
 static int32_t check_fleet_shape_arrays(tebgpu_ctx* ctx, const TebFleetShapes* sh, bool kind, bool companions,
                                         bool vertices);
 
 static int32_t stage_fleet_shapes(tebgpu_ctx* ctx, const TebFleetShapes* sh, cudaStream_t st, FleetLib* lib, bool kind,
-                                  bool companions, bool rows = true) {
+                                  bool companions, bool rows = true, double* reach = nullptr) {
   if (!sh) { ctx->err = "fleet shapes == NULL"; return TEBGPU_ERR_INVALID_ARG; }
   if (sh->K < 1 || sh->K > TEB_FLEET_MAX_KINDS) { ctx->err = "shapes K outside 1 .. TEB_FLEET_MAX_KINDS"; return TEBGPU_ERR_INVALID_ARG; }
   if (sh->PV_cap < 0) { ctx->err = "shapes PV_cap < 0"; return TEBGPU_ERR_INVALID_ARG; }
@@ -2483,6 +2490,7 @@ static int32_t stage_fleet_shapes(tebgpu_ctx* ctx, const TebFleetShapes* sh, cud
   std::vector<FleetPart> parts(P);
   std::vector<int32_t> kpart(K + 1), kvert(K + 1, 0);
   std::vector<double> wv;
+  double e_lib = 0.0;
   for (int k = 0; k < K; ++k) {
     kpart[k] = sh->kind_parts[k];
     int points = 0;
@@ -2497,6 +2505,8 @@ static int32_t stage_fleet_shapes(tebgpu_ctx* ctx, const TebFleetShapes* sh, cud
       const double* u = sh->vertices + 2 * (size_t)v0;
       for (int i = 0; i < 2 * n; ++i)
         if (!std::isfinite(u[i])) { ctx->err = "a shape point is not finite"; return TEBGPU_ERR_INVALID_ARG; }
+      const double rad = type == TEB_OBST_CIRCULAR && sh->part_radius ? sh->part_radius[p] : 0.0;
+      for (int i = 0; i < n; ++i) e_lib = std::max(e_lib, std::sqrt(u[2 * i] * u[2 * i] + u[2 * i + 1] * u[2 * i + 1]) + rad);
       FleetPart& f = parts[p];
       f = FleetPart{0.0, 0.0, 0.0, type, 0, 0, 0};
       if (one) {
@@ -2551,7 +2561,51 @@ static int32_t stage_fleet_shapes(tebgpu_ctx* ctx, const TebFleetShapes* sh, cud
   lib->cv = sh->custom_vertices;
   lib->heading = sh->heading;
   lib->row_kind = sh->row_kind;
+  if (reach) *reach = e_lib;
   return TEBGPU_OK;
+}
+
+/* E_r: the circumscribed radius of a footprint model, the largest distance from the robot's position of a point of
+ * its footprint (DESIGN §4) */
+static double footprint_reach(const TebParams& p) {
+  auto norm = [](double x, double y) { return std::sqrt(x * x + y * y); };
+  switch (p.footprint_type) {
+    case TEB_FOOTPRINT_CIRCULAR: return std::fabs(p.footprint_radius);
+    case TEB_FOOTPRINT_TWO_CIRCLES:
+      return std::max(std::fabs(p.footprint_front_offset) + std::fabs(p.footprint_front_radius),
+                      std::fabs(p.footprint_rear_offset) + std::fabs(p.footprint_rear_radius));
+    case TEB_FOOTPRINT_LINE:
+      return std::max(norm(p.footprint_line[0], p.footprint_line[1]), norm(p.footprint_line[2], p.footprint_line[3]));
+    case TEB_FOOTPRINT_POLYGON: {
+      double e = 0.0;
+      for (int i = 0; i < p.footprint_vertex_count; ++i)
+        e = std::max(e, norm(p.footprint_vertices[2 * i], p.footprint_vertices[2 * i + 1]));
+      return e;
+    }
+    default: return 0.0;
+  }
+}
+
+/* the selection rule of a shaped obstacle step, checked before anything is staged: *exact false for
+ * TEB_FLEET_SELECT_CENTRES; for TEB_FLEET_SELECT_FOOTPRINTS the context's footprint, which must be finite */
+static int32_t check_fleet_select(tebgpu_ctx* ctx, const TebFleetShapes* sh, bool* exact) {
+  *exact = false;
+  if (!sh) { ctx->err = "fleet shapes == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (sh->select == TEB_FLEET_SELECT_CENTRES) return TEBGPU_OK;
+  if (sh->select != TEB_FLEET_SELECT_FOOTPRINTS) { ctx->err = "shapes select is not a TEB_FLEET_SELECT_*"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!std::isfinite(footprint_reach(ctx->params))) { ctx->err = "the context's footprint is not finite"; return TEBGPU_ERR_INVALID_ARG; }
+  *exact = true;
+  return TEBGPU_OK;
+}
+
+/* the footprints' rule of a step of range fa->range over a library of reach e_lib: R' = (range + E_r + E_lib)(1 +
+ * 2^-16), each operation rounded on its own (inf for range inf) */
+static FleetFootprints fleet_footprints(const tebgpu_ctx* ctx, const TebFleetArgs* fa, double e_lib) {
+  FleetFootprints f;
+  f.pre = (fa->range + footprint_reach(ctx->params) + e_lib) * FLEET_H_MARGIN;
+  f.fp = ctx->d_fp;
+  f.fp_type = ctx->params.footprint_type;
+  return f;
 }
 
 /* the shapes' per-robot arrays a shaped step reads: kind (array and publish steps), the companions (table, publish and
@@ -2586,8 +2640,12 @@ int32_t tebgpu_fleet_obstacles_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs
   if (rc) return rc;
   if (!fa->pose || !fa->last_cmd) { ctx->err = "missing required fleet array"; return TEBGPU_ERR_INVALID_ARG; }
   cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  bool exact;
+  if ((rc = check_fleet_select(ctx, sh, &exact))) return rc;
   FleetLib lib;
-  if ((rc = stage_fleet_shapes(ctx, sh, st, &lib, true, false))) return rc;
+  double e_lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, st, &lib, true, false, true, &e_lib))) return rc;
+  if (exact) return issue_fleet(ctx, fa, st, nullptr, FleetShaped{lib}, fleet_footprints(ctx, fa, e_lib));
   return issue_fleet(ctx, fa, st, nullptr, FleetShaped{lib});
 }
 
@@ -2600,11 +2658,15 @@ int32_t tebgpu_fleet_obstacles_shaped(tebgpu_ctx* ctx, const TebFleetArgs* fa, c
   ca.radius = zero.data();
   int32_t rc = check_fleet_args(ctx, &ca);
   if (rc || (rc = check_fleet_host(ctx, &ca))) return rc;     /* scenes and own counts first: the checks below read them */
+  bool exact;
+  if ((rc = check_fleet_select(ctx, sh, &exact))) return rc;
   FleetLib lib;
-  if ((rc = stage_fleet_shapes(ctx, sh, ctx->stream, &lib, true, false))) return rc;
+  double e_lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, ctx->stream, &lib, true, false, true, &e_lib))) return rc;
   if ((rc = check_fleet_shape_values(ctx, fa, sh, sh->kind, R))) return rc;
   ca.radius = nullptr;
-  return run_fleet_host(ctx, &ca, nullptr, sh, &lib);
+  const FleetFootprints f = fleet_footprints(ctx, fa, e_lib);
+  return run_fleet_host(ctx, &ca, nullptr, sh, &lib, exact ? &f : nullptr);
 }
 
 int32_t tebgpu_fleet_publish_shaped_device(tebgpu_ctx* ctx, const TebFleetArgs* fa, const TebFleetShapes* sh,
@@ -2642,8 +2704,12 @@ int32_t tebgpu_fleet_obstacles_table_shaped_device(tebgpu_ctx* ctx, const TebFle
   int32_t rc = check_fleet_args(ctx, fa, false);
   if (rc || (rc = check_fleet_table(ctx, fa, t))) return rc;
   cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  bool exact;
+  if ((rc = check_fleet_select(ctx, sh, &exact))) return rc;
   FleetLib lib;
-  if ((rc = stage_fleet_shapes(ctx, sh, st, &lib, false, true))) return rc;
+  double e_lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, st, &lib, false, true, true, &e_lib))) return rc;
+  if (exact) return issue_fleet(ctx, fa, st, t, FleetShaped{lib}, fleet_footprints(ctx, fa, e_lib));
   return issue_fleet(ctx, fa, st, t, FleetShaped{lib});
 }
 
@@ -2651,8 +2717,11 @@ int32_t tebgpu_fleet_obstacles_table_shaped(tebgpu_ctx* ctx, const TebFleetArgs*
                                             const TebFleetTable* t) {
   int32_t rc = check_fleet_args(ctx, fa, false);
   if (rc || (rc = check_fleet_table(ctx, fa, t)) || (rc = check_fleet_table_host(ctx, fa, t))) return rc;
+  bool exact;
+  if ((rc = check_fleet_select(ctx, sh, &exact))) return rc;
   FleetLib lib;
-  if ((rc = stage_fleet_shapes(ctx, sh, ctx->stream, &lib, false, true))) return rc;
+  double e_lib;
+  if ((rc = stage_fleet_shapes(ctx, sh, ctx->stream, &lib, false, true, true, &e_lib))) return rc;
   std::vector<int32_t> live_kinds;
   for (int q = 0; q < t->T; ++q) {
     if (!t->rows[q].live) continue;
@@ -2660,7 +2729,8 @@ int32_t tebgpu_fleet_obstacles_table_shaped(tebgpu_ctx* ctx, const TebFleetArgs*
     live_kinds.push_back(sh->row_kind[q]);
   }
   if ((rc = check_fleet_shape_values(ctx, fa, sh, live_kinds.data(), live_kinds.size()))) return rc;
-  return run_fleet_table_host(ctx, fa, t, sh, &lib);
+  const FleetFootprints f = fleet_footprints(ctx, fa, e_lib);
+  return run_fleet_table_host(ctx, fa, t, sh, &lib, exact ? &f : nullptr);
 }
 
 int32_t tebgpu_compute_cost(tebgpu_ctx* ctx, const TebBatch* bt, const TebOptimizeArgs* args) {

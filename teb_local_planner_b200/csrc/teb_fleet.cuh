@@ -15,7 +15,10 @@
  *
  * Both search kernels take a writer, what the kept list becomes: FleetCircles, one TEB_OBST_CIRCULAR row per neighbour
  * (the circle steps), or FleetShaped, each neighbour as its kind's parts from a TebFleetShapes library (the _shaped
- * steps). The contract is at TebFleetShapes in include/teb_b200.h.
+ * steps). The contract is at TebFleetShapes in include/teb_b200.h. Beside the writer they take a selection rule:
+ * FleetCentres, d2 <= range^2 on the centres (the circle steps and TebFleetShapes.select 0), or FleetFootprints, the
+ * centres' prefilter at R' and then the gap from the context's footprint to the candidate's placed parts (fleet_gap, one
+ * out-of-line routine both searches call), the gap taking d2's place as the list's key (DESIGN §4).
  *
  * The CTA stages FLEET_TILE robots' (x, y, world) at a time (the table build (x, y, world, live)); lane l of a warp tests candidates l, l + 32, ... of the
  * tile against its robot, and the warp keeps the nearest min(max_rows, C_cap - own) neighbours as a list sorted by
@@ -37,6 +40,7 @@
 #include <climits>
 #include <cmath>
 
+#include "teb_device.cuh"
 #include "teb_frame.h"
 
 namespace tebgpu {
@@ -372,6 +376,149 @@ struct FleetShaped {
   }
 };
 
+/* the selection rules of the search kernels (TebFleetShapes.select), beside the writer. FleetCentres: d2 <= range^2 on
+ * the centres, key d2 (the circle steps and select = TEB_FLEET_SELECT_CENTRES). FleetFootprints: the centres' prefilter
+ * d2 <= pre^2, then the exact test gap <= range, key gap, the gap from fleet_gap (only with the FleetShaped writer,
+ * whose library places the candidate's parts). reach(a): the distance of the centres' test. */
+struct FleetCentres {
+  static constexpr bool EXACT = false;
+  __device__ __forceinline__ double reach(const TebFleetArgs& a) const { return a.range; }
+};
+
+struct FleetFootprints {
+  static constexpr bool EXACT = true;
+  /* the grid builds keep 512 threads per CTA, and so ptxas' cap of 128 registers, with 28 bytes of spill stores and 84
+   * of loads: 256 threads spill nothing (140 registers) but run one CTA of 8 warps per SM and took 1.6x the time at
+   * 8192 and 32768 robots (DESIGN §8) */
+  double pre;            /* R' = (range + E_r + E_lib)(1 + 2^-16), on the host (DESIGN §4) */
+  const double* fp;      /* KParams.fp_geom of the context: its footprint definition (FP_*) */
+  int fp_type;           /* TebParams.footprint_type of the context */
+  __device__ __forceinline__ double reach(const TebFleetArgs&) const { return pre; }
+};
+
+/* the distance from the footprint (fp_type, fp) of a robot at (px, py) with cos / sin (c, s) of its heading to one
+ * placed part: the points ov[0 .. ok) (Line, Polygon) or the point (ox, oy) (Point, Circular of radius orad). The pair
+ * loop of generic_distance, value only, over the same inline pair routines (closest_on_segment, seg_seg_dist), so that
+ * it is the optimizer's static distance (robot_obstacle_distance_only at t = 0) without passing the local point buffer
+ * into the optimizer's out-of-line routine, whose loads would then no longer all be global. */
+__device__ __forceinline__ double fleet_part_distance(int fp_type, const double* __restrict__ fp, double px, double py,
+                                                      double c, double s, const double* ov, int ok, double ox,
+                                                      double oy, double orad, int otype) {
+  const bool olist = ov != nullptr;
+  const bool obst_first = otype == TEB_OBST_LINE;
+  const int oe = ok <= 2 ? 1 : ok;
+  double best = 1.7976931348623157e308;
+  const int nsub = fp_type == TEB_FOOTPRINT_TWO_CIRCLES ? 2 : 1;
+  for (int sub = 0; sub < nsub; ++sub) {
+    int rk = 1;
+    double rrad = 0;
+    if (fp_type == TEB_FOOTPRINT_CIRCULAR) rrad = fp[FP_RADIUS];
+    else if (fp_type == TEB_FOOTPRINT_TWO_CIRCLES) rrad = sub == 0 ? fp[FP_FRONT_RAD] : fp[FP_REAR_RAD];
+    else if (fp_type == TEB_FOOTPRINT_LINE) rk = 2;
+    else if (fp_type == TEB_FOOTPRINT_POLYGON) rk = (int)fp[FP_COUNT];
+    const int re = rk <= 2 ? 1 : rk;
+    double sbest = 1.7976931348623157e308;
+    for (int i = 0; i < re; ++i) {
+      double r0x, r0y, r1x, r1y;
+      if (fp_type == TEB_FOOTPRINT_LINE || fp_type == TEB_FOOTPRINT_POLYGON) {
+        const double* lv = fp + (fp_type == TEB_FOOTPRINT_LINE ? FP_LINE : FP_VERTS);
+        const int i1 = (i + 1) % rk;
+        const double ax = lv[2 * i], ay = lv[2 * i + 1], bx = lv[2 * i1], by = lv[2 * i1 + 1];
+        r0x = px + c * ax - s * ay; r0y = py + s * ax + c * ay;
+        r1x = px + c * bx - s * by; r1y = py + s * bx + c * by;
+      } else {
+        double off = 0;
+        if (fp_type == TEB_FOOTPRINT_TWO_CIRCLES) off = sub == 0 ? fp[FP_FRONT_OFF] : -fp[FP_REAR_OFF];
+        r0x = r1x = px + off * c; r0y = r1y = py + off * s;
+      }
+      for (int j = 0; j < oe; ++j) {
+        double o0x, o0y, o1x, o1y;
+        if (olist) {
+          const int j1 = (j + 1) % ok;
+          o0x = ov[2 * j]; o0y = ov[2 * j + 1];
+          o1x = ov[2 * j1]; o1y = ov[2 * j1 + 1];
+        } else { o0x = o1x = ox; o0y = o1y = oy; }
+        const int pk = olist ? ok : 1;
+        double ax, ay, bx, by, d;
+        if (rk == 1 && pk == 1) {
+          d = sqrt((r0x - o0x) * (r0x - o0x) + (r0y - o0y) * (r0y - o0y));
+        } else if (rk == 1) {
+          closest_on_segment(r0x, r0y, o0x, o0y, o1x, o1y, bx, by);
+          d = sqrt((r0x - bx) * (r0x - bx) + (r0y - by) * (r0y - by));
+        } else if (pk == 1) {
+          closest_on_segment(o0x, o0y, r0x, r0y, r1x, r1y, ax, ay);
+          d = sqrt((o0x - ax) * (o0x - ax) + (o0y - ay) * (o0y - ay));
+        } else if (obst_first) {
+          d = seg_seg_dist(o0x, o0y, o1x, o1y, r0x, r0y, r1x, r1y, bx, by, ax, ay);
+        } else {
+          d = seg_seg_dist(r0x, r0y, r1x, r1y, o0x, o0y, o1x, o1y, ax, ay, bx, by);
+        }
+        if (d < sbest) sbest = d;
+      }
+    }
+    const double dsub = sbest - orad - rrad;
+    if (dsub <= best) best = dsub;
+  }
+  return best;
+}
+
+/* the gap from the footprint (fp_type, fp) of a robot at (rx, ry, rth) to the parts
+ * of kind `kind` of a candidate at (qx, qy, qth): the minimum over the parts of fleet_part_distance, each part placed as
+ * FleetShaped::write places and writes it (fleet_place with the same sincos, a Polygon finalised by the same closure
+ * check). NaN pair values are skipped inside fleet_part_distance as generic_distance skips them, so with finite radii
+ * no part's distance is NaN; -inf for a kind outside 0 .. K - 1, so that such a neighbour is kept first and ends its list
+ * as the writer ends it. Out of line: both searches run this one routine, so they write the same
+ * bytes; the robot's sin / cos are taken here, so that the searches keep one double live across their scans, not two. */
+__device__ __noinline__ double fleet_gap(int fp_type, const double* fp, double rx, double ry, double rth,
+                                         const FleetPart* part, const int32_t* kpart, const int32_t* kvert,
+                                         const double* wv, int K, int kind, double qx, double qy, double qth) {
+  if (kind < 0 || kind >= K) return -INFINITY;
+  double rs, rc, sn, cs;
+  sincos(rth, &rs, &rc);
+  sincos(qth, &sn, &cs);
+  double pts[2 * TEB_FLEET_MAX_KIND_VERTICES];
+  const int p1 = __ldg(kpart + kind + 1), w0 = __ldg(kvert + kind);
+  double g = INFINITY;
+  for (int p = __ldg(kpart + kind); p < p1; ++p) {
+    const FleetPart& P = part[p];
+    const int type = __ldg(&P.type);
+    double d;
+    if (type == TEB_OBST_POINT || type == TEB_OBST_CIRCULAR) {
+      double ox, oy;
+      fleet_place(qx, qy, sn, cs, __ldg(&P.cx), __ldg(&P.cy), ox, oy);
+      d = fleet_part_distance(fp_type, fp, rx, ry, rc, rs, nullptr, 1, ox, oy,
+                              type == TEB_OBST_CIRCULAR ? __ldg(&P.radius) : 0.0, type);
+    } else {
+      int n = __ldg(&P.nv);
+      const double2* u = reinterpret_cast<const double2*>(wv) + w0 + __ldg(&P.woff);
+      for (int v = 0; v < n; ++v) {
+        const double2 b = __ldg(u + v);
+        fleet_place(qx, qy, sn, cs, b.x, b.y, pts[2 * v], pts[2 * v + 1]);
+      }
+      if (type == TEB_OBST_POLYGON && teb_eigen_is_approx(pts[0], pts[1], pts[2 * n - 2], pts[2 * n - 1])) --n;
+      d = fleet_part_distance(fp_type, fp, rx, ry, rc, rs, pts, n, 0.0, 0.0, 0.0, type);
+    }
+    if (d < g) g = d;
+  }
+  return g;
+}
+
+/* the gap of candidate q (at (qx, qy)) of the warp's robot under FleetFootprints: its kind and heading from the
+ * caller's arrays or the table's companions */
+template <bool TABLE>
+__device__ __forceinline__ double fleet_gap_of(const TebFleetArgs& a, const FleetLib& L, const FleetFootprints& f,
+                                               double rx, double ry, double rth, size_t q, double qx, double qy) {
+  const int kind = TABLE ? L.row_kind[q] : L.kind[q];
+  const double th = TABLE ? L.heading[q] : a.pose[3 * q + 2];
+  return fleet_gap(f.fp_type, f.fp, rx, ry, rth, L.part, L.kpart, L.kvert, L.wv, L.K, kind, qx, qy, th);
+}
+
+/* the warp's robot's heading (FleetFootprints): pose[r] of the array step, heading[first + r] of the table step */
+template <bool TABLE>
+__device__ __forceinline__ double fleet_robot_heading(const TebFleetArgs& a, const FleetLib& L, int r, int self) {
+  return TABLE ? L.heading[self] : a.pose[3 * (size_t)r + 2];
+}
+
 /* the outputs of the warp's robot r < R through the writer w; a robot that does not write gets needed -1 and its status */
 template <bool TABLE, class W>
 __device__ __forceinline__ void fleet_finish(const TebFleetArgs& a, const TebFleetTable& t, const FleetRobot& m, int r,
@@ -388,9 +535,9 @@ __device__ __forceinline__ void fleet_finish(const TebFleetArgs& a, const TebFle
 
 /* claims: [S] robots per scene from k_fleet_claim, or NULL when TebFleetArgs.scene is NULL (scene r, never shared).
  * TABLE: robot r is row t.first + r of t and the candidates are its T rows; otherwise t is not read. */
-template <bool TABLE, class W = FleetCircles>
+template <bool TABLE, class W = FleetCircles, class S = FleetCentres>
 __global__ void __launch_bounds__(FLEET_THREADS, W::MIN_CTAS) k_fleet_obstacles(const TebFleetArgs a, const int32_t* claims,
-                                                                   const TebFleetTable t, const W writer) {
+                                                                   const TebFleetTable t, const W writer, const S sel) {
   __shared__ double sx[FLEET_TILE], sy[FLEET_TILE];
   __shared__ int sw[FLEET_TILE];
   __shared__ int sl[TABLE ? FLEET_TILE : 1];
@@ -425,11 +572,14 @@ __global__ void __launch_bounds__(FLEET_THREADS, W::MIN_CTAS) k_fleet_obstacles(
     }
     if (valid) K = min(a.max_rows, a.C_cap - own);
   }
-  const double range2 = __dmul_rn(a.range, a.range);
+  const double range2 = __dmul_rn(sel.reach(a), sel.reach(a));
   /* slot `lane` of the list (empty: +inf / INT_MAX, above every real key) and the key of slot K - 1 */
   double kd = INFINITY, td = INFINITY;
   int kq = INT_MAX, tq = INT_MAX;
   int needed = 0;
+  double rth = 0.0;
+  if constexpr (S::EXACT)
+    if (valid) rth = fleet_robot_heading<TABLE>(a, writer.L, r, self);
 
   for (int base = 0; base < N; base += FLEET_TILE) {
     const int nt = min(FLEET_TILE, N - base);
@@ -458,6 +608,12 @@ __global__ void __launch_bounds__(FLEET_THREADS, W::MIN_CTAS) k_fleet_obstacles(
         const double dx = __dsub_rn(sx[j], xr), dy = __dsub_rn(sy[j], yr);
         d2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
         in = d2 <= range2;
+      }
+      if constexpr (S::EXACT) {
+        if (in) {
+          d2 = fleet_gap_of<TABLE>(a, writer.L, sel, xr, yr, rth, (size_t)q, sx[j], sy[j]);
+          in = d2 <= a.range;
+        }
       }
       FLEET_TAKE(in, d2, q, K, lane, kd, kq, td, tq, needed);
     }
@@ -560,20 +716,23 @@ __global__ void __launch_bounds__(CLAIM_THREADS) k_fleet_scatter(const int N, co
 /* k_fleet_obstacles' step with the candidates taken from the grid: the buckets of the robot's 3 x 3 cells (a bucket two
  * cells share is scanned once, so no candidate is met twice) and the far list; a robot in the far list meets every
  * candidate, one never in range none. Every candidate met takes k_fleet_obstacles' exact test and list. */
-template <bool TABLE, class W = FleetCircles>
+template <bool TABLE, class W = FleetCircles, class S = FleetCentres>
 __global__ void __launch_bounds__(FLEET_THREADS, W::MIN_CTAS) k_fleet_obstacles_grid(const TebFleetArgs a, const int32_t* claims,
                                                                         const TebFleetTable t, const FleetGrid g,
-                                                                        const W writer) {
+                                                                        const W writer, const S sel) {
   const int lane = threadIdx.x & 31;
   const int r = blockIdx.x * FLEET_WARPS + (threadIdx.x >> 5);
   if (r >= a.R) return;                    /* warp-uniform */
   const int self = TABLE ? t.first + r : r;
   const int N = TABLE ? t.T : a.R;
   const FleetRobot m = fleet_robot<TABLE>(a, claims, t, r, true);
-  const double range2 = __dmul_rn(a.range, a.range);
+  const double range2 = __dmul_rn(sel.reach(a), sel.reach(a));
   double kd = INFINITY, td = INFINITY;
   int kq = INT_MAX, tq = INT_MAX;
   int needed = 0;
+  double rth = 0.0;
+  if constexpr (S::EXACT)
+    if (m.valid) rth = fleet_robot_heading<TABLE>(a, writer.L, r, self);
   /* lane's candidate q (-1: none) through the exact test into the list */
   auto meet = [&](int q) {
     bool in = false;
@@ -587,6 +746,12 @@ __global__ void __launch_bounds__(FLEET_THREADS, W::MIN_CTAS) k_fleet_obstacles_
         const double dx = __dsub_rn(x, m.x), dy = __dsub_rn(y, m.y);
         d2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
         in = d2 <= range2;
+        if constexpr (S::EXACT) {
+          if (in) {
+            d2 = fleet_gap_of<TABLE>(a, writer.L, sel, m.x, m.y, rth, (size_t)q, x, y);
+            in = d2 <= a.range;
+          }
+        }
       }
     }
     FLEET_TAKE(in, d2, q, m.K, lane, kd, kq, td, tq, needed);
