@@ -538,6 +538,74 @@ typedef struct TebFrameArgs {
   double*       obst_vertices;     /* [S][PV_cap][2] out (the batch's vertex pool): the moved vertices of the rows written */
 } TebFrameArgs;
 
+/* Every robot's local costmap cut out of a shared static map (tebgpu_costmap_window): what costmap_2d computes for a
+ * local costmap with rolling_window: true and a static layer, the raster TebLocalPlannerROS reads every cycle
+ * (teb_local_planner_ros.cpp:478-504 through updateObstacleContainerWithCostmap, and CostmapModel for the feasibility
+ * check). The maps are uploaded once; the windows are written in TebCostmapArgs' layout (cost / grid / origin), so the
+ * window feeds tebgpu_costmap_obstacles(_tf)_device and tebgpu_check_feasible_costmap_device on the same stream unchanged.
+ *
+ * costmap_2d is not part of the reference checkout; this restates ROS Noetic navigation's Costmap2D::mapToWorld /
+ * worldToMap / getSizeInMetersX / updateOrigin, the rolling branch of LayeredCostmap::updateMap and the rolling branch of
+ * StaticLayer::updateCosts with interpretValue. Every product and sum is rounded on its own (no FMA contraction). Robot s,
+ * with (sx, sy) = grid[s], (ox, oy, r) = origin[s] and (rx, ry) = robot[s]:
+ *   1. Origin, carried between cycles: size_m = (sx - 1 + 0.5) * r (getSizeInMetersX, likewise y); new_ox = rx - size_m
+ *      / 2; cell_ox = (new_ox - ox) / r truncated toward zero (C's (int) conversion; computed as trunc() in double, which
+ *      agrees wherever the int conversion is defined); ox' = ox + cell_ox * r. The same for y. origin[s] is read as the
+ *      previous cycle's origin and (ox', oy', r) written back: the caller initialises it once.
+ *   2. Every cell gets the default: NO_INFORMATION (255) with track_unknown_space, otherwise FREE_SPACE (0).
+ *   3. Cell (i, j), 0 <= i < sx, 0 <= j < sy, has the centre wx = ox' + (i + 0.5) * r, wy = oy' + (j + 0.5) * r
+ *      (mapToWorld). costmap_to_map[s] (lookupTransform(map_frame, global_frame)) moves it into the map frame with tf2's
+ *      arithmetic (basis = Matrix3x3::setRotation(q), p = ((b0 wx + b1 wy) + b2 0) + t per row, as TebFrameArgs);
+ *      costmap_to_map == NULL is the identity: no arithmetic, p = (wx, wy). In map m = map_id[s] (mox, moy, mr) =
+ *      TebStaticMaps.origin[m], (msx, msy) = size[m]: off the map when px < mox or py < moy; otherwise mx = (int)((px -
+ *      mox) / mr), my likewise, on the map when mx < msx and my < msy (a quotient >= msx, NaN or past the int range is
+ *      off the map). An on-map cell takes interpretValue(data[offset[m] + my * msx + mx]); an off-map cell keeps the
+ *      default. The map's yaw is ignored, as the static layer ignores it; map and window resolutions may differ.
+ *   4. interpretValue(v), v the OccupancyGrid byte read as unsigned char: v == unknown_cost_value: 255 with
+ *      track_unknown_space, else 0; then v >= lethal_threshold: 254 (LETHAL_OBSTACLE); then trinary_costmap: 0; else
+ *      (unsigned char)((double)v / lethal_threshold * 254).
+ * The window is cost[s][j * sx + i]; the bytes sx * sy .. cell_cap - 1 of the row get the default too, so every byte of
+ * the output is defined.
+ *
+ * Where this and costmap_2d part ways: in costmap_2d the cells outside the static layer's bounds box (the map's extent,
+ * taken in map coordinates and applied in the costmap's frame) keep what updateOrigin shifted in from the previous cycle;
+ * here every cell the map does not cover gets the default. Only the static layer is built: no obstacle, voxel or
+ * inflation layer, no footprint clearing, no use_maximum.
+ *
+ * A robot whose map_id is outside 0 .. W - 1, whose map has a size < 1, a non-positive or non-finite resolution or bytes
+ * past pool_bytes, or whose sx or sy < 1, sx * sy > cell_cap or resolution is non-positive or not finite gets an
+ * all-default row, keeps its origin and a status other than TEB_COSTMAP_WINDOW_OK (the device entry point); the host
+ * entry point refuses the same inputs with TEBGPU_ERR_INVALID_ARG. */
+typedef struct TebStaticMaps {
+  int32_t W;                    /* maps, >= 1 */
+  int32_t unknown_cost_value;   /* StaticLayer unknown_cost_value as the byte it compares with, 0 .. 255 (default -1: 255) */
+  int32_t lethal_threshold;     /* 0 .. 255 (default 100; costmap_2d clamps its parameter to 0 .. 100) */
+  int32_t track_unknown_space;  /* default true */
+  int32_t trinary_costmap;      /* default true */
+  int32_t _pad;
+  int64_t pool_bytes;           /* bytes of data */
+  const uint8_t* data;          /* [pool_bytes] the OccupancyGrids' bytes, map m row-major at offset[m]: cell (mx, my) at
+                                   offset[m] + my * msx + mx (nav_msgs/OccupancyGrid's data, int8 read as unsigned char) */
+  const int64_t* offset;        /* [W] */
+  const int32_t* size;          /* [W][2] msx, msy */
+  const double*  origin;        /* [W][3] mox, moy, mr (info.origin.position.x / y, info.resolution) */
+} TebStaticMaps;
+
+typedef struct TebCostmapWindowArgs {
+  int32_t S;                    /* robots, 1 .. max_scenes */
+  int32_t cell_cap;             /* raster bytes per robot (stride of cost), >= 1 */
+  const double*  robot;         /* [S][3] x, y, yaw of the robot in the costmap's global frame (only x, y are read) */
+  const int32_t* map_id;        /* [S] */
+  const double*  costmap_to_map;/* [S][7] or NULL: tx, ty, tz, qx, qy, qz, qw (NULL: the identity) */
+  double*        origin;        /* [S][3] in/out: ox, oy, r (TebCostmapArgs.origin); r is read only */
+  const int32_t* grid;          /* [S][2] sx, sy (TebCostmapArgs.grid) */
+  uint8_t*       cost;          /* [S][cell_cap] out (TebCostmapArgs.cost) */
+  int32_t*       status;        /* [S] out: TEB_COSTMAP_WINDOW_* */
+} TebCostmapWindowArgs;
+#define TEB_COSTMAP_WINDOW_OK       0
+#define TEB_COSTMAP_WINDOW_BAD_MAP  1   /* map_id out of range, or the map's size, resolution or bytes out of range */
+#define TEB_COSTMAP_WINDOW_BAD_GRID 2   /* sx or sy < 1, sx * sy > cell_cap, or a non-positive / non-finite resolution */
+
 /* The controller state of every robot between cycles, and the two steps of TebLocalPlannerROS::computeVelocityCommands
  * around plan() that read and write it: tebgpu_backup_modes, the oscillation half of configureBackupModes
  * (teb_local_planner_ros.cpp:980-1016, with FailureDetector of recovery_behaviors.cpp), after tebgpu_local_plan and
@@ -644,7 +712,7 @@ typedef struct TebCycleArgs {
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
  * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs, 13 TebHsigFactors, 14 TebFleetArgs,
- * 15 TebFleetRow, 16 TebFleetTable, 17 TebFleetShapes. */
+ * 15 TebFleetRow, 16 TebFleetTable, 17 TebFleetShapes, 18 TebStaticMaps, 19 TebCostmapWindowArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -789,6 +857,19 @@ int32_t tebgpu_local_plan_tf_device(tebgpu_ctx* ctx, const TebBatch* batch, cons
 int32_t tebgpu_costmap_obstacles_tf(tebgpu_ctx* ctx, const TebCostmapArgs* args, const TebFrameArgs* frames);
 int32_t tebgpu_costmap_obstacles_tf_device(tebgpu_ctx* ctx, const TebCostmapArgs* args, const TebFrameArgs* frames,
                                            void* cuda_stream);
+
+/* Every robot's local costmap window cut out of the static maps, as defined at TebStaticMaps: window, then convert,
+ * plan and check on the same stream. Two launches: one thread per robot snaps the origin and writes the status, then
+ * CTAs of 256 threads write each robot's row of cell_cap bytes in 16-byte stores, each lane 16 consecutive cells, the
+ * map bytes read through the read-only cache (tebgpu_get_info key 20: the second launch's grid in CTAs). Argument errors
+ * (NULL maps, args or required arrays, S outside 1 .. max_scenes, cell_cap < 1, W < 1, pool_bytes < 0,
+ * unknown_cost_value or lethal_threshold outside 0 .. 255) return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a
+ * limit) before anything is launched. tebgpu_costmap_window: HOST buffers, synchronous; the maps are uploaded by every
+ * call, and the robots the device entry point marks bad are refused with TEBGPU_ERR_INVALID_ARG. tebgpu_costmap_window_
+ * device: DEVICE buffers (the maps' arrays too), stream ordered as tebgpu_optimize_batch_device, does not synchronise. */
+int32_t tebgpu_costmap_window(tebgpu_ctx* ctx, const TebStaticMaps* maps, const TebCostmapWindowArgs* args);
+int32_t tebgpu_costmap_window_device(tebgpu_ctx* ctx, const TebStaticMaps* maps, const TebCostmapWindowArgs* args,
+                                     void* cuda_stream);
 
 /* The two controller steps around plan(), as defined at TebCycleArgs. One thread per band, so that the detector's sums
  * run in the reference's order (tebgpu_get_info key 17). A fleet cycle on one stream: tebgpu_costmap_obstacles_device,

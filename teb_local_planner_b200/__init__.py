@@ -76,6 +76,10 @@ def load_library(build_if_missing=False):
     L.tebgpu_costmap_obstacles_tf.argtypes = [vp, C.POINTER(abi.TebCostmapArgs), C.POINTER(abi.TebFrameArgs)]
     L.tebgpu_costmap_obstacles_tf_device.restype = C.c_int32
     L.tebgpu_costmap_obstacles_tf_device.argtypes = [vp, C.POINTER(abi.TebCostmapArgs), C.POINTER(abi.TebFrameArgs), vp]
+    L.tebgpu_costmap_window.restype = C.c_int32
+    L.tebgpu_costmap_window.argtypes = [vp, C.POINTER(abi.TebStaticMaps), C.POINTER(abi.TebCostmapWindowArgs)]
+    L.tebgpu_costmap_window_device.restype = C.c_int32
+    L.tebgpu_costmap_window_device.argtypes = [vp, C.POINTER(abi.TebStaticMaps), C.POINTER(abi.TebCostmapWindowArgs), vp]
     L.tebgpu_local_plan_tf.restype = C.c_int32
     L.tebgpu_local_plan_tf.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs),
                                        C.POINTER(abi.TebFrameArgs)]
@@ -179,7 +183,8 @@ def load_library(build_if_missing=False):
                                 abi.TebPlanInput, abi.TebFeasibilityArgs, abi.TebTrajectoryArgs, abi.TebCostmapArgs,
                                 abi.TebLocalPlanArgs, abi.TebCycleArgs, abi.TebCostmapWorld, abi.TebFrameArgs,
                                 abi.TebHsigFactors, abi.TebFleetArgs))) + ((15, None), (16, abi.TebFleetTable),
-                                                                (17, abi.TebFleetShapes)):
+                                                                (17, abi.TebFleetShapes), (18, abi.TebStaticMaps),
+                                                                (19, abi.TebCostmapWindowArgs)):
         if st is None:
             if L.tebgpu_sizeof(which) != abi.FLEET_ROW_DTYPE.itemsize:
                 raise RuntimeError(f"ABI mismatch for TebFleetRow: C {L.tebgpu_sizeof(which)} vs FLEET_ROW_DTYPE "
@@ -428,6 +433,43 @@ class TebGpu:
     def last_costmap_grid(self):
         """grid in CTAs (one per scene) of the last costmap conversion, 0 before the first"""
         return self.info(15)
+
+    def costmap_window(self, maps, robot, map_id, origin, grid, cell_cap=None, costmap_to_map=None):
+        """Every robot's local costmap cut out of the static maps (tebgpu_costmap_window), host buffers, as
+        include/teb_b200.h defines it at TebStaticMaps: maps an abi.TebStaticMaps of host arrays (abi.make_static_maps),
+        robot [S][3], map_id [S], origin [S][3] (ox, oy, resolution: the previous cycle's origin), grid [S][2] (sx, sy),
+        cell_cap (None: the largest sx * sy rounded up to 16 bytes), costmap_to_map [S][7] or None (the identity).
+        Returns (cost [S][cell_cap] uint8, origin [S][3] the snapped origins, status [S] int32 TEB_COSTMAP_WINDOW_*);
+        the arguments are not modified."""
+        import numpy as np
+        robot = np.ascontiguousarray(robot, dtype=np.float64).reshape(-1, 3)
+        S = robot.shape[0]
+        mid = np.ascontiguousarray(map_id, dtype=np.int32).reshape(S)
+        org = np.array(origin, dtype=np.float64).reshape(S, 3)
+        grid = np.ascontiguousarray(grid, dtype=np.int32).reshape(S, 2)
+        if cell_cap is None:
+            cell_cap = max(16, (int((grid[:, 0].astype(np.int64) * grid[:, 1]).max()) + 15) // 16 * 16)
+        tf = None if costmap_to_map is None else np.ascontiguousarray(costmap_to_map, dtype=np.float64).reshape(S, 7)
+        cost = np.zeros((S, int(cell_cap)), np.uint8)
+        status = np.zeros(S, np.int32)
+        wa = abi.TebCostmapWindowArgs()
+        wa.S, wa.cell_cap = S, int(cell_cap)
+        wa.robot, wa.map_id, wa.costmap_to_map = abi.ptr(robot), abi.ptr(mid), abi.ptr(tf)
+        wa.origin, wa.grid, wa.cost, wa.status = abi.ptr(org), abi.ptr(grid), abi.ptr(cost), abi.ptr(status)
+        self._check(self.lib.tebgpu_costmap_window(self.ctx, C.byref(maps), C.byref(wa)), "tebgpu_costmap_window")
+        return cost, org, status
+
+    def costmap_window_device(self, maps, args, stream=None):
+        """tebgpu_costmap_window_device: the same step over DEVICE memory (maps: an abi.TebStaticMaps of device arrays;
+        args: an abi.TebCostmapWindowArgs of device pointers, whose cost / grid / origin are the TebCostmapArgs arrays
+        the costmap conversion and the costmap check read next). Stream ordered on `stream` (a cudaStream_t handle;
+        None: the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_costmap_window_device(self.ctx, C.byref(maps), C.byref(args), stream),
+                    "tebgpu_costmap_window_device")
+
+    def last_window_grid(self):
+        """grid in CTAs of the last costmap window's raster launch, 0 before the first"""
+        return self.info(20)
 
     def local_plan(self, global_plan, plan_begin, plan_end, robot, robot_vel, grid, origin, P_cap, V_cap=None,
                    scene_id=None, via_count=None, infeasible_count=None, since_infeasible=None, costmap_to_plan=None,

@@ -235,6 +235,52 @@ class TebFrameArgs(C.Structure):
                 ("custom_to_costmap", C.c_void_p), ("custom_vertices", C.c_void_p), ("obst_vertices", C.c_void_p)]
 
 
+class TebStaticMaps(C.Structure):
+    """The static maps of tebgpu_costmap_window: W OccupancyGrids in one byte pool (offset [W] int64, size [W][2] int32
+    msx, msy, origin [W][3] mox, moy, resolution) and StaticLayer's interpretValue parameters; host or device pointers"""
+    _fields_ = [("W", _i), ("unknown_cost_value", _i), ("lethal_threshold", _i), ("track_unknown_space", _i),
+                ("trinary_costmap", _i), ("_pad", _i), ("pool_bytes", C.c_int64), ("data", C.c_void_p),
+                ("offset", C.c_void_p), ("size", C.c_void_p), ("origin", C.c_void_p)]
+
+
+class TebCostmapWindowArgs(C.Structure):
+    """Every robot's rolling window (tebgpu_costmap_window): robot poses, map ids, optional costmap -> map transforms,
+    the origins carried between cycles, the window sizes, and the cost / status outputs; host or device pointers"""
+    _fields_ = [("S", _i), ("cell_cap", _i), ("robot", C.c_void_p), ("map_id", C.c_void_p),
+                ("costmap_to_map", C.c_void_p), ("origin", C.c_void_p), ("grid", C.c_void_p), ("cost", C.c_void_p),
+                ("status", C.c_void_p)]
+
+
+# TEB_COSTMAP_WINDOW_*: each robot's status after tebgpu_costmap_window
+TEB_COSTMAP_WINDOW_OK, TEB_COSTMAP_WINDOW_BAD_MAP, TEB_COSTMAP_WINDOW_BAD_GRID = 0, 1, 2
+
+
+def make_static_maps(grids, origins, unknown_cost_value=-1, lethal_threshold=100, track_unknown_space=True,
+                     trinary_costmap=True):
+    """The static maps of tebgpu_costmap_window from nav_msgs/OccupancyGrid data: grids, a list of W int8 arrays
+    [msy][msx] (row my holds cells my * msx .. my * msx + msx - 1, the message's data), origins [W][3] (origin x, y,
+    resolution). The defaults are StaticLayer's. Returns (TebStaticMaps of host pointers, dict of the numpy arrays it
+    points into: data [pool_bytes] uint8, offset [W] int64, size [W][2] int32, origin [W][3] float64), the dict also
+    kept on the struct as `arrays`; upload the arrays and set the pointers for the _device entry point."""
+    grids = [np.asarray(g) for g in grids]
+    if any(g.ndim != 2 or g.dtype not in (np.int8, np.uint8) for g in grids):
+        raise ValueError("each grid must be a 2-D int8 (or uint8) array [msy][msx]")
+    size = np.array([(g.shape[1], g.shape[0]) for g in grids], np.int32).reshape(-1, 2)
+    offset = np.zeros(len(grids), np.int64)
+    if len(grids) > 1:
+        offset[1:] = np.cumsum([g.size for g in grids[:-1]])
+    data = (np.concatenate([g.reshape(-1).view(np.uint8) for g in grids]) if grids else np.zeros(0, np.uint8))
+    origin = np.ascontiguousarray(origins, dtype=np.float64).reshape(len(grids), 3)
+    m = TebStaticMaps()
+    m.W, m.pool_bytes = len(grids), int(data.size)
+    m.unknown_cost_value, m.lethal_threshold = int(unknown_cost_value) & 0xFF, int(lethal_threshold)
+    m.track_unknown_space, m.trinary_costmap = int(bool(track_unknown_space)), int(bool(trinary_costmap))
+    arrays = dict(data=data, offset=offset, size=size, origin=origin)
+    m.data, m.offset, m.size, m.origin = ptr(data), ptr(offset), ptr(size), ptr(origin)
+    m.arrays = arrays
+    return m, arrays
+
+
 class TebHsigFactors(C.Structure):
     """Every scene's factor table of the 2-D H-signature (tebgpu_hsig_factors): factor [S][M_cap][2] float64, the
     mantissa of Q_l = 1 / prod_j (o_l - o_j); factor_exp [S][M_cap] int32, its binary exponent (INT32_MIN for 0);

@@ -23,6 +23,7 @@
 #include "teb_plan.cuh"
 #include "teb_feasible.cuh"
 #include "teb_costmap.cuh"
+#include "teb_costmap_window.cuh"
 #include "teb_local_plan.cuh"
 #include "teb_cycle.cuh"
 #include "teb_fleet.cuh"
@@ -133,6 +134,10 @@ struct tebgpu_ctx {
   size_t ccost_bytes = 0, cgrid_bytes = 0, corigin_bytes = 0, crobot_bytes = 0, ccustom_bytes = 0, ccount_bytes = 0,
          cobst_bytes = 0, cocount_bytes = 0, cneeded_bytes = 0;
   long long last_costmap_grid = 0;    /* grid in CTAs of the last k_costmap_obstacles launch */
+  /* costmap windows: the host-buffer entry point's maps, inputs and outputs, staged in one buffer grown by the first
+   * call that needs more */
+  char* d_cwin = nullptr; size_t cwin_bytes = 0;
+  long long last_window_grid = 0;     /* grid in CTAs of the last k_costmap_window launch */
   /* local plan: the host-buffer entry point's inputs and outputs, staged in one buffer grown by the first call that
    * needs more */
   char* d_lplan = nullptr; size_t lplan_bytes = 0;
@@ -260,6 +265,8 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 15: return (int32_t)sizeof(TebFleetRow);
     case 16: return (int32_t)sizeof(TebFleetTable);
     case 17: return (int32_t)sizeof(TebFleetShapes);
+    case 18: return (int32_t)sizeof(TebStaticMaps);
+    case 19: return (int32_t)sizeof(TebCostmapWindowArgs);
     default: return -1;
   }
 }
@@ -289,6 +296,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 17: return ctx->last_cycle_grid;
     case 18: return ctx->last_fleet_grid;
     case 19: return ctx->last_fleet_search;
+    case 20: return ctx->last_window_grid;
     default: return -1;
   }
 }
@@ -300,7 +308,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
                   c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
-                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid, c->d_fshape};
+                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid, c->d_fshape, c->d_cwin};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -1856,6 +1864,88 @@ int32_t tebgpu_costmap_obstacles_tf(tebgpu_ctx* ctx, const TebCostmapArgs* ca, c
     if (rows)
       CUDA_TRY(ctx, cudaMemcpyAsync(ca->obstacles + s * M, ctx->d_cobst + s * M, rows * sizeof(TebObstacle), cudaMemcpyDeviceToHost, st));
   }
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* argument checks of both costmap window entry points: nothing is launched when one fails */
+static int32_t check_window_args(tebgpu_ctx* ctx, const TebStaticMaps* m, const TebCostmapWindowArgs* wa) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!m || !wa) { ctx->err = "static maps or window args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (wa->S < 1 || wa->cell_cap < 1) { ctx->err = "bad window dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (wa->S > ctx->lim.max_scenes) { ctx->err = "window robots exceed the context's max_scenes"; return TEBGPU_ERR_CAPACITY; }
+  if (m->W < 1 || m->pool_bytes < 0) { ctx->err = "bad static map dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (m->unknown_cost_value < 0 || m->unknown_cost_value > 255 || m->lethal_threshold < 0 || m->lethal_threshold > 255) {
+    ctx->err = "unknown_cost_value / lethal_threshold outside 0 .. 255"; return TEBGPU_ERR_INVALID_ARG;
+  }
+  if ((m->pool_bytes > 0 && !m->data) || !m->offset || !m->size || !m->origin) { ctx->err = "missing static map array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!wa->robot || !wa->map_id || !wa->origin || !wa->grid || !wa->cost || !wa->status) { ctx->err = "missing required window array"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_costmap_window_origin, then k_costmap_window, on arguments already checked */
+static int32_t issue_window(tebgpu_ctx* ctx, const TebStaticMaps* m, const TebCostmapWindowArgs* wa, cudaStream_t st) {
+  const unsigned strips = (unsigned)std::min<long long>(std::max<long long>(((long long)wa->cell_cap + WINDOW_STRIP_BYTES - 1) / WINDOW_STRIP_BYTES, 1), 65535);
+  k_costmap_window_origin<<<(wa->S + WINDOW_THREADS - 1) / WINDOW_THREADS, WINDOW_THREADS, 0, st>>>(*m, *wa);
+  const dim3 grid((unsigned)wa->S, strips);
+  if (wa->costmap_to_map) k_costmap_window<true><<<grid, WINDOW_THREADS, 0, st>>>(*m, *wa);
+  else k_costmap_window<false><<<grid, WINDOW_THREADS, 0, st>>>(*m, *wa);
+  ctx->last_window_grid = (long long)wa->S * strips;
+  ctx->launches = 2;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_costmap_window_device(tebgpu_ctx* ctx, const TebStaticMaps* m, const TebCostmapWindowArgs* wa,
+                                     void* cuda_stream) {
+  const int32_t rc = check_window_args(ctx, m, wa);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_window(ctx, m, wa, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_costmap_window(tebgpu_ctx* ctx, const TebStaticMaps* m, const TebCostmapWindowArgs* wa) {
+  int32_t rc = check_window_args(ctx, m, wa);
+  if (rc) return rc;
+  /* the robots the device entry point would answer with a default row are refused here, before anything runs */
+  for (int s = 0; s < wa->S; ++s) {
+    const int st = costmap_window_status(*m, *wa, s);
+    if (st == TEB_COSTMAP_WINDOW_BAD_MAP) { ctx->err = "map_id[s] out of range, or its map's size, resolution or bytes"; return TEBGPU_ERR_INVALID_ARG; }
+    if (st != TEB_COSTMAP_WINDOW_OK) { ctx->err = "grid[s] outside 1 .. cell_cap cells, or a bad resolution"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t S = wa->S, W = m->W, cells = S * (size_t)wa->cell_cap, pool = (size_t)m->pool_bytes;
+  const bool tf = wa->costmap_to_map != nullptr;
+  /* one staging buffer: every array at a 256-byte aligned offset, so the raster rows keep their alignment mod 16 */
+  size_t off = 0;
+  auto slot = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_data = slot(pool), o_moff = slot(W * 8), o_msize = slot(W * 2 * 4), o_morg = slot(W * 3 * sizeof(double)),
+               o_robot = slot(S * 3 * sizeof(double)), o_id = slot(S * 4), o_tf = slot(tf ? S * 7 * sizeof(double) : 0),
+               o_origin = slot(S * 3 * sizeof(double)), o_grid = slot(S * 2 * 4), o_cost = slot(cells), o_status = slot(S * 4);
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_cwin, &ctx->cwin_bytes, off, st))) return rc;
+  char* d = ctx->d_cwin;
+  auto up = [&](size_t o, const void* src, size_t bytes) -> int32_t {
+    if (src && bytes) CUDA_TRY(ctx, cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, st));
+    return TEBGPU_OK;
+  };
+  if ((rc = up(o_data, m->data, pool)) || (rc = up(o_moff, m->offset, W * 8)) || (rc = up(o_msize, m->size, W * 2 * 4)) ||
+      (rc = up(o_morg, m->origin, W * 3 * sizeof(double))) || (rc = up(o_robot, wa->robot, S * 3 * sizeof(double))) ||
+      (rc = up(o_id, wa->map_id, S * 4)) || (rc = up(o_tf, wa->costmap_to_map, tf ? S * 7 * sizeof(double) : 0)) ||
+      (rc = up(o_origin, wa->origin, S * 3 * sizeof(double))) || (rc = up(o_grid, wa->grid, S * 2 * 4)))
+    return rc;
+  TebStaticMaps dm = *m;
+  dm.data = pool ? (const uint8_t*)(d + o_data) : nullptr;
+  dm.offset = (const int64_t*)(d + o_moff); dm.size = (const int32_t*)(d + o_msize); dm.origin = (const double*)(d + o_morg);
+  TebCostmapWindowArgs da = *wa;
+  da.robot = (const double*)(d + o_robot); da.map_id = (const int32_t*)(d + o_id);
+  da.costmap_to_map = tf ? (const double*)(d + o_tf) : nullptr;
+  da.origin = (double*)(d + o_origin); da.grid = (const int32_t*)(d + o_grid);
+  da.cost = (uint8_t*)(d + o_cost); da.status = (int32_t*)(d + o_status);
+  if ((rc = issue_window(ctx, &dm, &da, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(wa->cost, da.cost, cells, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(wa->origin, da.origin, S * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(wa->status, da.status, S * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
 }
