@@ -606,6 +606,109 @@ typedef struct TebCostmapWindowArgs {
 #define TEB_COSTMAP_WINDOW_BAD_MAP  1   /* map_id out of range, or the map's size, resolution or bytes out of range */
 #define TEB_COSTMAP_WINDOW_BAD_GRID 2   /* sx or sy < 1, sx * sy > cell_cap, or a non-positive / non-finite resolution */
 
+/* Every robot's obstacle layer, marked and cleared from its sensor points (tebgpu_costmap_obstacle_layer): what
+ * costmap_2d's ObstacleLayer adds to a local costmap, the cells where the sensors see something the static map lacks. The
+ * caller owns each robot's layer grid (layer / layer_origin), kept between cycles; the result is written into the master
+ * raster in TebCostmapArgs' layout (cost / grid / origin), so tebgpu_costmap_obstacles(_tf)_device and
+ * tebgpu_check_feasible_costmap_device read it unchanged on the same stream. mode TEB_OBSTACLE_LAYER_COMBINE runs after
+ * tebgpu_costmap_window in the same cycle, on top of the static window; TEB_OBSTACLE_LAYER_STANDALONE is a local costmap
+ * with the obstacle layer as its only plugin.
+ *
+ * costmap_2d is not part of the reference checkout; this restates ROS Noetic navigation (costmap_2d 1.17):
+ * ObstacleLayer::updateBounds / raytraceFreespace / updateFootprint / updateCosts, Costmap2D::updateOrigin / worldToMap /
+ * cellDistance / raytraceLine / bresenham2D / setConvexPolygonCost / convexFillCells / polygonOutlineCells,
+ * costmap_2d::transformFootprint, CostmapLayer::updateWithOverwrite / updateWithMax and the height filter of
+ * ObservationBuffer::bufferCloud. Every product and sum is rounded on its own (no FMA contraction). Robot s, with (sx, sy)
+ * = grid[s], r = origin[s][2], the layer default d = 255 with track_unknown_space, else 0:
+ *   1. Origin and shift. (ox, oy) = layer_origin[s] moves as the window's origin does (costmap_window_snap, TebStaticMaps
+ *      step 1) toward the robot: (cx, cy) the whole cells moved, (ox', oy') = (ox + cx r, oy + cy r). Layer cell (i, j)
+ *      takes the previous cell (i + cx, j + cy) when that lies in the grid, d otherwise (a move of sx / sy cells or more,
+ *      or a NaN one, leaves every cell d). Combine: (ox', oy') must equal origin[s][0..1] bit for bit (the window just
+ *      wrote it), else TEB_OBSTACLE_LAYER_ORIGIN_MISMATCH. Standalone: (ox', oy') is written to origin[s][0..1] and the
+ *      master row is first reset to master_default, the LayeredCostmap's own default byte.
+ *   2. Height filter (bufferCloud): a point is kept when min_obstacle_height <= z <= max_obstacle_height, the float z
+ *      compared with the doubles; it applies to marking and clearing alike.
+ *   3. Clearing, when clearing != 0 (raytraceFreespace). With (so_x, so_y) = sensor_origin[s]: when worldToMap of the
+ *      sensor fails there is no clearing this call (flag TEB_OBSTACLE_LAYER_SENSOR_OFF_MAP). Otherwise each kept point
+ *      (wx, wy) with a = wx - so_x, b = wy - so_y is clamped by four tests in order: wx < ox': t = (ox' - so_x) / a, wx =
+ *      ox', wy = so_y + b t; wy < oy': t = (oy' - so_y) / b, wx = so_x + a t, wy = oy'; wx > ex = ox' + sx r: t = (ex -
+ *      so_x) / a, wx = ex - .001, wy = so_y + b t (t of the unshifted end); wy > ey likewise. A point whose clamped
+ *      worldToMap fails is skipped; otherwise raytraceLine from the sensor's cell to it with max_length = cellDistance
+ *      (raytrace_range) = (unsigned)max(0, ceil(raytrace_range / r)) (saturated at UINT_MAX) writes FREE_SPACE (0) to
+ *      every cell visited: dx, dy the integer deltas, dist = hypot(dx, dy) (sqrt of the exact sum of squares, the
+ *      correctly rounded hypot), scale = dist == 0 ? 1 : min(1, max_length / dist), the major axis the x axis when |dx|
+ *      >= |dy|; bresenham2D runs (unsigned)(scale abs_da) steps from error_b = abs_da / 2 and visits the cell it ends on.
+ *   4. Marking, when marking != 0, after all clearing: a kept point (px, py, pz) is skipped when pz >
+ *      layer_max_obstacle_height, when ((px - so_x)^2 + (py - so_y)^2) + (pz - so_z)^2 >= obstacle_range^2, or when its
+ *      worldToMap fails; otherwise its cell becomes LETHAL_OBSTACLE (254).
+ *   5. Footprint clearing, when F >= 3 (updateFootprint / setConvexPolygonCost): the footprint placed at robot[s]
+ *      (transformFootprint: x + (px cos - py sin), y + (px sin + py cos)); when a vertex's worldToMap fails nothing is
+ *      cleared (flag TEB_OBSTACLE_LAYER_FOOTPRINT_OFF_MAP); otherwise the cells of convexFillCells get FREE_SPACE.
+ *      convexFillCells restated: the outline is raytraceLine over every edge and the closing edge, both ends and
+ *      duplicates kept, swap-sorted by x (stable), then a column loop takes the cells two at a time and appends each
+ *      column's fill to the vector it reads. Every column from the least to the greatest vertex x holds at least two
+ *      outline cells (each vertex ends one edge and starts the next; a column between them is crossed on the way out and
+ *      on the way back), so each pair lies in its own column, the loop never reaches the cells it appended, and the fill
+ *      is, per column, every cell from the least to the greatest outline y. That span is what the device writes.
+ *   6. Combination over the sx * sy cells: combination_method 0 updateWithOverwrite (a layer cell of 255 is skipped,
+ *      another is copied), 1 updateWithMax (a layer cell of 255 is skipped, another replaces a master cell that is 255
+ *      or smaller than it), anything else leaves the master as it is (the layer is still updated).
+ * worldToMap: off the map when wx < ox' or wy < oy'; otherwise mx = (int)((wx - ox') / r), my likewise, on the map when
+ * mx < sx and my < sy; a quotient that is NaN or not below the size (where C's int conversion is undefined or the cell
+ * lies past the map) is off the map. NaN and infinite coordinates follow the same arithmetic. Every phase writes one
+ * value, so the order of stores inside a phase does not matter; only the phase boundaries are kept. The layer bytes of a
+ * row past sx * sy get d; the master bytes past sx * sy are left (combine) or master_default (standalone).
+ *
+ * Where this and costmap_2d part ways: costmap_2d combines the layer into the master only inside the bounds box of the
+ * cycle (the sensor origin with raytrace_range around it, the marks and the placed footprint); outside it the master
+ * keeps what updateOrigin shifted in. Here the layer is combined over the whole window. Outside the box the layer holds
+ * exactly what its own shift carried, so when the previous master row was made this way (the static window of the same
+ * map cell below, then this combination), combining again gives what the master's shift carried; they part where a cell
+ * that only this cycle shifted in lies outside the box (the window's default against the window's map cell, or, in
+ * standalone mode, master_default against the combination of d). One observation per robot per call: several sources and
+ * observation_persistence are not built, and clearing every source before marking any cannot be had from two calls. The
+ * device's sin / cos place the footprint. The grid size is fixed per robot: a caller who changes it resets the layer, as
+ * matchSize would.
+ *
+ * A robot whose sx or sy < 1, sx * sy > cell_cap, resolution is non-positive or not finite, or whose layer_origin or
+ * robot x / y is not finite (its snapped origin would be NaN) gets TEB_OBSTACLE_LAYER_BAD_GRID, one whose point_count
+ * is outside 0 .. P_cap TEB_OBSTACLE_LAYER_BAD_POINTS; such a robot and one with ORIGIN_MISMATCH keep their layer and layer_origin, their master row untouched (combine) or all
+ * master_default (standalone) and their origin (the device entry point); the host entry point refuses them. */
+typedef struct TebObstacleLayerArgs {
+  int32_t S;                     /* robots, 1 .. max_scenes */
+  int32_t cell_cap;              /* bytes per robot of layer and cost, 1 .. tebgpu_get_info key 21 */
+  int32_t P_cap;                 /* points per robot (stride of points), >= 0 */
+  int32_t F;                     /* footprint points, 0 .. TEB_COSTMAP_FOOTPRINT_MAX; F < 3: no footprint clearing */
+  int32_t mode;                  /* TEB_OBSTACLE_LAYER_COMBINE or _STANDALONE */
+  int32_t combination_method;    /* 0 overwrite, 1 maximum, anything else: not combined */
+  int32_t track_unknown_space;   /* the layer's (its default 255, else 0) */
+  int32_t master_default;        /* standalone: the byte the master row is reset to, 0 .. 255 */
+  int32_t clearing, marking;     /* the observation source's flags */
+  double obstacle_range, raytrace_range;            /* >= 0 */
+  double min_obstacle_height, max_obstacle_height;  /* the observation source's height filter */
+  double layer_max_obstacle_height;                 /* the layer's max_obstacle_height */
+  const double*  footprint;      /* [F][2] HOST (both entry points), finite: the footprint in the robot frame */
+  const float*   points;         /* [S][P_cap][3] x, y, z in the costmap's global frame (NULL when P_cap is 0) */
+  const int32_t* point_count;    /* [S] */
+  const double*  sensor_origin;  /* [S][3] x, y, z of the observation's origin in the global frame */
+  const double*  robot;          /* [S][3] x, y, yaw of the robot in the global frame */
+  const int32_t* grid;           /* [S][2] sx, sy (TebCostmapArgs.grid) */
+  uint8_t*       layer;          /* [S][cell_cap] in/out: the layer grid */
+  double*        layer_origin;   /* [S][2] in/out: the origin the layer was last written at */
+  double*        origin;         /* [S][3] TebCostmapArgs.origin: read (combine), ox, oy written (standalone); r read */
+  uint8_t*       cost;           /* [S][cell_cap] in/out: the master raster (TebCostmapArgs.cost) */
+  int32_t*       status;         /* [S] out: TEB_OBSTACLE_LAYER_* */
+  int32_t*       flags;          /* [S] out or NULL: TEB_OBSTACLE_LAYER_SENSOR_OFF_MAP | _FOOTPRINT_OFF_MAP */
+} TebObstacleLayerArgs;
+#define TEB_OBSTACLE_LAYER_COMBINE          0
+#define TEB_OBSTACLE_LAYER_STANDALONE       1
+#define TEB_OBSTACLE_LAYER_OK               0
+#define TEB_OBSTACLE_LAYER_BAD_GRID         1   /* sizes, cell_cap, resolution, non-finite layer_origin or robot x / y */
+#define TEB_OBSTACLE_LAYER_BAD_POINTS       2   /* point_count outside 0 .. P_cap */
+#define TEB_OBSTACLE_LAYER_ORIGIN_MISMATCH  3   /* combine: the snapped layer origin is not the master's */
+#define TEB_OBSTACLE_LAYER_SENSOR_OFF_MAP   1   /* flag: the sensor origin is off the layer, no clearing */
+#define TEB_OBSTACLE_LAYER_FOOTPRINT_OFF_MAP 2  /* flag: a placed footprint vertex is off the layer, no footprint clearing */
+
 /* The controller state of every robot between cycles, and the two steps of TebLocalPlannerROS::computeVelocityCommands
  * around plan() that read and write it: tebgpu_backup_modes, the oscillation half of configureBackupModes
  * (teb_local_planner_ros.cpp:980-1016, with FailureDetector of recovery_behaviors.cpp), after tebgpu_local_plan and
@@ -712,7 +815,8 @@ typedef struct TebCycleArgs {
 /* sizeof() of the ABI structs, for binding sanity checks. which: 0 TebParams, 1 TebObstacle, 2 TebBatch,
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
  * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs, 13 TebHsigFactors, 14 TebFleetArgs,
- * 15 TebFleetRow, 16 TebFleetTable, 17 TebFleetShapes, 18 TebStaticMaps, 19 TebCostmapWindowArgs. */
+ * 15 TebFleetRow, 16 TebFleetTable, 17 TebFleetShapes, 18 TebStaticMaps, 19 TebCostmapWindowArgs,
+ * 20 TebObstacleLayerArgs. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -870,6 +974,20 @@ int32_t tebgpu_costmap_obstacles_tf_device(tebgpu_ctx* ctx, const TebCostmapArgs
 int32_t tebgpu_costmap_window(tebgpu_ctx* ctx, const TebStaticMaps* maps, const TebCostmapWindowArgs* args);
 int32_t tebgpu_costmap_window_device(tebgpu_ctx* ctx, const TebStaticMaps* maps, const TebCostmapWindowArgs* args,
                                      void* cuda_stream);
+
+/* Every robot's obstacle layer, as defined at TebObstacleLayerArgs: (window,) obstacle layer, then convert, plan and
+ * check on the same stream. One launch, one CTA of 256 threads per robot with the robot's layer row staged in dynamic
+ * shared memory: the shifted row, then every point's ray walked by one thread, the marks, the footprint's column spans
+ * by one warp, then the layer row stored in place and the master row combined in 16-byte stores. cell_cap is bounded by
+ * the opt-in shared memory a CTA may have (tebgpu_get_info key 21, in bytes): past it TEBGPU_ERR_CAPACITY. Argument
+ * errors (NULL args or required arrays, S outside 1 .. max_scenes, cell_cap < 1, P_cap < 0, F outside 0 ..
+ * TEB_COSTMAP_FOOTPRINT_MAX, a non-finite footprint point, a negative or NaN range, mode not COMBINE / STANDALONE,
+ * master_default outside 0 .. 255) return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit) before anything is
+ * launched. tebgpu_costmap_obstacle_layer: HOST buffers, synchronous; robots the device entry point would mark with a
+ * status other than TEB_OBSTACLE_LAYER_OK are refused with TEBGPU_ERR_INVALID_ARG. tebgpu_costmap_obstacle_layer_device:
+ * DEVICE buffers (footprint on the host), stream ordered as tebgpu_optimize_batch_device, does not synchronise. */
+int32_t tebgpu_costmap_obstacle_layer(tebgpu_ctx* ctx, const TebObstacleLayerArgs* args);
+int32_t tebgpu_costmap_obstacle_layer_device(tebgpu_ctx* ctx, const TebObstacleLayerArgs* args, void* cuda_stream);
 
 /* The two controller steps around plan(), as defined at TebCycleArgs. One thread per band, so that the detector's sums
  * run in the reference's order (tebgpu_get_info key 17). A fleet cycle on one stream: tebgpu_costmap_obstacles_device,
@@ -1274,7 +1392,8 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * of the last backup-modes or finish-cycle launch (k_backup_modes / k_finish_cycle, 128 bands per CTA; 0 before the
  * first), 18 grid in CTAs of the last fleet-obstacle launch (k_fleet_obstacles or k_fleet_obstacles_grid, FLEET_WARPS
  * robots per CTA; 0 before the first), 19 the search that launch ran (TEBGPU_FLEET_SEARCH_ALL_PAIRS, _GRID or
- * _ONE_BUCKET; -1 before the first).
+ * _ONE_BUCKET; -1 before the first), 20 grid in CTAs of the last costmap window raster launch, 21 the largest cell_cap
+ * tebgpu_costmap_obstacle_layer takes (bytes of a robot's row in the opt-in shared memory of one CTA).
  * Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */

@@ -80,6 +80,10 @@ def load_library(build_if_missing=False):
     L.tebgpu_costmap_window.argtypes = [vp, C.POINTER(abi.TebStaticMaps), C.POINTER(abi.TebCostmapWindowArgs)]
     L.tebgpu_costmap_window_device.restype = C.c_int32
     L.tebgpu_costmap_window_device.argtypes = [vp, C.POINTER(abi.TebStaticMaps), C.POINTER(abi.TebCostmapWindowArgs), vp]
+    L.tebgpu_costmap_obstacle_layer.restype = C.c_int32
+    L.tebgpu_costmap_obstacle_layer.argtypes = [vp, C.POINTER(abi.TebObstacleLayerArgs)]
+    L.tebgpu_costmap_obstacle_layer_device.restype = C.c_int32
+    L.tebgpu_costmap_obstacle_layer_device.argtypes = [vp, C.POINTER(abi.TebObstacleLayerArgs), vp]
     L.tebgpu_local_plan_tf.restype = C.c_int32
     L.tebgpu_local_plan_tf.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs),
                                        C.POINTER(abi.TebFrameArgs)]
@@ -184,7 +188,8 @@ def load_library(build_if_missing=False):
                                 abi.TebLocalPlanArgs, abi.TebCycleArgs, abi.TebCostmapWorld, abi.TebFrameArgs,
                                 abi.TebHsigFactors, abi.TebFleetArgs))) + ((15, None), (16, abi.TebFleetTable),
                                                                 (17, abi.TebFleetShapes), (18, abi.TebStaticMaps),
-                                                                (19, abi.TebCostmapWindowArgs)):
+                                                                (19, abi.TebCostmapWindowArgs),
+                                                                (20, abi.TebObstacleLayerArgs)):
         if st is None:
             if L.tebgpu_sizeof(which) != abi.FLEET_ROW_DTYPE.itemsize:
                 raise RuntimeError(f"ABI mismatch for TebFleetRow: C {L.tebgpu_sizeof(which)} vs FLEET_ROW_DTYPE "
@@ -470,6 +475,47 @@ class TebGpu:
     def last_window_grid(self):
         """grid in CTAs of the last costmap window's raster launch, 0 before the first"""
         return self.info(20)
+
+    def costmap_obstacle_layer(self, points, point_count, sensor_origin, robot, grid, layer, layer_origin, origin, cost,
+                               footprint=None, flags=True, **params):
+        """Every robot's obstacle layer marked and cleared from its sensor points (tebgpu_costmap_obstacle_layer), host
+        buffers, as include/teb_b200.h defines it at TebObstacleLayerArgs: points [S][P_cap][3] float32, point_count [S],
+        sensor_origin [S][3], robot [S][3] (x, y, yaw), grid [S][2], layer [S][cell_cap] uint8 and layer_origin [S][2]
+        (the previous cycle's), origin [S][3] and cost [S][cell_cap] (the master raster), footprint [F][2] or None;
+        params: the keywords of abi.make_obstacle_layer_args. Returns (layer, layer_origin, cost, origin, status, flags)
+        as new arrays (flags None when flags is False); the arguments are not modified."""
+        import numpy as np
+        pts = np.ascontiguousarray(points, dtype=np.float32)
+        S = pts.shape[0]
+        pts = pts.reshape(S, -1, 3)
+        cnt = np.ascontiguousarray(point_count, dtype=np.int32).reshape(S)
+        sen = np.ascontiguousarray(sensor_origin, dtype=np.float64).reshape(S, 3)
+        rob = np.ascontiguousarray(robot, dtype=np.float64).reshape(S, 3)
+        grd = np.ascontiguousarray(grid, dtype=np.int32).reshape(S, 2)
+        lay = np.array(layer, dtype=np.uint8).reshape(S, -1)
+        lorg = np.array(layer_origin, dtype=np.float64).reshape(S, 2)
+        org = np.array(origin, dtype=np.float64).reshape(S, 3)
+        cst = np.array(cost, dtype=np.uint8).reshape(S, -1)
+        status = np.zeros(S, np.int32)
+        fl = np.zeros(S, np.int32) if flags else None
+        a = abi.make_obstacle_layer_args(S, lay.shape[1], pts.shape[1], footprint, **params)
+        a.points, a.point_count, a.sensor_origin, a.robot = abi.ptr(pts), abi.ptr(cnt), abi.ptr(sen), abi.ptr(rob)
+        a.grid, a.layer, a.layer_origin, a.origin = abi.ptr(grd), abi.ptr(lay), abi.ptr(lorg), abi.ptr(org)
+        a.cost, a.status, a.flags = abi.ptr(cst), abi.ptr(status), abi.ptr(fl)
+        self._check(self.lib.tebgpu_costmap_obstacle_layer(self.ctx, C.byref(a)), "tebgpu_costmap_obstacle_layer")
+        return lay, lorg, cst, org, status, fl
+
+    def costmap_obstacle_layer_device(self, args, stream=None):
+        """tebgpu_costmap_obstacle_layer_device: the same step over DEVICE memory (args: an abi.TebObstacleLayerArgs of
+        device pointers, the footprint on the host; cost / grid / origin are the TebCostmapArgs arrays the costmap
+        conversion and the costmap check read next). Stream ordered on `stream` (a cudaStream_t handle; None: the
+        context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_costmap_obstacle_layer_device(self.ctx, C.byref(args), stream),
+                    "tebgpu_costmap_obstacle_layer_device")
+
+    def obstacle_layer_max_cell_cap(self):
+        """the largest cell_cap the obstacle layer takes: a robot's row in the opt-in shared memory of one CTA"""
+        return self.info(21)
 
     def local_plan(self, global_plan, plan_begin, plan_end, robot, robot_vel, grid, origin, P_cap, V_cap=None,
                    scene_id=None, via_count=None, infeasible_count=None, since_infeasible=None, costmap_to_plan=None,

@@ -281,6 +281,49 @@ def make_static_maps(grids, origins, unknown_cost_value=-1, lethal_threshold=100
     return m, arrays
 
 
+class TebObstacleLayerArgs(C.Structure):
+    """Every robot's obstacle layer (tebgpu_costmap_obstacle_layer): the parameters of the observation source and the
+    layer, the footprint (HOST pointer), the points, the layer grids carried between cycles and the master raster in
+    TebCostmapArgs' layout; host or device pointers (make_obstacle_layer_args)"""
+    _fields_ = [("S", _i), ("cell_cap", _i), ("P_cap", _i), ("F", _i), ("mode", _i), ("combination_method", _i),
+                ("track_unknown_space", _i), ("master_default", _i), ("clearing", _i), ("marking", _i),
+                ("obstacle_range", C.c_double), ("raytrace_range", C.c_double), ("min_obstacle_height", C.c_double),
+                ("max_obstacle_height", C.c_double), ("layer_max_obstacle_height", C.c_double),
+                ("footprint", C.c_void_p), ("points", C.c_void_p), ("point_count", C.c_void_p),
+                ("sensor_origin", C.c_void_p), ("robot", C.c_void_p), ("grid", C.c_void_p), ("layer", C.c_void_p),
+                ("layer_origin", C.c_void_p), ("origin", C.c_void_p), ("cost", C.c_void_p), ("status", C.c_void_p),
+                ("flags", C.c_void_p)]
+
+
+# TEB_OBSTACLE_LAYER_*: the modes, each robot's status and its flags after tebgpu_costmap_obstacle_layer
+TEB_OBSTACLE_LAYER_COMBINE, TEB_OBSTACLE_LAYER_STANDALONE = 0, 1
+TEB_OBSTACLE_LAYER_OK, TEB_OBSTACLE_LAYER_BAD_GRID, TEB_OBSTACLE_LAYER_BAD_POINTS, TEB_OBSTACLE_LAYER_ORIGIN_MISMATCH = 0, 1, 2, 3
+TEB_OBSTACLE_LAYER_SENSOR_OFF_MAP, TEB_OBSTACLE_LAYER_FOOTPRINT_OFF_MAP = 1, 2
+
+
+def make_obstacle_layer_args(S, cell_cap, P_cap, footprint=None, mode=TEB_OBSTACLE_LAYER_COMBINE, combination_method=1,
+                             track_unknown_space=True, master_default=255, clearing=True, marking=True,
+                             obstacle_range=2.5, raytrace_range=3.0, min_obstacle_height=0.0, max_obstacle_height=2.0,
+                             layer_max_obstacle_height=2.0, **arrays):
+    """A TebObstacleLayerArgs; the defaults are ObstacleLayer's and ObservationBuffer's (costmap_2d 1.17). footprint:
+    [F][2] in the robot frame, or None; kept on the struct as `footprint_array`. arrays: the pointer fields by name
+    (points, point_count, sensor_origin, robot, grid, layer, layer_origin, origin, cost, status, flags)."""
+    a = TebObstacleLayerArgs()
+    a.S, a.cell_cap, a.P_cap, a.mode, a.combination_method = S, cell_cap, P_cap, mode, combination_method
+    a.track_unknown_space, a.master_default = int(bool(track_unknown_space)), int(master_default)
+    a.clearing, a.marking = int(bool(clearing)), int(bool(marking))
+    a.obstacle_range, a.raytrace_range = obstacle_range, raytrace_range
+    a.min_obstacle_height, a.max_obstacle_height = min_obstacle_height, max_obstacle_height
+    a.layer_max_obstacle_height = layer_max_obstacle_height
+    fp = None if footprint is None else np.ascontiguousarray(footprint, dtype=np.float64).reshape(-1, 2)
+    a.F = 0 if fp is None else fp.shape[0]
+    a.footprint = ptr(fp)
+    a.footprint_array = fp
+    for k, v in arrays.items():
+        setattr(a, k, v)
+    return a
+
+
 class TebHsigFactors(C.Structure):
     """Every scene's factor table of the 2-D H-signature (tebgpu_hsig_factors): factor [S][M_cap][2] float64, the
     mantissa of Q_l = 1 / prod_j (o_l - o_j); factor_exp [S][M_cap] int32, its binary exponent (INT32_MIN for 0);

@@ -24,6 +24,7 @@
 #include "teb_feasible.cuh"
 #include "teb_costmap.cuh"
 #include "teb_costmap_window.cuh"
+#include "teb_costmap_obstacle_layer.cuh"
 #include "teb_local_plan.cuh"
 #include "teb_cycle.cuh"
 #include "teb_fleet.cuh"
@@ -138,6 +139,10 @@ struct tebgpu_ctx {
    * call that needs more */
   char* d_cwin = nullptr; size_t cwin_bytes = 0;
   long long last_window_grid = 0;     /* grid in CTAs of the last k_costmap_window launch */
+  /* obstacle layers: the largest row k_costmap_obstacle_layer stages in shared memory, and the host-buffer entry point's
+   * arrays staged in one buffer grown by the first call that needs more */
+  long long olayer_max_cap = 0;
+  char* d_olayer = nullptr; size_t olayer_bytes = 0;
   /* local plan: the host-buffer entry point's inputs and outputs, staged in one buffer grown by the first call that
    * needs more */
   char* d_lplan = nullptr; size_t lplan_bytes = 0;
@@ -267,6 +272,7 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 17: return (int32_t)sizeof(TebFleetShapes);
     case 18: return (int32_t)sizeof(TebStaticMaps);
     case 19: return (int32_t)sizeof(TebCostmapWindowArgs);
+    case 20: return (int32_t)sizeof(TebObstacleLayerArgs);
     default: return -1;
   }
 }
@@ -297,6 +303,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 18: return ctx->last_fleet_grid;
     case 19: return ctx->last_fleet_search;
     case 20: return ctx->last_window_grid;
+    case 21: return ctx->olayer_max_cap;
     default: return -1;
   }
 }
@@ -308,7 +315,8 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_plan, c->d_feas, c->d_qcount, c->d_queries, c->d_tbands, c->d_tpoints, c->d_tprof, c->d_ttraj,
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
                   c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
-                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid, c->d_fshape, c->d_cwin};
+                  c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid, c->d_fshape, c->d_cwin,
+                  c->d_olayer};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -527,6 +535,16 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
   CUDA_TRY(c, cudaFuncSetAttribute(k_lm_step_t<1, KB_BCR_THREADS, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   tebgpu_default_params(&c->params);
   c->have_params = true;
+  {
+    /* the obstacle layer stages a robot's row in the opt-in shared memory the kernel's own arrays leave */
+    int optin = 0;
+    cudaFuncAttributes fa{};
+    CUDA_TRY(c, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    CUDA_TRY(c, cudaFuncGetAttributes(&fa, k_costmap_obstacle_layer));
+    c->olayer_max_cap = ((long long)optin - (long long)fa.sharedSizeBytes) & ~15LL;
+    CUDA_TRY(c, cudaFuncSetAttribute(k_costmap_obstacle_layer, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)c->olayer_max_cap));
+  }
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   return TEBGPU_OK;
 }
@@ -1946,6 +1964,96 @@ int32_t tebgpu_costmap_window(tebgpu_ctx* ctx, const TebStaticMaps* m, const Teb
   CUDA_TRY(ctx, cudaMemcpyAsync(wa->cost, da.cost, cells, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(wa->origin, da.origin, S * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(wa->status, da.status, S * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* argument checks of both obstacle-layer entry points: nothing is launched when one fails */
+static int32_t check_obstacle_layer_args(tebgpu_ctx* ctx, const TebObstacleLayerArgs* a) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!a) { ctx->err = "obstacle layer args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->S < 1 || a->cell_cap < 1 || a->P_cap < 0) { ctx->err = "bad obstacle layer dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->S > ctx->lim.max_scenes) { ctx->err = "obstacle layer robots exceed the context's max_scenes"; return TEBGPU_ERR_CAPACITY; }
+  if (a->cell_cap > ctx->olayer_max_cap) { ctx->err = "cell_cap exceeds the shared memory of one CTA (tebgpu_get_info key 21)"; return TEBGPU_ERR_CAPACITY; }
+  if (a->F < 0 || a->F > TEB_COSTMAP_FOOTPRINT_MAX) { ctx->err = "F outside 0 .. TEB_COSTMAP_FOOTPRINT_MAX"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->F > 0 && !a->footprint) { ctx->err = "footprint == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  for (int k = 0; k < 2 * a->F; ++k)
+    if (!std::isfinite(a->footprint[k])) { ctx->err = "non-finite footprint point"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!(a->obstacle_range >= 0) || !(a->raytrace_range >= 0)) { ctx->err = "negative or NaN range"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->mode != TEB_OBSTACLE_LAYER_COMBINE && a->mode != TEB_OBSTACLE_LAYER_STANDALONE) { ctx->err = "unknown obstacle layer mode"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->master_default < 0 || a->master_default > 255) { ctx->err = "master_default outside 0 .. 255"; return TEBGPU_ERR_INVALID_ARG; }
+  if ((a->P_cap > 0 && !a->points) || !a->point_count || !a->sensor_origin || !a->robot || !a->grid || !a->layer ||
+      !a->layer_origin || !a->origin || !a->cost || !a->status) { ctx->err = "missing required obstacle layer array"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_costmap_obstacle_layer on arguments already checked: the footprint travels in the launch's parameter block */
+static int32_t issue_obstacle_layer(tebgpu_ctx* ctx, const TebObstacleLayerArgs* a, cudaStream_t st) {
+  ObstacleLayerDev d;
+  std::memset(&d, 0, sizeof(d));
+  d.a = *a;
+  d.a.footprint = nullptr;
+  if (a->F) std::memcpy(d.fp, a->footprint, (size_t)a->F * 2 * sizeof(double));
+  k_costmap_obstacle_layer<<<a->S, OL_THREADS, ((size_t)a->cell_cap + 15) & ~(size_t)15, st>>>(d);
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_costmap_obstacle_layer_device(tebgpu_ctx* ctx, const TebObstacleLayerArgs* a, void* cuda_stream) {
+  const int32_t rc = check_obstacle_layer_args(ctx, a);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_obstacle_layer(ctx, a, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_costmap_obstacle_layer(tebgpu_ctx* ctx, const TebObstacleLayerArgs* a) {
+  int32_t rc = check_obstacle_layer_args(ctx, a);
+  if (rc) return rc;
+  /* the robots the device entry point would mark bad are refused here, before anything runs */
+  for (int s = 0; s < a->S; ++s) {
+    double nox, noy, cx, cy;
+    const int st = obstacle_layer_status(*a, s, &nox, &noy, &cx, &cy);
+    if (st == TEB_OBSTACLE_LAYER_BAD_GRID) { ctx->err = "grid[s] outside 1 .. cell_cap cells, a bad resolution, or a non-finite layer_origin or robot x / y"; return TEBGPU_ERR_INVALID_ARG; }
+    if (st == TEB_OBSTACLE_LAYER_BAD_POINTS) { ctx->err = "point_count[s] outside 0 .. P_cap"; return TEBGPU_ERR_INVALID_ARG; }
+    if (st != TEB_OBSTACLE_LAYER_OK) { ctx->err = "the snapped layer origin differs from origin[s]"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t S = a->S, cells = S * (size_t)a->cell_cap, pts = S * (size_t)a->P_cap * 3 * sizeof(float);
+  /* one staging buffer: every array at a 256-byte aligned offset, so the rows keep their alignment mod 16 */
+  size_t off = 0;
+  auto slot = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_pts = slot(pts), o_count = slot(S * 4), o_sensor = slot(S * 3 * sizeof(double)),
+               o_robot = slot(S * 3 * sizeof(double)), o_grid = slot(S * 2 * 4), o_layer = slot(cells),
+               o_lorg = slot(S * 2 * sizeof(double)), o_origin = slot(S * 3 * sizeof(double)), o_cost = slot(cells),
+               o_status = slot(S * 4), o_flags = slot(S * 4);
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_olayer, &ctx->olayer_bytes, off, st))) return rc;
+  char* d = ctx->d_olayer;
+  auto up = [&](size_t o, const void* src, size_t bytes) -> int32_t {
+    if (src && bytes) CUDA_TRY(ctx, cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, st));
+    return TEBGPU_OK;
+  };
+  if ((rc = up(o_pts, a->points, pts)) || (rc = up(o_count, a->point_count, S * 4)) ||
+      (rc = up(o_sensor, a->sensor_origin, S * 3 * sizeof(double))) || (rc = up(o_robot, a->robot, S * 3 * sizeof(double))) ||
+      (rc = up(o_grid, a->grid, S * 2 * 4)) || (rc = up(o_layer, a->layer, cells)) ||
+      (rc = up(o_lorg, a->layer_origin, S * 2 * sizeof(double))) || (rc = up(o_origin, a->origin, S * 3 * sizeof(double))) ||
+      (rc = up(o_cost, a->cost, cells)))
+    return rc;
+  TebObstacleLayerArgs da = *a;
+  da.points = pts ? (const float*)(d + o_pts) : nullptr;
+  da.point_count = (const int32_t*)(d + o_count); da.sensor_origin = (const double*)(d + o_sensor);
+  da.robot = (const double*)(d + o_robot); da.grid = (const int32_t*)(d + o_grid);
+  da.layer = (uint8_t*)(d + o_layer); da.layer_origin = (double*)(d + o_lorg); da.origin = (double*)(d + o_origin);
+  da.cost = (uint8_t*)(d + o_cost); da.status = (int32_t*)(d + o_status);
+  da.flags = a->flags ? (int32_t*)(d + o_flags) : nullptr;
+  if ((rc = issue_obstacle_layer(ctx, &da, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->layer, da.layer, cells, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->layer_origin, da.layer_origin, S * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->origin, da.origin, S * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->cost, da.cost, cells, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->status, da.status, S * 4, cudaMemcpyDeviceToHost, st));
+  if (a->flags) CUDA_TRY(ctx, cudaMemcpyAsync(a->flags, da.flags, S * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaStreamSynchronize(st));
   return TEBGPU_OK;
 }

@@ -39,12 +39,17 @@ TEB_HD inline int costmap_window_status(const TebStaticMaps& m, const TebCostmap
   return TEB_COSTMAP_WINDOW_OK;
 }
 
-/* updateOrigin along one axis: o the previous origin, p the robot's coordinate, n the window's cells */
-TEB_HD inline double costmap_window_snap(double o, double p, int n, double r) {
+/* updateOrigin's whole-cell move along one axis (a double: NaN or past the int range where the origin is): o the previous
+ * origin, p the robot's coordinate, n the window's cells */
+TEB_HD inline double costmap_window_cells(double o, double p, int n, double r) {
   const double size_m = teb_mul(teb_add((double)(n - 1), 0.5), r); /* getSizeInMetersX */
   const double target = teb_add(p, -(size_m / 2));
-  const double cells = trunc(teb_add(target, -o) / r);
-  return teb_add(o, teb_mul(cells, r));
+  return trunc(teb_add(target, -o) / r);
+}
+
+/* updateOrigin along one axis: the new origin */
+TEB_HD inline double costmap_window_snap(double o, double p, int n, double r) {
+  return teb_add(o, teb_mul(costmap_window_cells(o, p, n, r), r));
 }
 
 /* StaticLayer::interpretValue of the byte v */
