@@ -709,6 +709,130 @@ typedef struct TebObstacleLayerArgs {
 #define TEB_OBSTACLE_LAYER_SENSOR_OFF_MAP   1   /* flag: the sensor origin is off the layer, no clearing */
 #define TEB_OBSTACLE_LAYER_FOOTPRINT_OFF_MAP 2  /* flag: a placed footprint vertex is off the layer, no footprint clearing */
 
+/* One observation source of the voxel layer (costmap_2d's observation_sources entry and its ObservationBuffer). */
+typedef struct TebObservationSource {
+  int32_t clearing, marking;                        /* the source's flags */
+  double obstacle_range, raytrace_range;            /* >= 0 */
+  double min_obstacle_height, max_obstacle_height;  /* the source's height filter */
+} TebObservationSource;
+
+/* Every robot's voxel layer, marked and cleared in 3-D from up to TEB_VOXEL_LAYER_MAX_SOURCES observation sources per
+ * call (tebgpu_costmap_voxel_layer): what costmap_2d's VoxelLayer adds to a local costmap. The layer keeps a column of
+ * z_voxels voxels per cell; a ray clears only the voxels it passes through, so an overhang seen in an earlier cycle (a
+ * table top) stays lethal while rays pass under it, where the 2-D obstacle layer would clear the cell. The caller owns
+ * each robot's voxel row (voxels), 2-D layer row (layer) and layer_origin, kept between cycles; a fresh robot starts
+ * at resetMaps: every column 0x0000FFFF, every layer byte d. The result is written into the master raster in
+ * TebCostmapArgs' layout exactly as TebObstacleLayerArgs writes it, after tebgpu_costmap_window, after
+ * tebgpu_costmap_obstacle_layer, or alone (mode TEB_VOXEL_LAYER_COMBINE / _STANDALONE, as there).
+ *
+ * costmap_2d is not part of the reference checkout; this restates ROS Noetic navigation (costmap_2d 1.17 and
+ * voxel_grid): VoxelLayer::updateBounds / raytraceFreespace / updateOrigin / resetMaps / worldToMap3D /
+ * worldToMap3DFloat / reconfigureCB, VoxelGrid::reset / markVoxelInMap / clearVoxelLineInMap / raytraceLine /
+ * bresenham3D with ClearVoxelInMap, GridOffset and ZOffset, VoxelGrid::bitsBelowThreshold, and from the obstacle layer
+ * the height filter, footprint clearing and updateWithOverwrite / updateWithMax (TebObstacleLayerArgs steps 2, 5, 6).
+ * Every product and sum is rounded on its own (no FMA contraction); min(a, b) = b < a ? b : a and max(a, b) = a < b ?
+ * b : a are std::min / std::max with costmap_2d's argument order, which decides the NaN cases. Robot s, with (sx, sy) =
+ * grid[s], r = origin[s][2], Z = z_voxels, d = 255 with track_unknown_space, else 0:
+ *   Column word. One uint32_t per cell: voxel z (0 .. Z - 1) is marked when bits z and z + 16 are set, free when both
+ *      are clear, unknown when only bit z is set; marked(col) = col >> 16, unknown(col) = (uint16)(col >> 16) ^
+ *      (uint16)col, and bits(n) is the number of set bits (bitsBelowThreshold(n, t) is bits(n) <= t). Reset writes
+ *      0x0000FFFF, so the 16 - Z bits above Z count as unknown for ever. reconfigureCB sets the layer's threshold to
+ *      U = unknown_threshold + (16 - Z): the unused bits are added back, and a fully cleared column (16 - Z unknown bits)
+ *      is FREE for every unknown_threshold >= 0. (Read without that offset, the defaults Z = 10, unknown_threshold 15 also
+ *      give FREE, but unknown_threshold 5 would give NO_INFORMATION; this step follows reconfigureCB.)
+ *   1. Origin and shift (updateOrigin, resetMaps): as TebObstacleLayerArgs step 1, the voxel row and the layer row
+ *      moved together by the same whole cells (costmap_window_cells); a cell shifted in gets 0x0000FFFF and d. The same
+ *      status rules and combine / standalone origin handling.
+ *   2. Height filter per source k (bufferCloud): a point of source k is kept when sources[k].min_obstacle_height <= z <=
+ *      sources[k].max_obstacle_height; it applies to the source's clearing and marking alike.
+ *   3. Clearing, for every source with clearing != 0 before any marking (updateBounds raytraces every clearing
+ *      observation first), raytraceFreespace with (so_x, so_y, so_z) = sensor_origin[s][k] and H = max_obstacle_height:
+ *      worldToMap3DFloat of the sensor gives (x0, y0, z0); when it fails there is no clearing from source k (flag
+ *      TEB_VOXEL_LAYER_SENSOR_OFF_MAP(k); also set when no point is kept, where costmap_2d returns before the test).
+ *      Each kept point (px, py, pz) as doubles: dist = sqrt(((px - so_x)^2 + (py - so_y)^2) + (pz - so_z)^2), f =
+ *      max(min(1, (dist - 2 r) / dist), 0) (the scaling_fact pull-back: f is 1 for a NaN quotient, 0 at dist 0); w =
+ *      f (p - so) + so per axis; a, b, c = w - so; t = 1; then t = max(0, min(t, ((H - 0.01) - so_z) / c)) when wz > H,
+ *      else t = min(t, (origin_z - so_z) / c) when wz < origin_z; then t = min(t, (ox' - so_x) / a) when wx < ox', min(t,
+ *      (oy' - so_y) / b) when wy < oy', min(t, (ex - so_x) / a) when wx > ex = ox' + ((sx - 1) + 0.5) r (getSizeInMetersX,
+ *      not the obstacle layer's sx r), min(t, (ey - so_y) / b) when wy > ey, each test on the pulled-back w; the end is
+ *      so + (a, b, c) t. A point whose worldToMap3DFloat fails is skipped (clearVoxelLineInMap's own endpoint test can
+ *      then never fail: it is the same comparison negated). Otherwise raytraceLine from (x0, y0, z0) to (x1, y1, z1),
+ *      with max_length = cellDistance(raytrace_range) as in the obstacle layer: integer deltas dx = (int)x1 - (int)x0
+ *      and likewise dy, dz; dist3 = sqrt(((x0 - x1)^2 + (y0 - y1)^2) + (z0 - z1)^2) of the float map coordinates; scale =
+ *      min(1, max_length / dist3) (1 for the NaN of 0 / 0 and for the inf of n / 0); the dominant axis is x when |dx| >=
+ *      max(|dy|, |dz|), else y when |dy| >= |dz|, else z; bresenham3D runs (unsigned)(scale |da|) steps, both minor
+ *      errors starting at |da| / 2, the offsets moving by sign() (sign(0) is -1) and the z mask (0x10001 << (int)z0)
+ *      shifting up or down (ZOffset), and visits the voxel it ends on. Every visit (ClearVoxelInMap) clears the voxel's
+ *      two bits, then, when bits(marked) <= mark_threshold, writes FREE_SPACE (0) to the layer cell if bits(unknown) <= U,
+ *      else NO_INFORMATION (255); when bits(marked) > mark_threshold it leaves the cell.
+ *   4. Marking, for every source with marking != 0, after all clearing: a kept point is skipped when pz > H, when ((px -
+ *      so_x)^2 + (py - so_y)^2) + (pz - so_z)^2 >= obstacle_range^2, or when worldToMap3D fails, with pz < origin_z placed
+ *      at origin_z (voxel 0); otherwise markVoxelInMap sets the voxel's two bits, and the layer cell becomes
+ *      LETHAL_OBSTACLE (254) when bits(marked) > mark_threshold.
+ *   5. Footprint clearing, when F >= 3: TebObstacleLayerArgs step 5 on the layer row only; the voxels keep their marks
+ *      (flag TEB_VOXEL_LAYER_FOOTPRINT_OFF_MAP when a vertex is off the map).
+ *   6. Combination: TebObstacleLayerArgs step 6, the same modes, methods and bytes past sx * sy (voxels past it: 0x0000FFFF).
+ * worldToMap3D(Float): off the map when wx < ox', wy < oy' or wz < origin_z; otherwise qx = (wx - ox') / r, qy likewise,
+ * qz = (wz - origin_z) / z_resolution, on the map when qx < sx, qy < sy and qz < Z (a NaN quotient is off the map);
+ * worldToMap3D takes (int) of each.
+ *
+ * Why the device may run every ray and every mark in parallel and still give these bytes: within step 3 a visit only
+ * removes bits from a column, so the last visit to a column, in any order, sees the column's final state; a visit whose
+ * state has bits(marked) > mark_threshold leaves the cell, and every earlier state had at least as many marked bits. So
+ * after step 3 a layer cell that some ray visited is FREE or NO_INFORMATION by the final column when bits(marked) <=
+ * mark_threshold, else what step 1 left; a cell no ray visited keeps what step 1 left. Step 4 only adds bits, so the
+ * last mark of a column sees its final state, and a marked cell becomes 254 exactly when its final column has
+ * bits(marked) > mark_threshold. Only the phase boundaries (shift, clear, mark, footprint, combine) are ordered.
+ *
+ * Where this and costmap_2d part ways, beyond TebObstacleLayerArgs' whole-window combination and device sin / cos:
+ * Z outside 1 .. 16 is an argument error (VoxelGrid clamps to 16 while the layer keeps its own size_z_);
+ * observation_persistence, expected_update_rate, inf_is_valid and the published voxel map are not built; the marking
+ * and clearing of one source read the same kept points (one observation per source per call).
+ *
+ * Bad robots as TebObstacleLayerArgs (TEB_VOXEL_LAYER_BAD_GRID, _BAD_POINTS for any source's point_count outside 0 ..
+ * P_cap, _ORIGIN_MISMATCH): they keep voxels, layer and layer_origin, their master row untouched (combine) or all
+ * master_default (standalone) and their origin (the device entry point); the host entry point refuses them. */
+#define TEB_VOXEL_LAYER_MAX_SOURCES 4
+typedef struct TebVoxelLayerArgs {
+  int32_t S;                     /* robots, 1 .. max_scenes */
+  int32_t cell_cap;              /* cells per robot (stride of voxels, layer and cost), 1 .. tebgpu_get_info key 22 */
+  int32_t P_cap;                 /* points per source and robot (stride of points), >= 0 */
+  int32_t K;                     /* observation sources, 1 .. TEB_VOXEL_LAYER_MAX_SOURCES */
+  int32_t F;                     /* footprint points, 0 .. TEB_COSTMAP_FOOTPRINT_MAX; F < 3: no footprint clearing */
+  int32_t mode;                  /* TEB_VOXEL_LAYER_COMBINE or _STANDALONE */
+  int32_t combination_method;    /* 0 overwrite, 1 maximum, anything else: not combined */
+  int32_t track_unknown_space;   /* the layer's (its default 255, else 0) */
+  int32_t master_default;        /* standalone: the byte the master row is reset to, 0 .. 255 */
+  int32_t z_voxels;              /* Z, 1 .. 16 (default 10) */
+  int32_t unknown_threshold;     /* the parameter, 0 .. 16 (default 15); the layer compares with it + (16 - Z) */
+  int32_t mark_threshold;        /* 0 .. 16 (default 0) */
+  double origin_z, z_resolution; /* finite; z_resolution > 0 (defaults 0, 0.2) */
+  double max_obstacle_height;    /* the layer's (default 2) */
+  const TebObservationSource* sources; /* [K] HOST (both entry points) */
+  const double*  footprint;      /* [F][2] HOST (both entry points), finite: the footprint in the robot frame */
+  const float*   points;         /* [S][K][P_cap][3] x, y, z in the costmap's global frame (NULL when P_cap is 0) */
+  const int32_t* point_count;    /* [S][K] */
+  const double*  sensor_origin;  /* [S][K][3] x, y, z of each source's origin in the global frame */
+  const double*  robot;          /* [S][3] x, y, yaw of the robot in the global frame */
+  const int32_t* grid;           /* [S][2] sx, sy (TebCostmapArgs.grid) */
+  uint32_t*      voxels;         /* [S][cell_cap] in/out: the column words */
+  uint8_t*       layer;          /* [S][cell_cap] in/out: the layer's 2-D grid */
+  double*        layer_origin;   /* [S][2] in/out: the origin both were last written at */
+  double*        origin;         /* [S][3] TebCostmapArgs.origin: read (combine), ox, oy written (standalone); r read */
+  uint8_t*       cost;           /* [S][cell_cap] in/out: the master raster (TebCostmapArgs.cost) */
+  int32_t*       status;         /* [S] out: TEB_VOXEL_LAYER_* */
+  int32_t*       flags;          /* [S] out or NULL: TEB_VOXEL_LAYER_SENSOR_OFF_MAP(k) | _FOOTPRINT_OFF_MAP */
+} TebVoxelLayerArgs;
+#define TEB_VOXEL_LAYER_COMBINE          0
+#define TEB_VOXEL_LAYER_STANDALONE       1
+#define TEB_VOXEL_LAYER_OK               0
+#define TEB_VOXEL_LAYER_BAD_GRID         1   /* sizes, cell_cap, resolution, non-finite layer_origin or robot x / y */
+#define TEB_VOXEL_LAYER_BAD_POINTS       2   /* a point_count outside 0 .. P_cap */
+#define TEB_VOXEL_LAYER_ORIGIN_MISMATCH  3   /* combine: the snapped layer origin is not the master's */
+#define TEB_VOXEL_LAYER_SENSOR_OFF_MAP(k) (1 << (k))  /* flag: source k's origin is off the grid, no clearing from it */
+#define TEB_VOXEL_LAYER_FOOTPRINT_OFF_MAP 16          /* flag: a placed footprint vertex is off the map */
+#define TEB_VOXEL_LAYER_UNKNOWN_COLUMN   0x0000FFFFu  /* VoxelGrid::reset's column */
+
 /* The controller state of every robot between cycles, and the two steps of TebLocalPlannerROS::computeVelocityCommands
  * around plan() that read and write it: tebgpu_backup_modes, the oscillation half of configureBackupModes
  * (teb_local_planner_ros.cpp:980-1016, with FailureDetector of recovery_behaviors.cpp), after tebgpu_local_plan and
@@ -816,7 +940,7 @@ typedef struct TebCycleArgs {
  * 3 TebOptimizeArgs, 4 TebGpuLimits, 5 TebPlanInput, 6 TebFeasibilityArgs, 7 TebTrajectoryArgs, 8 TebCostmapArgs,
  * 9 TebLocalPlanArgs, 10 TebCycleArgs, 11 TebCostmapWorld, 12 TebFrameArgs, 13 TebHsigFactors, 14 TebFleetArgs,
  * 15 TebFleetRow, 16 TebFleetTable, 17 TebFleetShapes, 18 TebStaticMaps, 19 TebCostmapWindowArgs,
- * 20 TebObstacleLayerArgs. */
+ * 20 TebObstacleLayerArgs, 21 TebVoxelLayerArgs, 22 TebObservationSource. */
 int32_t tebgpu_sizeof(int32_t which);
 
 /* Context life cycle. One context = one device + one stream + its device workspaces.
@@ -988,6 +1112,23 @@ int32_t tebgpu_costmap_window_device(tebgpu_ctx* ctx, const TebStaticMaps* maps,
  * DEVICE buffers (footprint on the host), stream ordered as tebgpu_optimize_batch_device, does not synchronise. */
 int32_t tebgpu_costmap_obstacle_layer(tebgpu_ctx* ctx, const TebObstacleLayerArgs* args);
 int32_t tebgpu_costmap_obstacle_layer_device(tebgpu_ctx* ctx, const TebObstacleLayerArgs* args, void* cuda_stream);
+
+/* Every robot's voxel layer, as defined at TebVoxelLayerArgs: (window, obstacle layer,) voxel layer, then convert, plan
+ * and check on the same stream. One launch, one CTA of 256 threads per robot with the robot's voxel row, layer row and a
+ * visited bitmap staged in dynamic shared memory: the shifted rows (16-byte loads), every clearing ray walked by one
+ * thread with shared-memory atomicAnd on the columns, one pass writing the visited cells' bytes, the marks with
+ * atomicOr, the footprint's column spans by one warp, then both rows stored in place and the master row combined in
+ * 16-byte stores. cell_cap is bounded by the opt-in shared memory of one CTA (tebgpu_get_info key 22): past it
+ * TEBGPU_ERR_CAPACITY. Argument errors (NULL args, sources or required arrays, S outside 1 .. max_scenes, cell_cap < 1,
+ * P_cap < 0, K outside 1 .. TEB_VOXEL_LAYER_MAX_SOURCES, F outside 0 .. TEB_COSTMAP_FOOTPRINT_MAX, a non-finite
+ * footprint point, a negative or NaN range, mode not COMBINE / STANDALONE, master_default outside 0 .. 255, z_voxels
+ * outside 1 .. 16, a threshold outside 0 .. 16, a non-finite origin_z, a z_resolution not positive and finite, voxels not
+ * 4-byte aligned) return TEBGPU_ERR_INVALID_ARG (TEBGPU_ERR_CAPACITY past a limit) before anything is launched.
+ * tebgpu_costmap_voxel_layer: HOST buffers, synchronous; robots the device entry point would mark with a status other
+ * than TEB_VOXEL_LAYER_OK are refused with TEBGPU_ERR_INVALID_ARG. tebgpu_costmap_voxel_layer_device: DEVICE buffers
+ * (sources and footprint on the host), stream ordered as tebgpu_optimize_batch_device, does not synchronise. */
+int32_t tebgpu_costmap_voxel_layer(tebgpu_ctx* ctx, const TebVoxelLayerArgs* args);
+int32_t tebgpu_costmap_voxel_layer_device(tebgpu_ctx* ctx, const TebVoxelLayerArgs* args, void* cuda_stream);
 
 /* The two controller steps around plan(), as defined at TebCycleArgs. One thread per band, so that the detector's sums
  * run in the reference's order (tebgpu_get_info key 17). A fleet cycle on one stream: tebgpu_costmap_obstacles_device,
@@ -1393,7 +1534,9 @@ int64_t tebgpu_last_launch_count(const tebgpu_ctx* ctx);
  * first), 18 grid in CTAs of the last fleet-obstacle launch (k_fleet_obstacles or k_fleet_obstacles_grid, FLEET_WARPS
  * robots per CTA; 0 before the first), 19 the search that launch ran (TEBGPU_FLEET_SEARCH_ALL_PAIRS, _GRID or
  * _ONE_BUCKET; -1 before the first), 20 grid in CTAs of the last costmap window raster launch, 21 the largest cell_cap
- * tebgpu_costmap_obstacle_layer takes (bytes of a robot's row in the opt-in shared memory of one CTA).
+ * tebgpu_costmap_obstacle_layer takes (bytes of a robot's row in the opt-in shared memory of one CTA), 22 the largest
+ * cell_cap tebgpu_costmap_voxel_layer takes (cells of a robot's voxel row, layer row and visited bits in the opt-in
+ * shared memory of one CTA, a multiple of 32).
  * Returns -1 for an unknown key. */
 #define TEBGPU_EVAL_BUILD_V1 0          /* k_trial_eval, first generation (TEBGPU_EVAL_V1=1): B CTAs */
 #define TEBGPU_EVAL_BUILD_EVAL2_WIDE 1  /* k_trial_eval2, up to 16 warps per band (2 B <= SMs): B CTAs */

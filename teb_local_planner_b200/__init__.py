@@ -84,6 +84,10 @@ def load_library(build_if_missing=False):
     L.tebgpu_costmap_obstacle_layer.argtypes = [vp, C.POINTER(abi.TebObstacleLayerArgs)]
     L.tebgpu_costmap_obstacle_layer_device.restype = C.c_int32
     L.tebgpu_costmap_obstacle_layer_device.argtypes = [vp, C.POINTER(abi.TebObstacleLayerArgs), vp]
+    L.tebgpu_costmap_voxel_layer.restype = C.c_int32
+    L.tebgpu_costmap_voxel_layer.argtypes = [vp, C.POINTER(abi.TebVoxelLayerArgs)]
+    L.tebgpu_costmap_voxel_layer_device.restype = C.c_int32
+    L.tebgpu_costmap_voxel_layer_device.argtypes = [vp, C.POINTER(abi.TebVoxelLayerArgs), vp]
     L.tebgpu_local_plan_tf.restype = C.c_int32
     L.tebgpu_local_plan_tf.argtypes = [vp, C.POINTER(abi.TebBatch), C.POINTER(abi.TebLocalPlanArgs),
                                        C.POINTER(abi.TebFrameArgs)]
@@ -189,7 +193,9 @@ def load_library(build_if_missing=False):
                                 abi.TebHsigFactors, abi.TebFleetArgs))) + ((15, None), (16, abi.TebFleetTable),
                                                                 (17, abi.TebFleetShapes), (18, abi.TebStaticMaps),
                                                                 (19, abi.TebCostmapWindowArgs),
-                                                                (20, abi.TebObstacleLayerArgs)):
+                                                                (20, abi.TebObstacleLayerArgs),
+                                                                (21, abi.TebVoxelLayerArgs),
+                                                                (22, abi.TebObservationSource)):
         if st is None:
             if L.tebgpu_sizeof(which) != abi.FLEET_ROW_DTYPE.itemsize:
                 raise RuntimeError(f"ABI mismatch for TebFleetRow: C {L.tebgpu_sizeof(which)} vs FLEET_ROW_DTYPE "
@@ -516,6 +522,51 @@ class TebGpu:
     def obstacle_layer_max_cell_cap(self):
         """the largest cell_cap the obstacle layer takes: a robot's row in the opt-in shared memory of one CTA"""
         return self.info(21)
+
+    def costmap_voxel_layer(self, points, point_count, sensor_origin, robot, grid, voxels, layer, layer_origin, origin,
+                            cost, sources, footprint=None, flags=True, **params):
+        """Every robot's voxel layer marked and cleared in 3-D from its sources' points (tebgpu_costmap_voxel_layer),
+        host buffers, as include/teb_b200.h defines it at TebVoxelLayerArgs: points [S][K][P_cap][3] float32,
+        point_count [S][K], sensor_origin [S][K][3], robot [S][3] (x, y, yaw), grid [S][2], voxels [S][cell_cap]
+        uint32, layer [S][cell_cap] uint8 and layer_origin [S][2] (the previous cycle's), origin [S][3] and cost
+        [S][cell_cap] (the master raster), sources: K TebObservationSource or dicts, footprint [F][2] or None; params:
+        the other keywords of abi.make_voxel_layer_args. Returns (voxels, layer, layer_origin, cost, origin, status,
+        flags) as new arrays (flags None when flags is False); the arguments are not modified."""
+        import numpy as np
+        K = len(sources)
+        pts = np.ascontiguousarray(points, dtype=np.float32)
+        S = pts.shape[0]
+        pts = pts.reshape(S, K, -1, 3)
+        cnt = np.ascontiguousarray(point_count, dtype=np.int32).reshape(S, K)
+        sen = np.ascontiguousarray(sensor_origin, dtype=np.float64).reshape(S, K, 3)
+        rob = np.ascontiguousarray(robot, dtype=np.float64).reshape(S, 3)
+        grd = np.ascontiguousarray(grid, dtype=np.int32).reshape(S, 2)
+        vox = np.array(voxels, dtype=np.uint32).reshape(S, -1)
+        lay = np.array(layer, dtype=np.uint8).reshape(S, -1)
+        lorg = np.array(layer_origin, dtype=np.float64).reshape(S, 2)
+        org = np.array(origin, dtype=np.float64).reshape(S, 3)
+        cst = np.array(cost, dtype=np.uint8).reshape(S, -1)
+        status = np.zeros(S, np.int32)
+        fl = np.zeros(S, np.int32) if flags else None
+        a = abi.make_voxel_layer_args(S, lay.shape[1], pts.shape[2], sources, footprint, **params)
+        a.points, a.point_count, a.sensor_origin, a.robot = abi.ptr(pts), abi.ptr(cnt), abi.ptr(sen), abi.ptr(rob)
+        a.grid, a.voxels, a.layer, a.layer_origin = abi.ptr(grd), abi.ptr(vox), abi.ptr(lay), abi.ptr(lorg)
+        a.origin, a.cost, a.status, a.flags = abi.ptr(org), abi.ptr(cst), abi.ptr(status), abi.ptr(fl)
+        self._check(self.lib.tebgpu_costmap_voxel_layer(self.ctx, C.byref(a)), "tebgpu_costmap_voxel_layer")
+        return vox, lay, lorg, cst, org, status, fl
+
+    def costmap_voxel_layer_device(self, args, stream=None):
+        """tebgpu_costmap_voxel_layer_device: the same step over DEVICE memory (args: an abi.TebVoxelLayerArgs of device
+        pointers, the sources and the footprint on the host; cost / grid / origin are the TebCostmapArgs arrays the
+        costmap conversion and the costmap check read next). Stream ordered on `stream` (a cudaStream_t handle; None:
+        the context's stream); does not synchronise."""
+        self._check(self.lib.tebgpu_costmap_voxel_layer_device(self.ctx, C.byref(args), stream),
+                    "tebgpu_costmap_voxel_layer_device")
+
+    def voxel_layer_max_cell_cap(self):
+        """the largest cell_cap the voxel layer takes: a robot's voxel row, layer row and visited bits in the opt-in
+        shared memory of one CTA"""
+        return self.info(22)
 
     def local_plan(self, global_plan, plan_begin, plan_end, robot, robot_vel, grid, origin, P_cap, V_cap=None,
                    scene_id=None, via_count=None, infeasible_count=None, since_infeasible=None, costmap_to_plan=None,

@@ -324,6 +324,72 @@ def make_obstacle_layer_args(S, cell_cap, P_cap, footprint=None, mode=TEB_OBSTAC
     return a
 
 
+class TebObservationSource(C.Structure):
+    """One observation source of the voxel layer: its clearing / marking flags, ranges and height filter"""
+    _fields_ = [("clearing", _i), ("marking", _i), ("obstacle_range", C.c_double), ("raytrace_range", C.c_double),
+                ("min_obstacle_height", C.c_double), ("max_obstacle_height", C.c_double)]
+
+
+class TebVoxelLayerArgs(C.Structure):
+    """Every robot's voxel layer (tebgpu_costmap_voxel_layer): the layer's parameters, the sources and the footprint
+    (HOST pointers), the points of every source, the voxel and layer rows carried between cycles and the master raster
+    in TebCostmapArgs' layout; host or device pointers (make_voxel_layer_args)"""
+    _fields_ = [("S", _i), ("cell_cap", _i), ("P_cap", _i), ("K", _i), ("F", _i), ("mode", _i),
+                ("combination_method", _i), ("track_unknown_space", _i), ("master_default", _i), ("z_voxels", _i),
+                ("unknown_threshold", _i), ("mark_threshold", _i), ("origin_z", C.c_double),
+                ("z_resolution", C.c_double), ("max_obstacle_height", C.c_double), ("sources", C.c_void_p),
+                ("footprint", C.c_void_p), ("points", C.c_void_p), ("point_count", C.c_void_p),
+                ("sensor_origin", C.c_void_p), ("robot", C.c_void_p), ("grid", C.c_void_p), ("voxels", C.c_void_p),
+                ("layer", C.c_void_p), ("layer_origin", C.c_void_p), ("origin", C.c_void_p), ("cost", C.c_void_p),
+                ("status", C.c_void_p), ("flags", C.c_void_p)]
+
+
+# TEB_VOXEL_LAYER_*: the modes, each robot's status and its flags after tebgpu_costmap_voxel_layer
+TEB_VOXEL_LAYER_MAX_SOURCES = 4
+TEB_VOXEL_LAYER_COMBINE, TEB_VOXEL_LAYER_STANDALONE = 0, 1
+TEB_VOXEL_LAYER_OK, TEB_VOXEL_LAYER_BAD_GRID, TEB_VOXEL_LAYER_BAD_POINTS, TEB_VOXEL_LAYER_ORIGIN_MISMATCH = 0, 1, 2, 3
+TEB_VOXEL_LAYER_FOOTPRINT_OFF_MAP = 16
+TEB_VOXEL_LAYER_UNKNOWN_COLUMN = 0x0000FFFF
+
+
+def TEB_VOXEL_LAYER_SENSOR_OFF_MAP(k):
+    return 1 << k
+
+
+def make_observation_source(clearing=True, marking=True, obstacle_range=2.5, raytrace_range=3.0,
+                            min_obstacle_height=0.0, max_obstacle_height=2.0):
+    """A TebObservationSource; the defaults are ObservationBuffer's (costmap_2d 1.17)"""
+    return TebObservationSource(int(bool(clearing)), int(bool(marking)), obstacle_range, raytrace_range,
+                                min_obstacle_height, max_obstacle_height)
+
+
+def make_voxel_layer_args(S, cell_cap, P_cap, sources, footprint=None, mode=TEB_VOXEL_LAYER_COMBINE,
+                          combination_method=1, track_unknown_space=True, master_default=255, z_voxels=10,
+                          unknown_threshold=15, mark_threshold=0, origin_z=0.0, z_resolution=0.2,
+                          max_obstacle_height=2.0, **arrays):
+    """A TebVoxelLayerArgs; the defaults are VoxelLayer's (costmap_2d 1.17). sources: a list of 1 ..
+    TEB_VOXEL_LAYER_MAX_SOURCES TebObservationSource or dicts of make_observation_source's keywords, kept on the struct
+    as `sources_array`; footprint: [F][2] in the robot frame, or None, kept as `footprint_array`. arrays: the pointer
+    fields by name (points, point_count, sensor_origin, robot, grid, voxels, layer, layer_origin, origin, cost, status,
+    flags)."""
+    a = TebVoxelLayerArgs()
+    src = [v if isinstance(v, TebObservationSource) else make_observation_source(**v) for v in sources]
+    a.S, a.cell_cap, a.P_cap, a.K, a.mode, a.combination_method = S, cell_cap, P_cap, len(src), mode, combination_method
+    a.track_unknown_space, a.master_default = int(bool(track_unknown_space)), int(master_default)
+    a.z_voxels, a.unknown_threshold, a.mark_threshold = z_voxels, unknown_threshold, mark_threshold
+    a.origin_z, a.z_resolution, a.max_obstacle_height = origin_z, z_resolution, max_obstacle_height
+    arr = (TebObservationSource * max(len(src), 1))(*src)
+    a.sources = C.cast(arr, C.c_void_p).value if src else None
+    a.sources_array = arr
+    fp = None if footprint is None else np.ascontiguousarray(footprint, dtype=np.float64).reshape(-1, 2)
+    a.F = 0 if fp is None else fp.shape[0]
+    a.footprint = ptr(fp)
+    a.footprint_array = fp
+    for k, v in arrays.items():
+        setattr(a, k, v)
+    return a
+
+
 class TebHsigFactors(C.Structure):
     """Every scene's factor table of the 2-D H-signature (tebgpu_hsig_factors): factor [S][M_cap][2] float64, the
     mantissa of Q_l = 1 / prod_j (o_l - o_j); factor_exp [S][M_cap] int32, its binary exponent (INT32_MIN for 0);

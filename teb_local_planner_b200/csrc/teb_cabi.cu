@@ -25,6 +25,7 @@
 #include "teb_costmap.cuh"
 #include "teb_costmap_window.cuh"
 #include "teb_costmap_obstacle_layer.cuh"
+#include "teb_costmap_voxel_layer.cuh"
 #include "teb_local_plan.cuh"
 #include "teb_cycle.cuh"
 #include "teb_fleet.cuh"
@@ -143,6 +144,10 @@ struct tebgpu_ctx {
    * arrays staged in one buffer grown by the first call that needs more */
   long long olayer_max_cap = 0;
   char* d_olayer = nullptr; size_t olayer_bytes = 0;
+  /* voxel layers: the largest row k_costmap_voxel_layer stages in shared memory (cells), and the host-buffer entry
+   * point's staging buffer */
+  long long vlayer_max_cap = 0;
+  char* d_vlayer = nullptr; size_t vlayer_bytes = 0;
   /* local plan: the host-buffer entry point's inputs and outputs, staged in one buffer grown by the first call that
    * needs more */
   char* d_lplan = nullptr; size_t lplan_bytes = 0;
@@ -273,6 +278,8 @@ int32_t tebgpu_sizeof(int32_t which) {
     case 18: return (int32_t)sizeof(TebStaticMaps);
     case 19: return (int32_t)sizeof(TebCostmapWindowArgs);
     case 20: return (int32_t)sizeof(TebObstacleLayerArgs);
+    case 21: return (int32_t)sizeof(TebVoxelLayerArgs);
+    case 22: return (int32_t)sizeof(TebObservationSource);
     default: return -1;
   }
 }
@@ -304,6 +311,7 @@ int64_t tebgpu_get_info(const tebgpu_ctx* ctx, int32_t which) {
     case 19: return ctx->last_fleet_search;
     case 20: return ctx->last_window_grid;
     case 21: return ctx->olayer_max_cap;
+    case 22: return ctx->vlayer_max_cap;
     default: return -1;
   }
 }
@@ -316,7 +324,7 @@ static void free_all(tebgpu_ctx* c) {
                   c->d_ccost, c->d_cgrid, c->d_corigin, c->d_crobot, c->d_ccustom, c->d_ccount, c->d_cobst, c->d_cocount,
                   c->d_cneeded, c->d_lplan, c->d_cycle, c->d_qcost, c->d_cframe, c->d_hsf_part, c->d_hsf_tab,
                   c->d_hs_part, c->d_hs_out, c->d_fclaim, c->d_fleet, c->d_ftable, c->d_fgrid, c->d_fshape, c->d_cwin,
-                  c->d_olayer};
+                  c->d_olayer, c->d_vlayer};
   for (void* p : ptrs)
     if (p) cudaFree(p);
 }
@@ -544,6 +552,11 @@ int32_t tebgpu_create(const TebGpuLimits* lim, int32_t device, tebgpu_ctx** out)
     c->olayer_max_cap = ((long long)optin - (long long)fa.sharedSizeBytes) & ~15LL;
     CUDA_TRY(c, cudaFuncSetAttribute(k_costmap_obstacle_layer, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)c->olayer_max_cap));
+    /* the voxel layer: 164 bytes per 32 cells (column words, layer bytes, visited bits) */
+    CUDA_TRY(c, cudaFuncGetAttributes(&fa, k_costmap_voxel_layer));
+    c->vlayer_max_cap = ((long long)optin - (long long)fa.sharedSizeBytes) / 164 * 32;
+    CUDA_TRY(c, cudaFuncSetAttribute(k_costmap_voxel_layer, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)voxel_layer_smem(c->vlayer_max_cap)));
   }
   CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   return TEBGPU_OK;
@@ -2048,6 +2061,107 @@ int32_t tebgpu_costmap_obstacle_layer(tebgpu_ctx* ctx, const TebObstacleLayerArg
   da.cost = (uint8_t*)(d + o_cost); da.status = (int32_t*)(d + o_status);
   da.flags = a->flags ? (int32_t*)(d + o_flags) : nullptr;
   if ((rc = issue_obstacle_layer(ctx, &da, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->layer, da.layer, cells, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->layer_origin, da.layer_origin, S * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->origin, da.origin, S * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->cost, da.cost, cells, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->status, da.status, S * 4, cudaMemcpyDeviceToHost, st));
+  if (a->flags) CUDA_TRY(ctx, cudaMemcpyAsync(a->flags, da.flags, S * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return TEBGPU_OK;
+}
+
+/* argument checks of both voxel-layer entry points: nothing is launched when one fails */
+static int32_t check_voxel_layer_args(tebgpu_ctx* ctx, const TebVoxelLayerArgs* a) {
+  if (!ctx) return TEBGPU_ERR_INVALID_ARG;
+  if (!a) { ctx->err = "voxel layer args == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->S < 1 || a->cell_cap < 1 || a->P_cap < 0) { ctx->err = "bad voxel layer dimensions"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->S > ctx->lim.max_scenes) { ctx->err = "voxel layer robots exceed the context's max_scenes"; return TEBGPU_ERR_CAPACITY; }
+  if (a->cell_cap > ctx->vlayer_max_cap) { ctx->err = "cell_cap exceeds the shared memory of one CTA (tebgpu_get_info key 22)"; return TEBGPU_ERR_CAPACITY; }
+  if (a->K < 1 || a->K > TEB_VOXEL_LAYER_MAX_SOURCES) { ctx->err = "K outside 1 .. TEB_VOXEL_LAYER_MAX_SOURCES"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!a->sources) { ctx->err = "sources == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  for (int k = 0; k < a->K; ++k)
+    if (!(a->sources[k].obstacle_range >= 0) || !(a->sources[k].raytrace_range >= 0)) { ctx->err = "negative or NaN range"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->F < 0 || a->F > TEB_COSTMAP_FOOTPRINT_MAX) { ctx->err = "F outside 0 .. TEB_COSTMAP_FOOTPRINT_MAX"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->F > 0 && !a->footprint) { ctx->err = "footprint == NULL"; return TEBGPU_ERR_INVALID_ARG; }
+  for (int k = 0; k < 2 * a->F; ++k)
+    if (!std::isfinite(a->footprint[k])) { ctx->err = "non-finite footprint point"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->mode != TEB_VOXEL_LAYER_COMBINE && a->mode != TEB_VOXEL_LAYER_STANDALONE) { ctx->err = "unknown voxel layer mode"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->master_default < 0 || a->master_default > 255) { ctx->err = "master_default outside 0 .. 255"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->z_voxels < 1 || a->z_voxels > 16) { ctx->err = "z_voxels outside 1 .. 16"; return TEBGPU_ERR_INVALID_ARG; }
+  if (a->unknown_threshold < 0 || a->unknown_threshold > 16 || a->mark_threshold < 0 || a->mark_threshold > 16) { ctx->err = "a voxel threshold outside 0 .. 16"; return TEBGPU_ERR_INVALID_ARG; }
+  if (!std::isfinite(a->origin_z) || !(a->z_resolution > 0) || !std::isfinite(a->z_resolution)) { ctx->err = "non-finite origin_z or a z_resolution not positive and finite"; return TEBGPU_ERR_INVALID_ARG; }
+  if ((a->P_cap > 0 && !a->points) || !a->point_count || !a->sensor_origin || !a->robot || !a->grid || !a->voxels ||
+      !a->layer || !a->layer_origin || !a->origin || !a->cost || !a->status) { ctx->err = "missing required voxel layer array"; return TEBGPU_ERR_INVALID_ARG; }
+  if (reinterpret_cast<uintptr_t>(a->voxels) & 3) { ctx->err = "voxels not 4-byte aligned"; return TEBGPU_ERR_INVALID_ARG; }
+  return TEBGPU_OK;
+}
+
+/* k_costmap_voxel_layer on arguments already checked: the sources and the footprint travel in the parameter block */
+static int32_t issue_voxel_layer(tebgpu_ctx* ctx, const TebVoxelLayerArgs* a, cudaStream_t st) {
+  VoxelLayerDev d;
+  std::memset(&d, 0, sizeof(d));
+  d.a = *a;
+  d.a.sources = nullptr;
+  d.a.footprint = nullptr;
+  std::memcpy(d.src, a->sources, (size_t)a->K * sizeof(TebObservationSource));
+  if (a->F) std::memcpy(d.fp, a->footprint, (size_t)a->F * 2 * sizeof(double));
+  k_costmap_voxel_layer<<<a->S, VL_THREADS, (size_t)voxel_layer_smem(a->cell_cap), st>>>(d);
+  ctx->launches = 1;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return TEBGPU_OK;
+}
+
+int32_t tebgpu_costmap_voxel_layer_device(tebgpu_ctx* ctx, const TebVoxelLayerArgs* a, void* cuda_stream) {
+  const int32_t rc = check_voxel_layer_args(ctx, a);
+  if (rc) return rc;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  return issue_voxel_layer(ctx, a, cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+
+int32_t tebgpu_costmap_voxel_layer(tebgpu_ctx* ctx, const TebVoxelLayerArgs* a) {
+  int32_t rc = check_voxel_layer_args(ctx, a);
+  if (rc) return rc;
+  /* the robots the device entry point would mark bad are refused here, before anything runs */
+  for (int s = 0; s < a->S; ++s) {
+    double nox, noy, cx, cy;
+    const int st = voxel_layer_status(*a, s, &nox, &noy, &cx, &cy);
+    if (st == TEB_VOXEL_LAYER_BAD_GRID) { ctx->err = "grid[s] outside 1 .. cell_cap cells, a bad resolution, or a non-finite layer_origin or robot x / y"; return TEBGPU_ERR_INVALID_ARG; }
+    if (st == TEB_VOXEL_LAYER_BAD_POINTS) { ctx->err = "a point_count[s] outside 0 .. P_cap"; return TEBGPU_ERR_INVALID_ARG; }
+    if (st != TEB_VOXEL_LAYER_OK) { ctx->err = "the snapped layer origin differs from origin[s]"; return TEBGPU_ERR_INVALID_ARG; }
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t S = a->S, SK = S * (size_t)a->K, cells = S * (size_t)a->cell_cap,
+               pts = SK * (size_t)a->P_cap * 3 * sizeof(float);
+  /* one staging buffer: every array at a 256-byte aligned offset, so the rows keep their alignment mod 16 */
+  size_t off = 0;
+  auto slot = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_pts = slot(pts), o_count = slot(SK * 4), o_sensor = slot(SK * 3 * sizeof(double)),
+               o_robot = slot(S * 3 * sizeof(double)), o_grid = slot(S * 2 * 4), o_vox = slot(cells * 4),
+               o_layer = slot(cells), o_lorg = slot(S * 2 * sizeof(double)), o_origin = slot(S * 3 * sizeof(double)),
+               o_cost = slot(cells), o_status = slot(S * 4), o_flags = slot(S * 4);
+  if ((rc = grow_mirror(ctx, (void**)&ctx->d_vlayer, &ctx->vlayer_bytes, off, st))) return rc;
+  char* d = ctx->d_vlayer;
+  auto up = [&](size_t o, const void* src, size_t bytes) -> int32_t {
+    if (src && bytes) CUDA_TRY(ctx, cudaMemcpyAsync(d + o, src, bytes, cudaMemcpyHostToDevice, st));
+    return TEBGPU_OK;
+  };
+  if ((rc = up(o_pts, a->points, pts)) || (rc = up(o_count, a->point_count, SK * 4)) ||
+      (rc = up(o_sensor, a->sensor_origin, SK * 3 * sizeof(double))) || (rc = up(o_robot, a->robot, S * 3 * sizeof(double))) ||
+      (rc = up(o_grid, a->grid, S * 2 * 4)) || (rc = up(o_vox, a->voxels, cells * 4)) || (rc = up(o_layer, a->layer, cells)) ||
+      (rc = up(o_lorg, a->layer_origin, S * 2 * sizeof(double))) || (rc = up(o_origin, a->origin, S * 3 * sizeof(double))) ||
+      (rc = up(o_cost, a->cost, cells)))
+    return rc;
+  TebVoxelLayerArgs da = *a;
+  da.points = pts ? (const float*)(d + o_pts) : nullptr;
+  da.point_count = (const int32_t*)(d + o_count); da.sensor_origin = (const double*)(d + o_sensor);
+  da.robot = (const double*)(d + o_robot); da.grid = (const int32_t*)(d + o_grid);
+  da.voxels = (uint32_t*)(d + o_vox); da.layer = (uint8_t*)(d + o_layer); da.layer_origin = (double*)(d + o_lorg);
+  da.origin = (double*)(d + o_origin); da.cost = (uint8_t*)(d + o_cost); da.status = (int32_t*)(d + o_status);
+  da.flags = a->flags ? (int32_t*)(d + o_flags) : nullptr;
+  if ((rc = issue_voxel_layer(ctx, &da, st))) return rc;
+  CUDA_TRY(ctx, cudaMemcpyAsync(a->voxels, da.voxels, cells * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(a->layer, da.layer, cells, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(a->layer_origin, da.layer_origin, S * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(ctx, cudaMemcpyAsync(a->origin, da.origin, S * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));

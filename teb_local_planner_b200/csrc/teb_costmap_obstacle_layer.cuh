@@ -164,6 +164,49 @@ __device__ __forceinline__ void ol_load_row(const uint8_t* row, int cap, Fn f) {
   }
 }
 
+/* updateWithOverwrite (0) / updateWithMax (1) of one cell, master m and layer l; anything else leaves the master */
+__device__ __forceinline__ uint8_t ol_combine(int method, uint8_t m, uint8_t l) {
+  if (l == TEB_COSTMAP_NO_INFORMATION || (method != 0 && method != 1)) return m;
+  if (method == 0) return l;
+  return (m == TEB_COSTMAP_NO_INFORMATION || m < l) ? l : m;
+}
+
+/* footprint clearing by the calling warp (lanes 0 .. 31): the footprint fp[F] placed at rb (x, y, yaw), its vertices'
+ * cells into vx / vy, then one column span per lane of row set to FREE_SPACE; when a placed vertex is off the map
+ * nothing is cleared and lane 0 ors off_bit into *flags */
+__device__ __forceinline__ void ol_clear_footprint(const double (*fp)[2], int F, const double* rb, double ox, double oy,
+                                                   double r, int sx, int sy, int* vx, int* vy, uint8_t* row, int* flags,
+                                                   int off_bit) {
+  const int lane = threadIdx.x;
+  const double c = cos(rb[2]), sn = sin(rb[2]);
+  bool off = false;
+  for (int k = lane; k < F; k += 32) {
+    const double px = fp[k][0], py = fp[k][1];
+    const double wx = teb_add(rb[0], teb_add(teb_mul(px, c), -teb_mul(py, sn)));
+    const double wy = teb_add(rb[1], teb_add(teb_mul(px, sn), teb_mul(py, c)));
+    off |= !ol_world_to_map(wx, wy, ox, oy, r, sx, sy, &vx[k], &vy[k]);
+  }
+  off = __any_sync(0xffffffffu, off);
+  __syncwarp();
+  if (off) {
+    if (lane == 0) *flags |= off_bit;
+  } else {
+    int xmin = INT_MAX, xmax = INT_MIN;
+    for (int k = 0; k < F; ++k) {
+      xmin = min(xmin, vx[k]);
+      xmax = max(xmax, vx[k]);
+    }
+    for (int x = xmin + lane; x <= xmax; x += 32) {
+      int lo = INT_MAX, hi = INT_MIN;
+      for (int k = 0; k < F; ++k) {
+        const int k1 = k + 1 < F ? k + 1 : 0;
+        ol_edge_span(vx[k], vy[k], vx[k1], vy[k1], x, lo, hi);
+      }
+      for (int y = lo; y <= hi; ++y) row[y * sx + x] = 0;
+    }
+  }
+}
+
 __global__ void __launch_bounds__(OL_THREADS) k_costmap_obstacle_layer(const __grid_constant__ ObstacleLayerDev d) {
   extern __shared__ __align__(16) uint8_t srow[];
   __shared__ int s_st, s_cx, s_cy, s_flags;
@@ -281,37 +324,10 @@ __global__ void __launch_bounds__(OL_THREADS) k_costmap_obstacle_layer(const __g
   }
   __syncthreads();
 
-  /* 5. footprint clearing by warp 0: the placed vertices' cells, then one column per lane */
-  if (a.F >= 3 && tid < 32) {
-    const double* rb = a.robot + 3 * (size_t)s;
-    const double c = cos(rb[2]), sn = sin(rb[2]);
-    bool off = false;
-    for (int k = tid; k < a.F; k += 32) {
-      const double px = d.fp[k][0], py = d.fp[k][1];
-      const double wx = teb_add(rb[0], teb_add(teb_mul(px, c), -teb_mul(py, sn)));
-      const double wy = teb_add(rb[1], teb_add(teb_mul(px, sn), teb_mul(py, c)));
-      off |= !ol_world_to_map(wx, wy, ox, oy, r, sx, sy, &s_vx[k], &s_vy[k]);
-    }
-    off = __any_sync(0xffffffffu, off);
-    __syncwarp();
-    if (off) {
-      if (tid == 0) s_flags |= TEB_OBSTACLE_LAYER_FOOTPRINT_OFF_MAP;
-    } else {
-      int xmin = INT_MAX, xmax = INT_MIN;
-      for (int k = 0; k < a.F; ++k) {
-        xmin = min(xmin, s_vx[k]);
-        xmax = max(xmax, s_vx[k]);
-      }
-      for (int x = xmin + tid; x <= xmax; x += 32) {
-        int lo = INT_MAX, hi = INT_MIN;
-        for (int k = 0; k < a.F; ++k) {
-          const int k1 = k + 1 < a.F ? k + 1 : 0;
-          ol_edge_span(s_vx[k], s_vy[k], s_vx[k1], s_vy[k1], x, lo, hi);
-        }
-        for (int y = lo; y <= hi; ++y) srow[y * sx + x] = 0;
-      }
-    }
-  }
+  /* 5. footprint clearing by warp 0 */
+  if (a.F >= 3 && tid < 32)
+    ol_clear_footprint(d.fp, a.F, a.robot + 3 * (size_t)s, ox, oy, r, sx, sy, s_vx, s_vy, srow, &s_flags,
+                       TEB_OBSTACLE_LAYER_FOOTPRINT_OFF_MAP);
   __syncthreads();
 
   /* 6. the layer row in place, then the master row combined over the window */
@@ -320,10 +336,7 @@ __global__ void __launch_bounds__(OL_THREADS) k_costmap_obstacle_layer(const __g
   auto combine = [&](int c, uint8_t m) -> uint8_t {
     if (standalone) m = mdef;
     if (c >= ncell) return m;
-    const uint8_t l = srow[c];
-    if (l == TEB_COSTMAP_NO_INFORMATION || (method != 0 && method != 1)) return m;
-    if (method == 0) return l;
-    return (m == TEB_COSTMAP_NO_INFORMATION || m < l) ? l : m;
+    return ol_combine(method, m, srow[c]);
   };
   if (standalone) ol_store_row<false>(mrow, cap, combine);
   else ol_store_row<true>(mrow, cap, combine);
